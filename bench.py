@@ -1,18 +1,19 @@
 #!/usr/bin/env python
 """Benchmark of the MLD sampling path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
                     [--config headline|1prompt|action512|novae1024] [--scaling weak|strong]
 
-Default (`--config headline`, the driver's line): motions/sec @ 50-step DDIM text-to-motion, batch 256
+Default (`--config headline`): motions/sec @ 50-step DDIM text-to-motion, batch 256
 (BASELINE.json configs[2]: 77-token CLIP context, latent 1x256, decode to 196x263, joints).  One "step" = one
 full pass of the hot path over one batch of synthetic input: 50 x (denoiser on 2B sequences + CFG + DDIM
 update) + VAE decode + feats2joints (+ the all-gather of finished motions when N > 1, through the C ABI:
 mldb_sample_gather).  Rank 0 prints ONE JSON line.  The other BASELINE configs (`--config`) print the same line
 for their own workload; `--scaling strong` shards a fixed total batch instead of B per GPU.
 ``--impl reference`` times the CPU restatement of the reference path (the oracle, pinned against the
-reference's own modules; the reference itself is Python and does not exist on the GPU box) on a bounded sample
-of the same workload.
+reference's own modules) on a bounded sample of the same workload.
+``--dump-outputs DIR`` writes what the last timed step returned (the arrays a caller of the path receives) as
+``DIR/<name>.npy`` in float32; inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -63,11 +64,28 @@ def _cpu_threads() -> int:
 
 
 def _peaks():
-    try:
-        with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
-            return json.load(f), "measured"
-    except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    """NVIDIA's data-sheet figures for the H100 SXM at 700 W (dense fp16/bf16, HBM3); not measured here."""
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "H100 SXM data sheet"
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(torch, out_dir, result):
+    """Write the arrays of one step's result as <name>.npy (float32).  At most DUMP_LIMIT_BYTES in all: a larger
+    array is replaced by a fixed, seeded sample of its elements (same indices in every run)."""
+    import numpy as np
+    arrays = result if isinstance(result, dict) else {"output": result}
+    arrays = {k: v.detach().float().cpu().contiguous() for k, v in arrays.items() if torch.is_tensor(v)}
+    budget = DUMP_LIMIT_BYTES // max(len(arrays), 1) // 4          # elements per array
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.numpy()
+        if a.size > budget:
+            idx = np.random.default_rng(20240607).choice(a.size, size=budget, replace=False)
+            idx.sort()
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a.astype(np.float32, copy=False))
 
 
 class ClockSampler:
@@ -231,8 +249,7 @@ def run_reference(args):
 
 # ------------------------------------------------------------------------------------ eager-PyTorch-on-GPU baseline
 def gpu_eager_baseline(torch, name, dev, eng_joints, cond_d, noise_d, lengths, B):
-    """The reference path restated in eager PyTorch (the oracle port; /root/reference does not exist on this
-    box) on the SAME B200: fp32 with TF32 off and on, CUDA-event timed, with the joint error of the TF32 run and
+    """The reference path restated in eager PyTorch (the oracle port) on the SAME GPU: fp32 with TF32 off and on, CUDA-event timed, with the joint error of the TF32 run and
     of this library against the fp32 eager result."""
     from oracle import mld_oracle as O
     w, _, oracle_run, _, sds, (mean, std) = build_case(name)
@@ -286,6 +303,8 @@ def main():
     ap.add_argument("--scaling", default="weak", choices=["weak", "strong"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-eager-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the arrays the last timed step returned as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -375,6 +394,8 @@ def main():
     elif not latent_model:
         e2e_out = torch.empty((T, B, 263), dtype=torch.float32).pin_memory()
 
+    last_out = [None]                                    # what the most recent timed step returned
+
     def timed(fn, K, W):
         for _ in range(W):
             fn()
@@ -387,7 +408,7 @@ def main():
         e0.record()
         for a, b in evs:
             a.record()
-            fn()
+            last_out[0] = fn()
             b.record()
         if world > 1 and latent_model:
             eng.gather_wait()                            # the last batch's gather is inside the timed region
@@ -406,6 +427,11 @@ def main():
     total_ms, per, launches = timed(step_device, args.steps, args.warmup)
     clk = clocks.stop() if rank == 0 else None
     _log(f"device-resident: {total_ms / args.steps:.1f} ms/step")
+    if args.dump_outputs and rank == 0:
+        res = last_out[0]
+        if world > 1 and latent_model and name != "action512":
+            res = {"joints": gathered[flip[0]]}          # the gathered motions of the last batch
+        dump_outputs(torch, args.dump_outputs, res)
     e2e_ms, _, _ = timed(step_e2e, args.steps, 1)
     _log(f"e2e: {e2e_ms / args.steps:.1f} ms/step")
 
@@ -428,44 +454,36 @@ def main():
         Bp = M // (2 * (2 + S))
         ops = {"qkv": 2.0 * M * 256 * 768, "ffn": 2.0 * M * 256 * 1024 * 2,
                "outproj_ln": 2.0 * M * 256 * 256, "attn": 4.0 * M * (1 + 1 + S) * 256}
-        kname = {"qkv": "k_gemm_tc<256,2,EPI_FAST> (QKV projection, N=768, K=256)",
-                 "ffn": "k_ffn_tc<2> (fused FFN: N=1024 up + GELU, N=256 down + residual + LayerNorm)",
-                 "outproj_ln": "k_gemm_tc<256,2,EPI_LN> (attention out-projection + residual + LayerNorm)",
-                 "attn": "k_attn_tc<64> (tcgen05 attention)"}
+        kname = {"qkv": "k_gemm_tc<256,EPI_FAST> (QKV projection, N=768, K=256)",
+                 "ffn": "k_ffn_tc (fused FFN: N=1024 up + GELU, N=256 down + residual + LayerNorm)",
+                 "outproj_ln": "k_gemm_tc<256,EPI_LN> (attention out-projection + residual + LayerNorm)",
+                 "attn": "k_attn_tc<64> (wgmma attention)"}
         times = {}
         for k in ops:
             times[k] = eng.profile_op(k, Bp, S, 10)
             _log(f"op {k}: {times[k]:.3f} ms")
         layer_ms = eng.profile_op("layer", Bp, S, 5)
         dom = max(times, key=times.get)
-        peak = peaks.get("bf16_tflops", 1590.0)
+        peak = peaks["bf16_tflops"]
         achieved = ops[dom] / (times[dom] * 1e-3) / 1e12
-        traffic, traffic_src = None, None
-        for fn in ("r02_traffic.json", "r01_traffic.json"):
-            try:
-                with open(os.path.join(ROOT, "profiles", fn)) as f:
-                    traffic = json.load(f).get(dom)
-                traffic_src = f"static: ncu --set full capture of this kernel, profiles/{fn} (not re-measured in this run)"
-                break
-            except Exception:
-                continue
+        traffic, traffic_src = None, "not measured"
         roof = {"bound": "tensor", "kernel": f"{kname[dom]}, M={M}",
                 "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak, "traffic": traffic,
                 "traffic_source": traffic_src,
-                "peak_source": peak_src + " bf16 burst (MEASURED_PEAKS.json)" if peak_src == "measured" else peak_src,
+                "peak_source": peak_src,
                 "note": "achieved = algorithmic 2*M*N*K per launch / CUDA-event time; the split-fp16 scheme issues 3 "
                         "tensor-core passes per algorithmic FLOP (tensor-pipe rate = 3x achieved)",
                 "tensor_pass_tflops": 3 * achieved,
-                "tensor_pass_frac_of_sustained": 3 * achieved / peaks.get("bf16_tflops_sustained", 1400.0),
+                "tensor_pass_frac_of_sustained": 3 * achieved / peaks["bf16_tflops_sustained"],
                 "op_ms": {k: round(v, 4) for k, v in times.items()}, "layer_ms": round(layer_ms, 4),
                 "op_tflops": {k: round(ops[k] / (times[k] * 1e-3) / 1e12, 1) for k in ops},
                 "path_tflops": w["flop_per_motion"] * value / 1e12,
-                "path_frac_of_sustained": w["flop_per_motion"] * value / 1e12 / peaks.get("bf16_tflops_sustained", 1400.0)}
+                "path_frac_of_sustained": w["flop_per_motion"] * value / 1e12 / peaks["bf16_tflops_sustained"]}
     elif rank == 0:
         roof = {"bound": "tensor" if name != "1prompt" else "hbm", "kernel": "whole path", "achieved": w["flop_per_motion"] * value / 1e12,
-                "peak": peaks.get("bf16_tflops_sustained", 1400.0), "unit": "TFLOP/s",
-                "frac": w["flop_per_motion"] * value / 1e12 / peaks.get("bf16_tflops_sustained", 1400.0), "traffic": None,
-                "note": "whole-path algorithmic FLOP rate against the sustained bf16 peak (per-kernel rooflines: headline config)"}
+                "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
+                "frac": w["flop_per_motion"] * value / 1e12 / peaks["bf16_tflops_sustained"], "traffic": None,
+                "note": "whole-path algorithmic FLOP rate against the data-sheet fp16 peak (per-kernel rooflines: headline config)"}
 
     eager = None
     if rank == 0 and world == 1 and name in ("headline", "1prompt") and not args.no_eager_baseline:
@@ -501,7 +519,7 @@ def main():
             "scaling": "strong" if strong else "weak", "vs_baseline": None,
             "dtype": "f16x2-split (fp32-equivalent, fp32 accumulate)", "data": "synthetic",
             "config": {"workload": w["workload"], "global_batch": world * B, "parallelism": f"batch-sharded dp{world}",
-                       "l2": "working set (activations > 700 MB at B=256) exceeds the 126 MB L2; no flush needed" if name == "headline"
+                       "l2": "working set (activations > 700 MB at B=256) exceeds the 50 MB L2; no flush needed" if name == "headline"
                              else "inputs + weights smaller than L2: steady-state (warm L2) numbers, as in the real loop",
                        "weights": "random-init (seeded), reference architecture"},
             "e2e": {"value": e2e_value, "unit": "motions/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},

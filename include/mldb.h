@@ -18,7 +18,7 @@
  *  - all work is enqueued on the `stream` argument (a cudaStream_t passed as void*), calls
  *    are asynchronous with respect to the host unless stated otherwise.
  *  - a handle is bound to one device and is not thread-safe (one handle per GPU/stream).
- *  - there is NO CPU fallback: a device that is not sm_100 makes mldb_create fail.
+ *  - there is NO CPU fallback: a device that is not sm_90 makes mldb_create fail.
  */
 #ifndef MLDB_H_
 #define MLDB_H_
@@ -97,7 +97,7 @@ typedef struct mldb_config {
 void mldb_default_config(mldb_config* cfg);
 
 /* Replaces: instantiate_from_config(cfg.model.{denoiser,motion_vae,scheduler})
- * (mld/models/modeltype/mld.py:56-83).  Fails unless `device` is an sm_100 GPU. */
+ * (mld/models/modeltype/mld.py:56-83).  Fails unless `device` is an sm_90 GPU. */
 int mldb_create(const mldb_config* cfg, int device, mldb_handle** out);
 void mldb_destroy(mldb_handle* h);
 
@@ -223,14 +223,14 @@ int mldb_profile_op(mldb_handle* h, const char* op, int32_t B, int32_t S_ctx, in
 int mldb_profile_steps(mldb_handle* h, const void* cond, const float* init_noise, int32_t B, int32_t S_ctx,
                        float* ms_out);
 
-/* Debug aid: in-kernel timeline of the tcgen05 kernels (GEMM / FFN / attention).  enable != 0 starts recording:
+/* Debug aid: in-kernel timeline of the wgmma kernels (GEMM / FFN / attention).  enable != 0 starts recording:
  * every warp role of CTA 0 appends {tag | warp << 16 | aux << 24, SM clock} at its pipeline events (tags in the
  * kernels' tl_event calls).  enable == 0 copies the events into out (HOST int64[2 * cap]), sets *count and stops.
  * Process-wide; recording costs one atomic per event in CTA 0 only. */
 int mldb_debug_timeline(int32_t enable, int64_t* out, int32_t cap, int32_t* count);
 
 /* Debug aid for the kernel unit tests: y = act(A W^T + b), or LayerNorm(A W^T + b + R) when gamma is
- * given, through the engine's GEMM operators (use_tc: 1 = tcgen05 path, 0 = CUDA-core path).
+ * given, through the engine's GEMM operators (use_tc: 1 = wgmma path, 0 = CUDA-core path).
  * A [M,K], R [M,N], out [M,N]: fp32 DEVICE; W [N,K], bias/gamma/beta [N]: fp32 HOST.  0 < K1 < K feeds
  * A as two concatenated sources (the skip-connection GEMM).  split_out != 0: the plain epilogue writes
  * split16 planes (the production path; N % 8 == 0) which are then widened to fp32.  Synchronous. */
@@ -239,8 +239,8 @@ int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float*
                     int32_t act, int32_t use_tc, int32_t split_out, float* out, void* stream);
 
 /* Debug aid: one post-norm FFN block y = LayerNorm(x + W2 gelu(W1 x + b1) + b2) through the engine's
- * operators (cross_attention.py:266-271).  mode 0 = CUDA-core kernels, 1 = tcgen05 GEMMs as two
- * launches, 2 = the fused tcgen05 FFN kernel.  X, out [M,d]: fp32 DEVICE; W1 [ff,d], W2 [d,ff],
+ * operators (cross_attention.py:266-271).  mode 0 = CUDA-core kernels, 1 = wgmma GEMMs as two
+ * launches, 2 = the fused wgmma FFN kernel.  X, out [M,d]: fp32 DEVICE; W1 [ff,d], W2 [d,ff],
  * b1 [ff], b2/gamma/beta [d]: fp32 HOST.  Synchronous. */
 int mldb_debug_ffn(mldb_handle* h, const float* X, const float* W1, const float* b1, const float* W2,
                    const float* b2, const float* gamma, const float* beta, int32_t M, int32_t d, int32_t ff,
@@ -251,7 +251,7 @@ int mldb_debug_ffn(mldb_handle* h, const float* X, const float* W1, const float*
  *               in_proj order; self-attention, Lk == Lq) - the layout the denoiser / VAE stacks use;
  *   KV != NULL: Q [nseq*Lq, heads*hd] and KV [nseq*Lk, 2*heads*hd] (k | v) - cross-attention.
  * lengths (device int32 [nseq], nullable): valid keys per sequence = min(Lk, kv_prefix + lengths[s]).
- * mode 0 = CUDA-core kernel, 1 = mma.sync kernel, 2 = tcgen05 kernel (product path).
+ * mode 0 = CUDA-core kernel, 1 = mma.sync kernel, 2 = wgmma kernel (product path).
  * out [nseq*Lq, heads*hd] fp32 DEVICE.  Synchronous. */
 int mldb_debug_attention(mldb_handle* h, const float* Q, const float* KV, const int32_t* lengths, int32_t kv_prefix,
                          int32_t nseq, int32_t Lq, int32_t Lk, int32_t heads, int32_t hd, int32_t mode, float* out,
@@ -264,11 +264,11 @@ int mldb_abi_version(void);
 int64_t mldb_launch_count(const mldb_handle* h);
 /* Which kernel every operator of the path was ENQUEUED on since the last reset (recorded launches: a CUDA
  * graph counts once, at capture).  out: HOST int64[MLDB_KSTAT_COUNT], index = MLDB_KSTAT_*.  Lets a caller
- * (and the tests) assert that nothing fell back from the tcgen05 kernels to the CUDA-core kernels. */
+ * (and the tests) assert that nothing fell back from the wgmma kernels to the CUDA-core kernels. */
 #define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue */
 #define MLDB_KSTAT_GEMM_LN_TC 1   /* k_gemm_tc, fused residual + LayerNorm epilogue */
 #define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block) */
-#define MLDB_KSTAT_ATTN_TC 3      /* k_attn_tc (tcgen05 attention) */
+#define MLDB_KSTAT_ATTN_TC 3      /* k_attn_tc (wgmma attention) */
 #define MLDB_KSTAT_ATTN_MMA 4     /* k_attn_mma (mma.sync attention; option attn=mma) */
 #define MLDB_KSTAT_ATTN_SIMT 5    /* k_attn_simt (CUDA cores) */
 #define MLDB_KSTAT_GEMM_SIMT 6    /* k_gemm_simt (CUDA cores: odd-K embeddings, time MLP, gemm=simt) */
@@ -281,8 +281,8 @@ int mldb_reset_kernel_stats(mldb_handle* h);
 
 /* Set an engine option by name.  Options only change HOW the same arithmetic is scheduled; results are
  * identical (gemm, attn: to fp32 re-association noise) for every setting (tests/test_gpu_kernels.py).
- *   "gemm"       "tc" | "simt"          tcgen05 kernels (default) or the CUDA-core reference kernels  MLDB_GEMM
- *   "attn"       "tc" | "mma" | "simt"  attention core: tcgen05 (default), mma.sync, CUDA cores       MLDB_ATTN
+ *   "gemm"       "tc" | "simt"          wgmma kernels (default) or the CUDA-core reference kernels  MLDB_GEMM
+ *   "attn"       "tc" | "mma" | "simt"  attention core: wgmma (default), mma.sync, CUDA cores       MLDB_ATTN
  *   "ffn_fused"  0 | 1                  fused FFN kernel k_ffn_tc (default 1)                         MLDB_FFN_FUSED
  *   "ffn_split"  0 | 1                  fused FFN: cut the tile groups that do not fill a whole round of the
  *                                        persistent grid along the hidden dimension (default 1; env MLDB_FFN_SPLIT).

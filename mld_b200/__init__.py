@@ -1,4 +1,4 @@
-"""mld_b200: B200-native (sm_100a) latent-diffusion sampling path for Motion Latent Diffusion.
+"""mld_b200: H100-native (sm_90a) latent-diffusion sampling path for Motion Latent Diffusion.
 
 The math lives in ``libmldb200.so`` (hand-written CUDA, C ABI in ``include/mldb.h``); this
 package is the torch-side mirror of the reference's interfaces for that path:

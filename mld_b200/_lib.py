@@ -1,6 +1,6 @@
 """ctypes binding of ``libmldb200.so`` (C ABI in ``include/mldb.h``).
 
-The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_100a).  There is no
+The library is built in-tree by ``__graft_entry__.build()`` (nvcc, sm_90a).  There is no
 Python/CPU fallback: a missing library is an ImportError with the build command, and every
 non-zero status from the C side becomes a ``RuntimeError`` carrying ``mldb_last_error()``.
 """
@@ -93,7 +93,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; "
-                "g.build()'` (nvcc, sm_100a). mld_b200 has no CPU or PyTorch fallback.")
+                "g.build()'` (nvcc, sm_90a). mld_b200 has no CPU or PyTorch fallback.")
         l = C.CDLL(LIB_PATH)
         for name, (res, args) in _SIGNATURES.items():
             fn = getattr(l, name)      # AttributeError if the ABI lost a symbol

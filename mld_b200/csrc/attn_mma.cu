@@ -5,7 +5,7 @@
 // with the same three-product scheme as the GEMMs:
 //     S = Qh Kh^T + Ql Kh^T + Qh Kl^T,      O = Ph Vh + Pl Vh + Ph Vl
 // (P = exp(S - max) is re-split into hi/lo fp16 in registers).  The sequences here are far too
-// short for a tcgen05 tile per head (a 128-row MMA would be >35 % padding at L = 79 and the PV
+// short for a wgmma tile per head (a 128-row MMA would be >35 % padding at L = 79 and the PV
 // operand would need an MN-major descriptor per 64-wide head slice); legacy mma.sync tiles of
 // 16 x 8 fit them exactly and attention is ~5 % of the path's FLOPs.
 // Replaces the attention core of nn.MultiheadAttention (cross_attention.py:264-266, 330-338):

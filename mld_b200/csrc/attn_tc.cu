@@ -1,63 +1,44 @@
-// Multi-head attention core on tcgen05 / TMEM / TMA for the split16 activation format.
+// Multi-head attention core on wgmma / TMA for the split16 activation format.
 // Replaces the attention core of nn.MultiheadAttention (cross_attention.py:264-266, 330-338):
 // scores scaled by 1/sqrt(head_dim), padded keys masked (-inf), softmax over keys, P @ V - for
-// every shape the sampling path uses: Lq, Lk in 1..256 (denoiser 79 / 3 tokens, VAE 196 / 198
+// every shape the sampling path uses: Lq in 1.., Lk in 1..256 (denoiser 79 / 3 tokens, VAE 196 / 198
 // frames, 1-2 memory tokens), head_dim 64 or 128.
 //
-// Work item = (sequence, head, 128-row query tile); persistent CTAs (one per SM) walk the items.
-// Keys are processed in blocks of 64 (the last block padded to a multiple of 16):
-//   S[:, kb]  = Q K_kb^T            M = 128, N = 64 | rem, K = head_dim  (A, B K-major)
-//   P[:, kb]  = exp2(scale*(S - max))  two exact passes over the WHOLE score row, which lives in
-//                                   TMEM (<= 256 columns) - no online rescaling
-//   O        += P[:, kb] V_kb       M = 128, N = 64 per 64-wide slice of the head, K = 64 | rem
-//                                   (A = P from shared memory, K-major; B = V_kb exactly as TMA
-//                                   delivers the [keys x d] box: an MN-major operand, no transpose)
-// every product in the 3-term split-fp16 form (hi.hi + lo.hi + hi.lo, fp32 accumulation in TMEM).
-//
-// Warp roles (18 warps):
-//   warps 0-7 / 8-15  two softmax groups; group g owns items j = g (mod 2).  One query row per TMEM lane,
-//                    TWO warps per lane quarter that split the key columns (16-key chunks alternate between
-//                    them): pass 1 partial max -> exchanged through shared memory, pass 2 exp2 + partial row
-//                    sum + P re-split to hi / lo fp16 written to shared memory in the UMMA K-major
-//                    SWIZZLE_128B layout, sums exchanged, then each warp normalises and stores half of the
-//                    O row.  (Measured on the first version, one warp per row: the softmax warps were bound
-//                    by exposed instruction latency - one active warp per SM sub-partition, ~7 cycles per
-//                    instruction - not by TMEM or MUFU throughput; twice the warps halve an item's latency.)
-//   warp 16          TMA producer: Q tile (own double buffer), then K blocks and V blocks through
-//                    one ring of 64-key slots, in exactly the order the MMA warp consumes them
-//   warp 17 / 18     the two MMA issuers: warp 17 (also the TMEM allocator) issues the S = Q K^T chains, warp 18
-//                    the O = P V chains.  They work on different accumulators, so nothing orders them but
-//                    the data (with two score buffers S(j+1) runs while a softmax group is busy with item
-//                    j).  One issuer for both was the kernel's pacer: the in-kernel timeline showed ~6.7k
-//                    cycles per item on that warp alone (39 MMAs x ~50 cycles of issue + ~9 barrier waits x
-//                    ~450 cycles), with the softmax warps idle 75 % of the time.
-// TMEM: S buffers (nkb*64 columns each) then two O buffers (head_dim columns each), <= 512 columns.
+// Work item = (sequence, head, 64-row query tile) = one warpgroup's MMA height.  A CTA (one per SM,
+// persistent) runs TWO independent pipelines, each a consumer warpgroup with its own Q buffer and
+// K / V ring and its own TMA warp in the producer warpgroup; while one warpgroup is in its softmax the
+// other one's MMAs keep the tensor cores busy.  Keys are processed in blocks of 64 (the last block
+// padded to a multiple of 16):
+//   S[:, kb]  = Q K_kb^T            M = 64, N = 64, K = head_dim            (A, B K-major in shared memory)
+//   P         = exp2(scale*(S - max))  two exact passes over the WHOLE score row, which lives in
+//                                   registers (<= 256 columns) - no online rescaling
+//   O        += P[:, kb] V_kb       M = 64, N = 64 per 64-wide slice of the head, K = 64 | rem
+//                                   (A = P from registers: the accumulator layout of 16 score columns IS
+//                                   the register-operand layout of a 16-deep k-step; B = V_kb exactly as
+//                                   TMA delivers the [keys x d] box: an MN-major operand, no transpose)
+// every product in the 3-term split-fp16 form (hi.hi + lo.hi + hi.lo, fp32 accumulation).
 #include <stdio.h>
 #include <stdlib.h>
+#include <string.h>
 
 #include "ops.cuh"
-#include <stdlib.h>
-#include <string.h>
 #include "tc_common.cuh"
 
 namespace {
 using namespace tc;
 
-constexpr int ATC_THREADS = 608;
-constexpr int WARP_TMA = 16, WARP_MMA = 17, WARP_MMA2 = 18;   // S issuer (+ TMEM allocator), PV issuer
-constexpr int RED_BYTES = 2 * 2 * 2 * 128 * 4;   // [group][max | sum][column half][row] exchange buffers
+constexpr int ATC_THREADS = 384;          // producer warpgroup (warps 0 / 1 feed pipelines 0 / 1) + two consumer warpgroups
 constexpr int KBLK = 64;                  // keys per block
-constexpr int P_BYTES = 2 * 16384;        // one P block: [128 rows x 64 keys] hi plane + lo plane
-constexpr int MAX_RS = 8;                 // ring slots (K / V blocks)
-constexpr int SMEM_LIMIT = 227 * 1024;
+constexpr int QROWS = 64;                 // query rows per item
+constexpr int MAX_KB = 4;                 // key blocks of the longest score row (256 keys)
+constexpr int PIPE_BYTES = 96 * 1024;     // shared memory of one pipeline: Q tile + K / V ring
+constexpr int MAX_RS = 5;                 // ring slots (head_dim 64: 5 x 16 KB, head_dim 128: 2 x 32 KB)
+constexpr int SMEM_BYTES = 2 * PIPE_BYTES + 256 + 1024;   // + barriers + alignment slack
 
 struct AtcParams {
   int nseq, heads, Lq, Lk;
-  int n_qt;                // 128-row query tiles per (sequence, head)
+  int n_qt;                // 64-row query tiles per (sequence, head)
   int nkb, rem;            // key blocks; keys (multiple of 16) in the last block
-  int QR;                  // rows of the Q box (multiple of 8, <= 128)
-  int QB, SB, RS;          // Q buffers, score buffers, ring slots
-  int NOB;                 // O accumulators in TMEM: 2, or 4 when 4 * HD columns fit next to the score buffers
   int q_col0, k_col0, v_col0;
   const int32_t* lengths; int kv_prefix, len_mod, seq0;
   __half* out_hi; __half* out_lo; int ld_out;
@@ -71,14 +52,22 @@ struct Item { int s, h, qt; };
 __device__ __forceinline__ Item decode_item(int item, const AtcParams& p) {
   Item it;
   if (p.reverse) item = p.items - 1 - item;
-  // runtime integer divisions showed up with ~10 % of this kernel's stall samples: one query tile and a
-  // power-of-two head count (every shipped config) need none
+  // one query tile and a power-of-two head count (every shipped config) need no runtime division
   int sh = item;
   it.qt = 0;
   if (p.n_qt > 1) { sh = item / p.n_qt; it.qt = item - sh * p.n_qt; }
   if (p.heads_log2 >= 0) { it.s = sh >> p.heads_log2; it.h = sh & (p.heads - 1); }
   else { it.s = sh / p.heads; it.h = sh - it.s * p.heads; }
   return it;
+}
+
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
 template <int HD>
@@ -88,366 +77,249 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
           const __grid_constant__ CUtensorMap tmRh, const __grid_constant__ CUtensorMap tmRl,    // rem-row boxes
           const AtcParams p) {
   constexpr int NS = HD / 64;                         // 64-wide slices of the head dimension
-  constexpr int SLOT_BYTES = 2 * NS * KBLK * 128;     // [plane][slice][64 keys x 128 B]
-  constexpr int SL_PLANE = NS * KBLK * 128;           // plane stride inside a slot
+  constexpr int TILE = KBLK * 128;                    // one [64 rows x 64 columns] swizzled tile (8 KB)
+  constexpr int SLOT_BYTES = 2 * NS * TILE;           // [plane][slice] tiles of one key block; the Q tile has the same shape
+  constexpr int SL_PLANE = NS * TILE;                 // plane stride inside a slot
+  constexpr int RS = PIPE_BYTES / SLOT_BYTES - 1;     // ring slots next to the Q tile
+  static_assert(RS >= 2 && RS <= MAX_RS, "ring depth");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  const int q_tile = p.QR * 128;                      // one [QR x 64] tile
-  const int q_bytes = 2 * NS * q_tile;                // [plane][slice] tiles
-  uint8_t* sQ = smem;
-  uint8_t* sR = sQ + p.QB * q_bytes;
-  uint8_t* sP = sR + p.RS * SLOT_BYTES;
-  float* s_red = reinterpret_cast<float*>(sP + 2 * P_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * P_BYTES + RED_BYTES);
-  uint64_t* q_full = bars;                  // [2]
-  uint64_t* q_empty = bars + 2;             // [2]
-  uint64_t* r_full = bars + 4;              // [MAX_RS]
-  uint64_t* r_empty = bars + 4 + MAX_RS;    // [MAX_RS]
-  uint64_t* s_full = bars + 4 + 2 * MAX_RS; // [2]
-  uint64_t* s_empty = s_full + 2;           // [2]
-  uint64_t* p_full = s_full + 4;            // [2]
-  uint64_t* p_empty = s_full + 6;           // [2]
-  uint64_t* o_full = s_full + 8;            // [4]
-  uint64_t* o_empty = s_full + 12;          // [4]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_full + 16);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * PIPE_BYTES);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   int tl_n = 0;                                       // debug-timeline event counter of this warp
   tl_event(p.tl, tl_n, 40);                       // kernel entry
-  const int items = p.nseq * p.heads * p.n_qt;
-  const int nlocal = (items - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  const int nkb = p.nkb, SB = p.SB, QB = p.QB, RS = p.RS, NOB = p.NOB;
-  const int scols = nkb * KBLK;                       // TMEM columns of one score buffer
+  const int nkb = p.nkb;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(smem_u32(&q_full[i]), 1);  mbar_init(smem_u32(&q_empty[i]), 1);
-      mbar_init(smem_u32(&s_full[i]), 1);  mbar_init(smem_u32(&s_empty[i]), 8);
-      mbar_init(smem_u32(&p_full[i]), 8);  mbar_init(smem_u32(&p_empty[i]), 1);
+    for (int g = 0; g < 2; ++g) {
+      uint64_t* b = bars + g * (2 + 2 * MAX_RS);
+      mbar_init(smem_u32(&b[0]), 1);                  // q_full (TMA tx)
+      mbar_init(smem_u32(&b[1]), 4);                  // q_empty (one arrival per warp of the consumer warpgroup)
+      for (int i = 0; i < MAX_RS; ++i) { mbar_init(smem_u32(&b[2 + i]), 1); mbar_init(smem_u32(&b[2 + MAX_RS + i]), 4); }
     }
-    for (int i = 0; i < 4; ++i) { mbar_init(smem_u32(&o_full[i]), 1);  mbar_init(smem_u32(&o_empty[i]), 8); }
-    for (int i = 0; i < MAX_RS; ++i) { mbar_init(smem_u32(&r_full[i]), 1); mbar_init(smem_u32(&r_empty[i]), 1); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmQh); tma_prefetch_desc(&tmQl); tma_prefetch_desc(&tmKh); tma_prefetch_desc(&tmKl);
   }
-  if (warp == WARP_MMA) tmem_alloc<1>(smem_u32(tmem_slot), 512);
   pdl_trigger();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                                         // q|k|v come from the previous kernel
   tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
 
-  if (warp == WARP_TMA) {
-    // ------------------------------------------------------------------ TMA producer
+  const bool producer = warp < 4;
+  const int g = producer ? (warp & 1) : (warp >> 2) - 1;    // pipeline of this warp
+  uint8_t* const sQ = smem + g * PIPE_BYTES;
+  uint8_t* const sR = sQ + SLOT_BYTES;
+  uint64_t* const q_full = bars + g * (2 + 2 * MAX_RS);
+  uint64_t* const q_empty = q_full + 1;
+  uint64_t* const r_full = q_full + 2;
+  uint64_t* const r_empty = r_full + MAX_RS;
+  const int pid = (int)blockIdx.x * 2 + g, npipes = (int)gridDim.x * 2;
+  const int nlocal = (p.items - pid + npipes - 1) / npipes;
+
+  if (producer) {
+    reg_dec<40>();
+    if (warp >= 2) return;
+    // ------------------------------------------------------------------ TMA producer of pipeline g:
+    // Q(j), the K blocks of item j, its V blocks - exactly the order the consumer takes them
     int rc = 0;                                       // ring position (K and V blocks, all items)
-    auto load_qk = [&](int j) {
-      const Item it = decode_item((int)blockIdx.x + j * (int)gridDim.x, p);
-      const int qb = j % QB;
-      mbar_wait(smem_u32(&q_empty[qb]), (((uint32_t)(j / QB)) & 1u) ^ 1u);
-      tl_event(p.tl, tl_n, 20, j);                                     // producer: Q(j) buffer free, loads issued
+    for (int j = 0; j < nlocal; ++j) {
+      const Item it = decode_item(pid + j * npipes, p);
+      mbar_wait(smem_u32(q_empty), ((uint32_t)j & 1u) ^ 1u);
+      tl_event(p.tl, tl_n, 20, j);                                     // producer: Q buffer free, loads issued
       if (elect_one()) {
-        const uint32_t full = smem_u32(&q_full[qb]);
-        mbar_expect_tx(full, (uint32_t)q_bytes);
-        const uint32_t base = smem_u32(sQ + qb * q_bytes);
-        const int r0 = it.s * p.Lq + it.qt * 128;
+        const uint32_t full = smem_u32(q_full);
+        mbar_expect_tx(full, (uint32_t)SLOT_BYTES);
+        const uint32_t base = smem_u32(sQ);
+        const int r0 = it.s * p.Lq + it.qt * QROWS;
 #pragma unroll
         for (int sl = 0; sl < NS; ++sl) {
-          tma_load_2d(base + sl * q_tile, &tmQh, full, p.q_col0 + it.h * HD + sl * 64, r0);
-          tma_load_2d(base + (NS + sl) * q_tile, &tmQl, full, p.q_col0 + it.h * HD + sl * 64, r0);
+          tma_load_2d(base + sl * TILE, &tmQh, full, p.q_col0 + it.h * HD + sl * 64, r0);
+          tma_load_2d(base + SL_PLANE + sl * TILE, &tmQl, full, p.q_col0 + it.h * HD + sl * 64, r0);
         }
       }
       __syncwarp();
-      for (int kb = 0; kb < nkb; ++kb, ++rc) {
-        const int sl_i = rc % RS;
-        mbar_wait(smem_u32(&r_empty[sl_i]), (((uint32_t)(rc / RS)) & 1u) ^ 1u);
-        if (elect_one()) {
-          const bool last = kb == nkb - 1;
-          const int rows = last ? p.rem : KBLK;
-          const uint32_t full = smem_u32(&r_full[sl_i]);
-          mbar_expect_tx(full, (uint32_t)(2 * NS * rows * 128));
-          const uint32_t base = smem_u32(sR + sl_i * SLOT_BYTES);
-          const int r0 = it.s * p.Lk + kb * KBLK;
+      for (int kv = 0; kv < 2; ++kv) {
+        const int col0 = (kv ? p.v_col0 : p.k_col0) + it.h * HD;
+        for (int kb = 0; kb < nkb; ++kb, ++rc) {
+          const int sl_i = rc % RS;
+          mbar_wait(smem_u32(&r_empty[sl_i]), (((uint32_t)(rc / RS)) & 1u) ^ 1u);
+          if (elect_one()) {
+            const bool last = kb == nkb - 1;
+            const int rows = last ? p.rem : KBLK;
+            const uint32_t full = smem_u32(&r_full[sl_i]);
+            mbar_expect_tx(full, (uint32_t)(2 * NS * rows * 128));
+            const uint32_t base = smem_u32(sR + sl_i * SLOT_BYTES);
+            const int r0 = it.s * p.Lk + kb * KBLK;
 #pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            const int c0 = p.k_col0 + it.h * HD + sl * 64;
-            tma_load_2d(base + sl * (KBLK * 128), last ? &tmRh : &tmKh, full, c0, r0);
-            tma_load_2d(base + SL_PLANE + sl * (KBLK * 128), last ? &tmRl : &tmKl, full, c0, r0);
-          }
-        }
-        __syncwarp();
-      }
-    };
-    auto load_v = [&](int j) {
-      const Item it = decode_item((int)blockIdx.x + j * (int)gridDim.x, p);
-      for (int kb = 0; kb < nkb; ++kb, ++rc) {
-        const int sl_i = rc % RS;
-        mbar_wait(smem_u32(&r_empty[sl_i]), (((uint32_t)(rc / RS)) & 1u) ^ 1u);
-        tl_event(p.tl, tl_n, 21, j);                                   // producer: slot free for V(j, kb)
-        if (elect_one()) {
-          const bool last = kb == nkb - 1;
-          const int rows = last ? p.rem : KBLK;
-          const uint32_t full = smem_u32(&r_full[sl_i]);
-          mbar_expect_tx(full, (uint32_t)(2 * NS * rows * 128));
-          const uint32_t base = smem_u32(sR + sl_i * SLOT_BYTES);
-          const int r0 = it.s * p.Lk + kb * KBLK;
-#pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            const int c0 = p.v_col0 + it.h * HD + sl * 64;
-            tma_load_2d(base + sl * (KBLK * 128), last ? &tmRh : &tmKh, full, c0, r0);
-            tma_load_2d(base + SL_PLANE + sl * (KBLK * 128), last ? &tmRl : &tmKl, full, c0, r0);
-          }
-        }
-        __syncwarp();
-      }
-    };
-    if (SB == 2 && nlocal > 0) load_qk(0);
-    for (int j = 0; j < nlocal; ++j) {
-      if (SB == 2) { if (j + 1 < nlocal) load_qk(j + 1); }
-      else load_qk(j);
-      load_v(j);
-    }
-  } else if (warp == WARP_MMA) {
-    // ------------------------------------------------------------------ MMA issuer 1: S(j) = Q K^T, block by block
-    // ring position of K(j, 0): the producer's order is K(0) | K(1) V(0) | K(2) V(1) | ... with two score
-    // buffers, K(0) V(0) | K(1) V(1) | ... with one
-    for (int j = 0; j < nlocal; ++j) {
-      const int qb = j % QB, sb = j % SB, g = j & 1;
-      const int rc0 = SB == 2 ? (j == 0 ? 0 : (2 * j - 1) * nkb) : 2 * j * nkb;
-      mbar_wait(smem_u32(&q_full[qb]), ((uint32_t)(j / QB)) & 1u);
-      // score buffer sb was last read by item j - SB, i.e. by softmax group (j - SB) & 1 as ITS item number
-      // (j - SB) >> 1.  The full / empty barriers are per GROUP (not per buffer): every waiter then sees the
-      // phases of its barrier one by one, whatever SB is (a parity wait must never lag two phases).
-      if (j >= SB) mbar_wait(smem_u32(&s_empty[(j - SB) & 1]), ((uint32_t)(j - SB) >> 1) & 1u);
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 22, j);                               // MMA: Q(j) landed, score buffer free
-      const uint32_t qbase = smem_u32(sQ + qb * q_bytes);
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int rc = rc0 + kb, sl_i = rc % RS;
-        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)(rc / RS)) & 1u);
-        tc_fence_after();
-        tl_event(p.tl, tl_n, 23, j);                             // MMA: K(j, kb) landed, S MMAs issue
-        if (elect_one()) {
-          const int n = kb == nkb - 1 ? p.rem : KBLK;
-          const uint32_t idesc_s = make_idesc(n, 128, false);
-          const uint32_t kbase = smem_u32(sR + sl_i * SLOT_BYTES);
-          const uint32_t tacc = tmem_base + (uint32_t)(sb * scols + kb * KBLK);
-#pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            uint64_t qh = make_desc(qbase + sl * q_tile), ql = make_desc(qbase + (NS + sl) * q_tile);
-            uint64_t kh = make_desc(kbase + sl * (KBLK * 128)), kl = make_desc(kbase + SL_PLANE + sl * (KBLK * 128));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              umma(tacc, ql, kh, idesc_s, (sl | kk) != 0 ? 1u : 0u);
-              umma(tacc, qh, kl, idesc_s, 1u);
-              umma(tacc, qh, kh, idesc_s, 1u);
-              qh += 2; ql += 2; kh += 2; kl += 2;     // next 16 elements of the head dimension: +32 B
+            for (int sl = 0; sl < NS; ++sl) {
+              tma_load_2d(base + sl * TILE, last ? &tmRh : &tmKh, full, col0 + sl * 64, r0);
+              tma_load_2d(base + SL_PLANE + sl * TILE, last ? &tmRl : &tmKl, full, col0 + sl * 64, r0);
             }
           }
-          umma_commit(smem_u32(&r_empty[sl_i]));      // the K block may be overwritten
-          if (kb == nkb - 1) {
-            umma_commit(smem_u32(&s_full[g]));
-            umma_commit(smem_u32(&q_empty[qb]));      // Q only feeds the scores
-          }
+          __syncwarp();
         }
-        __syncwarp();
-      }
-      tl_event(p.tl, tl_n, 24, j);                               // MMA: S(j) issued
-    }
-  } else if (warp == WARP_MMA2) {
-    // ------------------------------------------------------------------ MMA issuer 2: O(j) = P V, block by block
-    const uint32_t idesc_o = make_idesc(64, 128, true);
-    const uint32_t sP_u = smem_u32(sP);
-    for (int j = 0; j < nlocal; ++j) {
-      const int ob = j % NOB;
-      // ring position of V(j, 0): after K(j + 1) with two score buffers - except for the last item, which has none
-      const int rc0 = (SB == 2 && j + 1 < nlocal) ? (2 * j + 2) * nkb : (2 * j + 1) * nkb;
-      mbar_wait(smem_u32(&o_empty[ob]), (((uint32_t)(j / NOB)) & 1u) ^ 1u);
-      tc_fence_after();
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int pseq = j * nkb + kb, pb = pseq & 1;
-        const int rc = rc0 + kb, sl_i = rc % RS;
-        mbar_wait(smem_u32(&p_full[pb]), ((uint32_t)pseq >> 1) & 1u);
-        tl_event(p.tl, tl_n, 25, j);                             // MMA: P(j, kb) written
-        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)(rc / RS)) & 1u);
-        tc_fence_after();
-        tl_event(p.tl, tl_n, 26, j);                             // MMA: V(j, kb) landed, PV MMAs issue
-        if (elect_one()) {
-          const int nks = (kb == nkb - 1 ? p.rem : KBLK) / 16;
-          const uint32_t vbase = smem_u32(sR + sl_i * SLOT_BYTES);
-          const uint32_t pbase = sP_u + pb * P_BYTES;
-#pragma unroll
-          for (int sl = 0; sl < NS; ++sl) {
-            const uint32_t tacc = tmem_base + (uint32_t)(SB * scols + ob * HD + sl * 64);
-            uint64_t ph = make_desc(pbase), pl = make_desc(pbase + 16384);
-            uint64_t vh = make_desc(vbase + sl * (KBLK * 128)), vl = make_desc(vbase + SL_PLANE + sl * (KBLK * 128));
-            for (int ks = 0; ks < nks; ++ks) {
-              umma(tacc, pl, vh, idesc_o, (kb | ks) != 0 ? 1u : 0u);
-              umma(tacc, ph, vl, idesc_o, 1u);
-              umma(tacc, ph, vh, idesc_o, 1u);
-              ph += 2; pl += 2;                       // next 16 keys of the K-major P tile: +32 B
-              vh += 128; vl += 128;                   // next 16 keys of the MN-major V tile: +2048 B
-            }
-          }
-          umma_commit(smem_u32(&r_empty[sl_i]));
-          umma_commit(smem_u32(&p_empty[pb]));
-          if (kb == nkb - 1) umma_commit(smem_u32(&o_full[ob]));
-        }
-        __syncwarp();
       }
     }
-  } else {
-    // ------------------------------------------------------------------ softmax + epilogue groups
-    const int g = warp >> 3;                  // group 0: warps 0-7, group 1: warps 8-15
-    const int q = warp & 3;                   // TMEM lane quarter this warp may access
-    const int hf = (warp >> 2) & 1;           // which half of the key chunks / of the O columns this warp handles
-    const int row = q * 32 + lane;            // query row of this thread inside the tile
-    const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-    const float sc = p.scale_log2e;
-    const int npad = (nkb - 1) * KBLK + p.rem;          // keys padded to 16
-    float* const red_max = s_red + g * 512;             // [half][row]
-    float* const red_sum = red_max + 256;
-    auto group_sync = [&]() { asm volatile("bar.sync %0, 256;" ::"r"(1 + g) : "memory"); };
-    // this warp's half of the O row / sum -> split16 -> global
-    auto epilogue = [&](int jj, float sum) {
-      const Item it = decode_item((int)blockIdx.x + jj * (int)gridDim.x, p);
-      const int ob = jj % NOB;
-      const int rows_valid = min(128, p.Lq - it.qt * 128);
-      const bool active = q * 32 < rows_valid;
-      mbar_wait(smem_u32(&o_full[ob]), ((uint32_t)(jj / NOB)) & 1u);
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 34, jj);                                    // softmax: O(jj) ready
-      if (active) {
-        const float inv = 1.0f / sum;
-        constexpr int OC = HD / 2;                           // O columns per warp
-        const uint32_t o_addr = tmem_base + lane_addr + (uint32_t)(SB * scols + ob * HD + hf * OC);
-        const int64_t o = ((int64_t)it.s * p.Lq + it.qt * 128 + row) * p.ld_out + it.h * HD + hf * OC;
-        uint4* const dh = reinterpret_cast<uint4*>(p.out_hi + o);
-        uint4* const dl = reinterpret_cast<uint4*>(p.out_lo + o);
-#pragma unroll
-        for (int c = 0; c < OC / 16; ++c) {
-          uint32_t r[16];
-          tmem_ld16(o_addr + (uint32_t)(c * 16), r);
-          uint32_t oh[8], ol[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            split2(__uint_as_float(r[2 * i]) * inv, __uint_as_float(r[2 * i + 1]) * inv, oh[i], ol[i]);
-          if (row < rows_valid) {
-            dh[2 * c] = make_uint4(oh[0], oh[1], oh[2], oh[3]);
-            dh[2 * c + 1] = make_uint4(oh[4], oh[5], oh[6], oh[7]);
-            dl[2 * c] = make_uint4(ol[0], ol[1], ol[2], ol[3]);
-            dl[2 * c + 1] = make_uint4(ol[4], ol[5], ol[6], ol[7]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      tl_event(p.tl, tl_n, 35, jj);                                    // softmax: epilogue done
-      if (lane == 0) mbar_arrive(smem_u32(&o_empty[ob]));
-    };
-    int pend = -1;                                       // item whose epilogue is still owed (NOB == 4)
-    float pend_sum = 0.0f;
-    for (int j = g; j < nlocal; j += 2) {
-      const Item it = decode_item((int)blockIdx.x + j * (int)gridDim.x, p);
-      const int sb = j % SB;
-      const int rows_valid = min(128, p.Lq - it.qt * 128);
-      const bool active = q * 32 < rows_valid;          // warp-uniform: this warp owns real query rows
-      int nk = p.Lk;
-      if (p.lengths) nk = min(p.Lk, p.kv_prefix + p.lengths[p.len_mod > 0 ? (p.seq0 + it.s) % p.len_mod : it.s]);
-      const uint32_t s_addr = tmem_base + lane_addr + (uint32_t)(sb * scols);
-      tl_event(p.tl, tl_n, 30, j);                                     // softmax: waiting for S(j)
-      mbar_wait(smem_u32(&s_full[g]), ((uint32_t)j >> 1) & 1u);
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 31, j);                                     // softmax: S(j) ready
-      // ---- pass 1: maximum over this warp's 16-key chunks (c = hf, hf + 2, ...), then over both halves
-      float mx = -INFINITY;
-      if (active) {
-#pragma unroll 1
-        for (int c = hf; c < npad / 16; c += 2) {
-          uint32_t r[16];
-          tmem_ld16(s_addr + (uint32_t)(c * 16), r);
-#pragma unroll
-          for (int i = 0; i < 16; ++i) mx = fmaxf(mx, (c * 16 + i < nk) ? __uint_as_float(r[i]) : -INFINITY);
-        }
-      }
-      red_max[hf * 128 + row] = mx;
-      tl_event(p.tl, tl_n, 32, j);                                     // softmax: pass 1 done
-      group_sync();
-      mx = fmaxf(mx, red_max[(hf ^ 1) * 128 + row]);
-      const float mc = (mx == -INFINITY) ? 0.0f : mx * sc;
-      // ---- pass 2: P = exp2(sc * s - sc * max) (unnormalised), fp32 partial row sum, P -> shared memory
-      // The two groups take turns on the p_empty barriers, so each sees only every other phase: its parity wait
-      // for "PV(pseq - 2) done" is only correct if the phase before that one (this group's own previous item)
-      // has completed - otherwise the wait aliases and passes at once.  Without the deferred epilogue that is
-      // implied (the group has read O(j - 2)); with it, it is checked here - long satisfied in steady state.
-      if (NOB == 4 && pend >= 0) mbar_wait(smem_u32(&o_full[pend % NOB]), ((uint32_t)(pend / NOB)) & 1u);
-      float sum = 0.0f;
-#pragma unroll 1
-      for (int kb = 0; kb < nkb; ++kb) {
-        const int pseq = j * nkb + kb, pb = pseq & 1;
-        mbar_wait(smem_u32(&p_empty[pb]), (((uint32_t)pseq >> 1) & 1u) ^ 1u);    // PV(pseq - 2) has read the buffer
-        if (active) {
-          const int nch = (kb == nkb - 1 ? p.rem : KBLK) / 16;
-          // row `row` of the [128 x 64] K-major SWIZZLE_128B tile: 16-B chunk index XOR (row & 7)
-          uint8_t* const prow = sP + pb * P_BYTES + row * 128;
-#pragma unroll 1
-          for (int c = hf; c < nch; c += 2) {
-            uint32_t r[16];
-            tmem_ld16(s_addr + (uint32_t)(kb * KBLK + c * 16), r);
-            uint32_t ph[8], pl[8];
-            const int k0 = kb * KBLK + c * 16;
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              float e0, e1;
-              asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(__uint_as_float(r[2 * i]), sc, -mc)));
-              asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(__uint_as_float(r[2 * i + 1]), sc, -mc)));
-              e0 = (k0 + 2 * i < nk) ? e0 : 0.0f;
-              e1 = (k0 + 2 * i + 1 < nk) ? e1 : 0.0f;
-              sum += e0 + e1;
-              split2(e0, e1, ph[i], pl[i]);
-            }
-            const int o0 = ((2 * c) ^ (row & 7)) << 4, o1 = ((2 * c + 1) ^ (row & 7)) << 4;
-            *reinterpret_cast<uint4*>(prow + o0) = make_uint4(ph[0], ph[1], ph[2], ph[3]);
-            *reinterpret_cast<uint4*>(prow + o1) = make_uint4(ph[4], ph[5], ph[6], ph[7]);
-            *reinterpret_cast<uint4*>(prow + 16384 + o0) = make_uint4(pl[0], pl[1], pl[2], pl[3]);
-            *reinterpret_cast<uint4*>(prow + 16384 + o1) = make_uint4(pl[4], pl[5], pl[6], pl[7]);
-          }
-          fence_proxy_async_smem();                      // generic-proxy writes -> tcgen05.mma reads
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&p_full[pb]));
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&s_empty[g]));     // the score buffer may be overwritten
-      red_sum[hf * 128 + row] = sum;
-      tl_event(p.tl, tl_n, 33, j);                                     // softmax: pass 2 done (P written)
-      group_sync();
-      sum += red_sum[(hf ^ 1) * 128 + row];
-      // ---- epilogue.  With four O accumulators the epilogue of this group's PREVIOUS item runs here instead
-      // (its PV chain retired long ago), so the group never waits for the tensor pipe between its softmax
-      // passes and its stores: the wait for O(j) used to be ~2.3k of the ~10k cycles a group spends per item.
-      if (NOB == 4) {
-        if (pend >= 0) epilogue(pend, pend_sum);
-        pend = j; pend_sum = sum;
-      } else {
-        epilogue(j, sum);
-      }
-    }
-    if (pend >= 0) epilogue(pend, pend_sum);
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
+  // -------------------------------------------------------------------- consumer warpgroup of pipeline g
+  reg_inc<232>();
+  const int cp = 2 * (lane & 3);                      // column offset inside an 8-column group
+  const int row = (warp & 3) * 16 + (lane >> 2);      // this thread's first query row (the second is row + 8)
+  const float sc = p.scale_log2e;
+  float S[MAX_KB][32];                                // the score row: [key block][accumulator fragment of 64 keys]
+  float O[NS][32];
+  int rc = 0;
+  for (int j = 0; j < nlocal; ++j) {
+    const Item it = decode_item(pid + j * npipes, p);
+    int nk = p.Lk;
+    if (p.lengths) nk = min(p.Lk, p.kv_prefix + p.lengths[p.len_mod > 0 ? (p.seq0 + it.s) % p.len_mod : it.s]);
+    mbar_wait(smem_u32(q_full), (uint32_t)j & 1u);
+    tl_event(p.tl, tl_n, 22, j);                                       // Q(j) landed
+    // ---- S = Q K^T, block by block; a block's ring slot is freed when the NEXT block's MMAs have been issued
+    const uint32_t qbase = smem_u32(sQ);
+#pragma unroll
+    for (int kb = 0; kb < MAX_KB; ++kb) {
+      if (kb < nkb) {
+        const int sl_i = (rc + kb) % RS;
+        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
+        const uint32_t kbase = smem_u32(sR + sl_i * SLOT_BYTES);
+        wg_fence();
+#pragma unroll
+        for (int sl = 0; sl < NS; ++sl) {
+          uint64_t qh = make_desc(qbase + sl * TILE), ql = make_desc(qbase + SL_PLANE + sl * TILE);
+          uint64_t kh = make_desc(kbase + sl * TILE), kl = make_desc(kbase + SL_PLANE + sl * TILE);
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            wgmma_ss_n64(S[kb], ql, kh, (sl | kk) != 0 ? 1u : 0u);
+            wgmma_ss_n64(S[kb], qh, kl, 1u);
+            wgmma_ss_n64(S[kb], qh, kh, 1u);
+            qh += 2; ql += 2; kh += 2; kl += 2;       // next 16 elements of the head dimension: +32 B
+          }
+        }
+        wg_commit();
+        if (kb > 0) {
+          wg_wait<1>();
+          if (lane == 0) mbar_arrive(smem_u32(&r_empty[(rc + kb - 1) % RS]));
+        }
+      }
+    }
+    wg_wait<0>();
+    if (lane == 0) {
+      mbar_arrive(smem_u32(&r_empty[(rc + nkb - 1) % RS]));
+      mbar_arrive(smem_u32(q_empty));                 // Q only feeds the scores
+    }
+    rc += nkb;
+#pragma unroll
+    for (int kb = 0; kb < MAX_KB; ++kb)
+      if (kb < nkb) acc_fence(S[kb]);
+    tl_event(p.tl, tl_n, 31, j);                                       // softmax: S(j) ready
+    // ---- pass 1: row maxima over the valid keys (a row is spread over the 4 lanes of a quad)
+    float mx0 = -INFINITY, mx1 = -INFINITY;
+#pragma unroll
+    for (int kb = 0; kb < MAX_KB; ++kb) {
+      if (kb < nkb) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool valid = kb * KBLK + 8 * jj + cp + e < nk;
+            mx0 = fmaxf(mx0, valid ? S[kb][4 * jj + e] : -INFINITY);
+            mx1 = fmaxf(mx1, valid ? S[kb][4 * jj + 2 + e] : -INFINITY);
+          }
+        }
+      }
+    }
+    mx0 = quad_max(mx0); mx1 = quad_max(mx1);
+    const float mc0 = (mx0 == -INFINITY) ? 0.0f : mx0 * sc, mc1 = (mx1 == -INFINITY) ? 0.0f : mx1 * sc;
+    // ---- pass 2: P = exp2(sc * s - sc * max) (unnormalised, in place), fp32 row sums
+    float sum0 = 0.0f, sum1 = 0.0f;
+#pragma unroll
+    for (int kb = 0; kb < MAX_KB; ++kb) {
+      if (kb < nkb) {
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const bool valid = kb * KBLK + 8 * jj + cp + e < nk;
+            float e0, e1;
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(S[kb][4 * jj + e], sc, -mc0)));
+            asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(S[kb][4 * jj + 2 + e], sc, -mc1)));
+            e0 = valid ? e0 : 0.0f;
+            e1 = valid ? e1 : 0.0f;
+            S[kb][4 * jj + e] = e0; S[kb][4 * jj + 2 + e] = e1;
+            sum0 += e0; sum1 += e1;
+          }
+        }
+      }
+    }
+    sum0 = quad_sum(sum0); sum1 = quad_sum(sum1);
+    tl_event(p.tl, tl_n, 33, j);                                       // softmax: pass 2 done
+    // ---- O = P V, block by block: P re-split to hi / lo fp16 A fragments, 16 keys per k-step
+#pragma unroll
+    for (int kb = 0; kb < MAX_KB; ++kb) {
+      if (kb < nkb) {
+        uint32_t ph[4][4], pl[4][4];
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) split2(S[kb][8 * ks + 2 * i], S[kb][8 * ks + 2 * i + 1], ph[ks][i], pl[ks][i]);
+        const int sl_i = (rc + kb) % RS;
+        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
+        const uint32_t vbase = smem_u32(sR + sl_i * SLOT_BYTES);
+        const int nks = (kb == nkb - 1 ? p.rem : KBLK) / 16;           // rows beyond `rem` of the slot are stale
+        wg_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          if (ks < nks) {
+#pragma unroll
+            for (int sl = 0; sl < NS; ++sl) {
+              // next 16 keys of the MN-major V tile: +2048 B
+              const uint64_t vh = make_desc(vbase + sl * TILE) + ks * 128, vl = make_desc(vbase + SL_PLANE + sl * TILE) + ks * 128;
+              wgmma_rs_n64_tb(O[sl], pl[ks], vh, (kb | ks) != 0 ? 1u : 0u);
+              wgmma_rs_n64_tb(O[sl], ph[ks], vl, 1u);
+              wgmma_rs_n64_tb(O[sl], ph[ks], vh, 1u);
+            }
+          }
+        }
+        wg_commit();
+        wg_wait<0>();
+        if (lane == 0) mbar_arrive(smem_u32(&r_empty[sl_i]));
+      }
+    }
+    rc += nkb;
+#pragma unroll
+    for (int sl = 0; sl < NS; ++sl) acc_fence(O[sl]);
+    tl_event(p.tl, tl_n, 34, j);                                       // O(j) ready
+    // ---- epilogue: O / sum -> split16 -> global
+    const float inv0 = 1.0f / sum0, inv1 = 1.0f / sum1;
+    const int qrow = it.qt * QROWS + row;
+    const int64_t o0 = ((int64_t)it.s * p.Lq + qrow) * p.ld_out + it.h * HD + cp, o1 = o0 + (int64_t)8 * p.ld_out;
+#pragma unroll
+    for (int sl = 0; sl < NS; ++sl) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        uint32_t h, l;
+        if (qrow < p.Lq) {
+          split2(O[sl][4 * jj] * inv0, O[sl][4 * jj + 1] * inv0, h, l);
+          *reinterpret_cast<uint32_t*>(p.out_hi + o0 + sl * 64 + 8 * jj) = h;
+          *reinterpret_cast<uint32_t*>(p.out_lo + o0 + sl * 64 + 8 * jj) = l;
+        }
+        if (qrow + 8 < p.Lq) {
+          split2(O[sl][4 * jj + 2] * inv1, O[sl][4 * jj + 3] * inv1, h, l);
+          *reinterpret_cast<uint32_t*>(p.out_hi + o1 + sl * 64 + 8 * jj) = h;
+          *reinterpret_cast<uint32_t*>(p.out_lo + o1 + sl * 64 + 8 * jj) = l;
+        }
+      }
+    }
+    tl_event(p.tl, tl_n, 35, j);                                       // epilogue done
+  }
   tl_event(p.tl, tl_n, 42);                       // kernel exit
-  if (warp == WARP_MMA) {
-    tc_fence_after();
-    tmem_dealloc<1>(tmem_base, 512);
-  }
 }
 
 PFN_tmapEncodeTiled g_encode = nullptr;
-int g_sm_count = 148;
+int g_sm_count = 132;
 bool g_ready = false;
 
 // fp16 plane [rows, cols]; box = 64 columns x box_rows rows, SWIZZLE_128B, out-of-bounds rows zero-filled
@@ -463,29 +335,11 @@ bool make_map(CUtensorMap* m, const __half* base, int rows, int cols, int box_ro
 
 // launch geometry for a shape; false when it does not fit
 bool plan_shape(const AttnArgs& a, AtcParams* p) {
-  const int ns = a.hd / 64;
   const int npad = (a.Lk + 15) & ~15;
   p->nkb = (npad + KBLK - 1) / KBLK;
   p->rem = npad - (p->nkb - 1) * KBLK;
-  p->n_qt = (a.Lq + 127) / 128;
-  p->QR = p->n_qt > 1 ? 128 : ((a.Lq + 7) & ~7);
-  const int scols = p->nkb * KBLK;
-  if (scols + 2 * a.hd > 512) return false;
-  p->SB = (2 * scols + 2 * a.hd <= 512) ? 2 : 1;
-  static const int max_nob = [] { const char* e = getenv("MLDB_ATTN_NOB"); return e ? atoi(e) : 4; }();   // A/B knob
-  p->NOB = (max_nob >= 4 && p->SB * scols + 4 * a.hd <= 512) ? 4 : 2;
-  const int q_bytes = 2 * ns * p->QR * 128, slot = 2 * ns * KBLK * 128;
-  const int fixed = 1024 + 2 * P_BYTES + RED_BYTES + 512;   // alignment slack + P ring + exchange buffers + barriers
-  for (int qb = 2; qb >= 1; --qb) {
-    const int left = SMEM_LIMIT - fixed - qb * q_bytes;
-    const int rs = left / slot;
-    if (rs >= 2) { p->QB = qb; p->RS = rs < MAX_RS ? rs : MAX_RS; return true; }
-  }
-  return false;
-}
-int smem_bytes(const AttnArgs& a, const AtcParams& p) {
-  const int ns = a.hd / 64;
-  return 1024 + p.QB * 2 * ns * p.QR * 128 + p.RS * 2 * ns * KBLK * 128 + 2 * P_BYTES + RED_BYTES + 512;
+  p->n_qt = (a.Lq + QROWS - 1) / QROWS;
+  return p->nkb <= MAX_KB;
 }
 
 }  // namespace
@@ -499,8 +353,8 @@ bool tc_attention_init(int device) {
     return false;
   g_encode = (PFN_tmapEncodeTiled)fn;
   cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, device);
-  if (cudaFuncSetAttribute(k_attn_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT) != cudaSuccess ||
-      cudaFuncSetAttribute(k_attn_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_LIMIT) != cudaSuccess)
+  if (cudaFuncSetAttribute(k_attn_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+      cudaFuncSetAttribute(k_attn_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
     return false;
   g_ready = true;
   return true;
@@ -519,7 +373,7 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   AtcParams p{};
   if (!plan_shape(a, &p)) return false;
   CUtensorMap mQh, mQl, mKh, mKl, mRh, mRl;
-  const bool ok = make_map(&mQh, a.q.hi, a.q.rows, a.q.cols, p.QR) && make_map(&mQl, a.q.lo(), a.q.rows, a.q.cols, p.QR) &&
+  const bool ok = make_map(&mQh, a.q.hi, a.q.rows, a.q.cols, QROWS) && make_map(&mQl, a.q.lo(), a.q.rows, a.q.cols, QROWS) &&
                   make_map(&mKh, a.kv.hi, a.kv.rows, a.kv.cols, KBLK) && make_map(&mKl, a.kv.lo(), a.kv.rows, a.kv.cols, KBLK) &&
                   make_map(&mRh, a.kv.hi, a.kv.rows, a.kv.cols, p.rem) && make_map(&mRl, a.kv.lo(), a.kv.rows, a.kv.cols, p.rem);
   if (!ok) return false;
@@ -530,18 +384,18 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   p.scale_log2e = 1.4426950408889634f / sqrtf((float)a.hd);
   p.tl = tc::mldb_timeline_buffer();
   // Snake order across the per-layer kernels: the GEMMs walk the token tiles upwards, attention and the fused FFN
-  // downwards, so every kernel starts on the rows its producer wrote LAST - those are still in the 126 MB L2,
-  // the rows written first (41-124 MB earlier) are not.  MLDB_SNAKE=0 turns it off (A/B).
+  // downwards, so every kernel starts on the rows its producer wrote LAST - those are the ones most likely to be
+  // still in L2.  MLDB_SNAKE=0 turns it off (A/B).
   static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
   p.reverse = snake;
   p.items = p.nseq * p.heads * p.n_qt;
   p.heads_log2 = -1;
   for (int k = 0; k < 8; ++k) if ((1 << k) == p.heads) p.heads_log2 = k;
-  const int items = a.nseq * a.heads * p.n_qt;
-  const int grid = items < g_sm_count ? items : g_sm_count;
+  const int pairs = (p.items + 1) / 2;                 // two pipelines per CTA
+  const int grid = pairs < g_sm_count ? pairs : g_sm_count;
   if (a.hd == 64)
-    launch_pdl(k_attn_tc<64>, dim3(grid), dim3(ATC_THREADS), (size_t)smem_bytes(a, p), st, mQh, mQl, mKh, mKl, mRh, mRl, p);
+    launch_pdl(k_attn_tc<64>, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
   else
-    launch_pdl(k_attn_tc<128>, dim3(grid), dim3(ATC_THREADS), (size_t)smem_bytes(a, p), st, mQh, mQl, mKh, mKl, mRh, mRl, p);
+    launch_pdl(k_attn_tc<128>, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
   return true;
 }

@@ -1,4 +1,4 @@
-// Shared device/host helpers for libmldb200 (sm_100a only).
+// Shared device/host helpers for libmldb200 (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -47,54 +47,10 @@ __device__ __forceinline__ float gelu_fast(float x) {
   const float erf_abs = fmaf(-poly * t, e, 1.0f);
   return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
-// ---- packed fp32 pairs (sm_100 FFMA2 / FMUL2 / FADD2: two IEEE fp32 operations per instruction)
-__device__ __forceinline__ uint64_t f2_pack(float a, float b) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(a), "f"(b));
-  return r;
-}
-__device__ __forceinline__ void f2_unpack(uint64_t v, float& a, float& b) { asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(v)); }
-__device__ __forceinline__ uint64_t f2_fma(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t f2_mul(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-// gelu_fast on two values at once: the same A&S 7.1.26 erf, polynomial and products on the packed pipe
-// (the MUFU rcp / ex2 and the sign transfer stay scalar).  y = 0.5x + 0.5x*erf(x/sqrt2).
-__device__ __forceinline__ void gelu_fast2(float& x0, float& x1) {
-  const uint64_t x = f2_pack(x0, x1);
-  const uint64_t z = f2_mul(f2_pack(fabsf(x0), fabsf(x1)), f2_pack(0.70710678118654752440f, 0.70710678118654752440f));
-  float d0, d1;
-  f2_unpack(f2_fma(f2_pack(0.3275911f, 0.3275911f), z, f2_pack(1.0f, 1.0f)), d0, d1);
-  float t0, t1;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t0) : "f"(d0));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t1) : "f"(d1));
-  const uint64_t t = f2_pack(t0, t1);
-  // -(a1 t + a2 t^2 + ... + a5 t^5) with negated coefficients, so erf = 1 + npoly*e needs no negation
-  uint64_t np = f2_fma(f2_pack(-1.061405429f, -1.061405429f), t, f2_pack(1.453152027f, 1.453152027f));
-  np = f2_fma(np, t, f2_pack(-1.421413741f, -1.421413741f));
-  np = f2_fma(np, t, f2_pack(0.284496736f, 0.284496736f));
-  np = f2_fma(np, t, f2_pack(-0.254829592f, -0.254829592f));
-  np = f2_mul(np, t);
-  float a0, a1;
-  f2_unpack(f2_mul(f2_mul(z, z), f2_pack(-1.4426950408889634f, -1.4426950408889634f)), a0, a1);
-  float e0, e1;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(a0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(a1));
-  float r0, r1;
-  f2_unpack(f2_fma(np, f2_pack(e0, e1), f2_pack(1.0f, 1.0f)), r0, r1);      // |erf|
-  const uint64_t hx = f2_mul(x, f2_pack(0.5f, 0.5f));
-  f2_unpack(f2_fma(hx, f2_pack(copysignf(r0, x0), copysignf(r1, x1)), hx), x0, x1);
-}
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization
-// attribute may begin (prologue: barrier init, TMEM alloc, weight staging) while its predecessor
+// attribute may begin (prologue: barrier init, descriptor prefetch) while its predecessor
 // drains; it must execute pdl_wait() before touching anything the predecessor produced or reads.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

@@ -359,7 +359,7 @@ static void op_gemm(mldb_handle* h, const GemmArgs& g, cudaStream_t st) {
   simt_gemm(g, st);
   kcount(h, MLDB_KSTAT_GEMM_SIMT);
 }
-// GEMM followed by residual + LayerNorm (one fused tcgen05 kernel when the tile covers a row)
+// GEMM followed by residual + LayerNorm (one fused wgmma kernel when the tile covers a row)
 static void op_gemm_ln(mldb_handle* h, GemmArgs g, LnArgs l, float* cf32, cudaStream_t st) {
   if (h->use_tc && tc_gemm_ln_supported(h->tc, g, l)) {
     if (!tc_gemm(h->tc, g, &l, st)) h->op_failed = true;
@@ -388,7 +388,7 @@ static void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st) {
 // the fused FFN block when the shape allows it, else the two GEMMs
 static void op_ffn(mldb_handle* h, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* cf32, cudaStream_t st) {
   if (h->use_tc && tc_ffn_supported(h->tc, g1, g2, l2)) {
-    // one launch: the hidden activations stay in shared memory / TMEM (gemm_tc.cu k_ffn_tc)
+    // one launch: the hidden activations stay in registers (gemm_tc.cu k_ffn_tc)
     int k = 0;                                     // which stream: its own scratch (branches run concurrently)
     for (int i = 0; i < mldb_handle::MAX_BRANCHES - 1; ++i) if (st == h->br_stream[i]) k = i + 1;
     if (!tc_ffn(h->tc, g1, g2, l2, h->ffn_scratch[k], h->ffn_flags[k], st)) h->op_failed = true;
@@ -624,7 +624,7 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   if (device < 0 || device >= ndev) FAIL(MLDB_ERR_INVALID, "no such CUDA device %d (no CPU fallback exists)", device);
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) FAIL(MLDB_ERR_UNSUPPORTED, "device %d is sm_%d%d; libmldb200 is sm_100a only", device, prop.major, prop.minor);
+  if (prop.major != 9) FAIL(MLDB_ERR_UNSUPPORTED, "device %d is sm_%d%d; libmldb200 is sm_90a only", device, prop.major, prop.minor);
   DeviceGuard guard(device);
   mldb_handle* h = new mldb_handle();
   h->cfg = *cfg; h->device = device; h->sm_count = prop.multiProcessorCount;
@@ -636,7 +636,7 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   mma_attention_init();
   h->tc = tc_create(device);
   if (!h->tc) { delete h; return MLDB_ERR_CUDA; }
-  if (!tc_attention_init(device)) { tc_destroy(h->tc); delete h; FAIL(MLDB_ERR_CUDA, "tcgen05 attention kernel: setup failed"); }
+  if (!tc_attention_init(device)) { tc_destroy(h->tc); delete h; FAIL(MLDB_ERR_CUDA, "wgmma attention kernel: setup failed"); }
   const char* env = getenv("MLDB_GEMM");
   if (env && !strcmp(env, "simt")) h->use_tc = false;
   env = getenv("MLDB_GRAPH");
@@ -1657,7 +1657,7 @@ extern "C" int mldb_profile_steps(mldb_handle* h, const void* cond, const float*
 
 // ----------------------------------------------------------------------------- debug aid
 // y = act(A W^T + b) or LayerNorm(A W^T + b + R) through the engine's GEMM operators, so tests can
-// compare the tcgen05 kernels with the CUDA-core kernels (and with torch) shape by shape.
+// compare the wgmma kernels with the CUDA-core kernels (and with torch) shape by shape.
 //   A [M,K] fp32 device; W [N,K], bias [N], gamma/beta [N] fp32 HOST (gamma == NULL: no LN);
 //   R [M,N] fp32 device or NULL; K1 < K splits A into two concatenated sources (skip connection);
 //   out [M,N] fp32 device.  use_tc: 1 tensor-core path, 0 CUDA-core path.  Synchronous.

@@ -117,14 +117,14 @@ struct mldb_handle {
   int64_t launches = 0;
   int64_t capture_nodes = 0;
   bool capturing = false;
-  bool use_tc = true;        // tcgen05 GEMMs (option gemm=simt switches to the CUDA-core path)
+  bool use_tc = true;        // wgmma GEMMs (option gemm=simt switches to the CUDA-core path)
   bool use_graph = true;
   // Concurrent sub-batches: the denoiser stack runs as `branches` independent sequence ranges on
   // parallel streams (parallel chains inside the captured graph), each with its own workspace rows,
-  // so one range's kernel tails (316 m-tiles on 148 SMs = 2.13 rounds) and kernel boundaries are
+  // so one range's kernel tails (316 m-tiles on 132 SMs = 2.39 rounds) and kernel boundaries are
   // filled by the other range's kernels.  1 = off.
   int branches = 2;
-  int attn_kind = 0;         // 0 = tcgen05 (attn_tc.cu), 1 = mma.sync (attn_mma.cu), 2 = CUDA-core; option `attn`
+  int attn_kind = 0;         // 0 = wgmma (attn_tc.cu), 1 = mma.sync (attn_mma.cu), 2 = CUDA-core; option `attn`
   // which kernel every operator of the path was ENQUEUED on (recorded launches, incl. graph capture);
   // read through mldb_kernel_stats so that tests can assert "nothing fell back to CUDA cores"
   int64_t kstat[MLDB_KSTAT_COUNT] = {};

@@ -1,34 +1,28 @@
-// tcgen05 (5th-gen tensor core) split-fp16 kernels for sm_100a: the persistent GEMM with fused
-// epilogues (k_gemm_tc) and the fused FFN block (k_ffn_tc).
+// Warpgroup-MMA (wgmma) split-fp16 kernels for sm_90a: the persistent GEMM with fused epilogues
+// (k_gemm_tc) and the fused FFN block (k_ffn_tc).
 //
-//   D[128 x BN] (fp32, TMEM) = A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T        per 128-row tile
+//   D[128 x BN] (fp32, registers) = A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T        per 128-row tile
 //
 // A = activations in the split16 format (two fp16 planes, row-major [M, K]); W = nn.Linear weight
 // [N, K] (PyTorch's [out, in] layout is already the K-major B operand), also split into hi/lo
-// planes.  Three kind::f16 MMAs per K-step reproduce the reference's fp32 GEMM to ~1e-6.
+// planes.  Three f16 MMAs per K-step reproduce the reference's fp32 GEMM to ~1e-6.
 //
-// CTA = 10 warps, one CTA per SM, persistent over tiles: warp 0 = TMA producer, warp 1 = TMEM
-// allocator + MMA issuer (both walk their loops warp-uniformly, one elect.sync lane issues), warps
-// 2..9 = epilogue.  Operands stream through a ring of 128B-swizzled shared-memory tiles (BK = 64
-// halves = one swizzle row) filled by cp.async.bulk.tensor (TMA) and released by tcgen05.commit;
-// accumulators are double-buffered in TMEM and read back with tcgen05.ld.  CG = 2 runs CTA pairs
-// (cta_group::2, M = 256 MMAs issued by the leader, each CTA stages its own A rows and half of the
-// W tile).
-// Epilogues:
-//   plain (LN = false): two warps per TMEM lane quarter split the columns; bias (+ positional
-//       table) + activation -> split16 (TMA bulk stores on the pair kernels, st.global through a
-//       warp transpose otherwise) / fp32 store.
-//   LayerNorm (LN = true, BN == N == 256): the eight epilogue warps form two groups of four that
-//       take alternate tiles (group g drains accumulator stage g), so a thread owns a COMPLETE row:
-//       bias + residual (coalesced loads through a warp transpose, prefetched two 32-column chunks
-//       ahead) + one-pass shifted statistics with the pre-norm row parked in TMEM, then normalise
-//       -> split16 -> TMA bulk stores.  No cross-warp exchange, rolled loops (the round-1 unrolled
-//       epilogue spent ~30 % of its stall samples on instruction fetch).
+// CTA = three warpgroups, one CTA per SM, persistent over tiles: warpgroup 0 gives its registers
+// away (setmaxnreg) and its first warp is the TMA producer; warpgroups 1 and 2 each own 64 rows of
+// the tile, issue wgmma.mma_async on operands that stream through a ring of 128B-swizzled
+// shared-memory tiles (BK = 64 halves = one swizzle row) and run the epilogue on their accumulator
+// registers while the producer already fills the ring for the next tile.
+// Epilogues (a thread holds column pairs of two rows, a row is spread over the 4 lanes of a quad):
+//   fast:      bias + activation -> split16, identity row mapping (the per-layer GEMMs)
+//   generic:   + positional table, row remapping, zeroed padding rows, fp32 output, ragged N
+//   LayerNorm: BN == N == 256, so a quad owns COMPLETE rows: bias + residual, exact two-pass
+//              statistics over the registers with quad shuffles, normalise -> split16.
 #include "gemm_tc.h"
 
 #include <stdio.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <string>
 #include <string.h>
 
@@ -40,6 +34,9 @@ namespace {
 using namespace tc;
 
 constexpr int BM = 128, BK = 64;
+constexpr int NUM_THREADS = 384;                     // producer warpgroup + two consumer warpgroups
+constexpr int CONSUMER_WARPS = 8;
+constexpr int MAX_N = 1024;
 
 // ------------------------------------------------------------------------------ parameters
 struct TcParams {
@@ -56,423 +53,168 @@ struct TcParams {
   // residual + LayerNorm epilogue
   const __half* res_hi; const __half* res_lo; int ld_res;
   const float* gamma; const float* beta;
-  int tma_out;   // the epilogue drains through TMA stores (maps tmOh / tmOl cover out + out_col0)
   long long* tl; // debug timeline (nullptr normally)
 };
 
-constexpr int EPI_WARPS = 8;
-constexpr int NUM_THREADS = 64 + EPI_WARPS * 32;     // producer warp + MMA warp + epilogue warps
-// The kernels with a LayerNorm epilogue (k_gemm_tc<EPI_LN>, k_ffn_tc) run SIXTEEN epilogue warps: the LayerNorm
-// of a 128 x 256 tile is a chain of TMEM loads, shared-memory transposes and conversions that is latency-bound
-// per warp (the in-kernel timeline showed ~12k cycles per tile on 8 warps, IPC < 0.4 per scheduler), so it gets
-// four warps per scheduler instead of two.  576 threads -> 112 registers per thread.
-constexpr int LN_WARPS = 16;
-constexpr int LN_THREADS = 64 + LN_WARPS * 32;
-constexpr int MAX_N = 1024;                          // bias staging capacity
-
 enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2 };     // epilogue variants of k_gemm_tc (see the kernel)
 
-template <int BN, int CG = 1, int EPI = EPI_GENERIC>
+template <int BN>
 struct TileCfg {
-  // The per-layer plain GEMMs (256-wide tiles on CTA pairs, fast epilogue) get a THREE-deep ring: with two
-  // 64 KB stages a stage's round trip (TMA issue -> L2 -> MMA -> commit -> producer wake-up) did not fit under
-  // one k-block of MMA work and the main loop ran at 2.1-2.6k cycles per k-block instead of 1.57k (in-kernel
-  // timeline).  The third stage is paid for by single-buffering the TMA-store staging and reading the bias
-  // straight from global memory (L1-resident broadcast loads) instead of staging it.
-  static constexpr bool DEEP = EPI == EPI_FAST && BN == 256 && CG == 2;
-  static constexpr int STAGES = (BN == 256 && !DEEP) ? 2 : 3;
   static constexpr int A_BYTES = BM * BK * 2;          // one plane of the A tile (16 KB)
-  static constexpr int W_BYTES = BN / CG * BK * 2;     // one plane of this CTA's part of the W tile
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
-  static constexpr int TMEM_COLS = 2 * BN;             // double-buffered accumulator
-  // per-warp staging: one 32 rows x 64 B transpose buffer (CG = 1: st.global epilogue) or {hi, lo} pairs of
-  // them (CG = 2: the epilogue drains through TMA bulk stores; two pairs alternate unless DEEP)
-  static constexpr int NEPI = EPI == EPI_LN ? LN_WARPS : EPI_WARPS;       // epilogue warps
-  static constexpr int STG_WARP = CG == 2 ? ((DEEP || EPI == EPI_LN) ? 4096 : 8192) : 2048;
-  static constexpr int STG_BYTES = NEPI * STG_WARP;
-  static constexpr int VEC_BYTES = DEEP ? 0 : MAX_N * 4 + 2 * 256 * 4;     // bias[MAX_N] + gamma[256] + beta[256]
-  static constexpr int PART_BYTES = EPI == EPI_LN ? 4 * 2 * 128 * 4 : 0;   // LayerNorm partial statistics
-  static constexpr int AUX_BYTES = VEC_BYTES + PART_BYTES + 256 + STG_BYTES;   // + barriers
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + AUX_BYTES + 1024;   // + alignment slack
+  static constexpr int W_BYTES = BN * BK * 2;          // one plane of the W tile
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;       // 96 KB (BN = 256) / 64 KB
+  static constexpr int STAGES = BN == 256 ? 2 : 3;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;   // + barriers + alignment slack
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-// fp32 x32 -> split16 hi/lo planes (64 B each) with packed conversions
-__device__ __forceinline__ void store_split_chunk(const float (&v)[32], __half* hi, __half* lo) {
-  uint32_t ph[16], pl[16];
+template <int BN>
+__device__ __forceinline__ void wgmma_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  if constexpr (BN == 256) wgmma_ss_n256(d, a, b, acc);
+  else if constexpr (BN == 128) wgmma_ss_n128(d, a, b, acc);
+  else wgmma_ss_n64(d, a, b, acc);
+}
+// one k-block (64 deep) of this warpgroup's [64 x BN] tile: 4 x (A_lo.W_hi + A_hi.W_lo + A_hi.W_hi)
+template <int BN>
+__device__ __forceinline__ void kblock_ss(float (&d)[BN / 2], uint32_t sAh, uint32_t sAl, uint32_t sWh, uint32_t sWl, bool first) {
+  uint64_t ah = make_desc(sAh), al = make_desc(sAl), wh = make_desc(sWh), wl = make_desc(sWl);
 #pragma unroll
-  for (int i = 0; i < 16; ++i) split2(v[2 * i], v[2 * i + 1], ph[i], pl[i]);
-  uint4* dh = reinterpret_cast<uint4*>(hi);
-  uint4* dl = reinterpret_cast<uint4*>(lo);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    dh[i] = make_uint4(ph[4 * i], ph[4 * i + 1], ph[4 * i + 2], ph[4 * i + 3]);
-    dl[i] = make_uint4(pl[4 * i], pl[4 * i + 1], pl[4 * i + 2], pl[4 * i + 3]);
+  for (int kk = 0; kk < BK / 16; ++kk) {
+    wgmma_ss<BN>(d, al, wh, (first && kk == 0) ? 0u : 1u);
+    wgmma_ss<BN>(d, ah, wl, 1u);
+    wgmma_ss<BN>(d, ah, wh, 1u);
+    ah += 2; al += 2; wh += 2; wl += 2;                // next 16-wide slice: +32 B (>> 4)
   }
 }
 
-// ---- warp-level transpose through shared memory so that global accesses are row-contiguous.
-// A thread owns one tile row (TMEM lane); a 32-column fp16 chunk of that row is 64 B = 4 x 16 B
-// slots.  Staging tile: 32 rows x 64 B, slot index XOR-swizzled with (row >> 1) & 3 (conflict-free
-// for both the row-owner pattern and the coalesced pattern: lane -> row i*8 + lane/4, slot lane%4).
-// The same image is what a SWIZZLE_64B tensor map with a 32 x 32 box reads / writes.
-__device__ __forceinline__ uint32_t stg_off(int row, int slot) {
-  return (uint32_t)(row * 64 + ((slot ^ ((row >> 1) & 3)) << 4));
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
-// registers (row-owner layout) -> global, 64-byte row segments written by 4 adjacent lanes
-__device__ __forceinline__ void store_plane_coalesced(uint8_t* stg, const uint32_t (&pk)[16], __half* gbase,
-                                                      int64_t ld, int rows_valid, int lane) {
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    *reinterpret_cast<uint4*>(stg + stg_off(lane, j)) = make_uint4(pk[4 * j], pk[4 * j + 1], pk[4 * j + 2], pk[4 * j + 3]);
-  __syncwarp();
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int rr = i * 8 + (lane >> 2), qq = lane & 3;
-    const uint4 val = *reinterpret_cast<const uint4*>(stg + stg_off(rr, qq));
-    if (rr < rows_valid) *reinterpret_cast<uint4*>(gbase + (int64_t)rr * ld + qq * 8) = val;
-  }
-  __syncwarp();
-}
-// fp32 x32 -> packed split16 words (hi and lo planes)
-__device__ __forceinline__ void pack_split(const float (&v)[32], uint32_t (&ph)[16], uint32_t (&pl)[16]) {
-#pragma unroll
-  for (int i = 0; i < 16; ++i) split2(v[2 * i], v[2 * i + 1], ph[i], pl[i]);
+__device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, float x0, float x1) {
+  uint32_t h, l;
+  split2(x0, x1, h, l);
+  *reinterpret_cast<uint32_t*>(hi + o) = h;
+  *reinterpret_cast<uint32_t*>(lo + o) = l;
 }
 
-__device__ __forceinline__ void ln_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(LN_WARPS * 32) : "memory"); }
-
-// x[i] = act(acc[i] * s + bias[i]) for one 32-column chunk; bias read as float4 broadcasts.
-template <int ACT>
-__device__ __forceinline__ void epi_chunk_fast(const uint32_t (&r)[32], float (&v)[32], const float* sb, float s) {
-  const float4* b4 = reinterpret_cast<const float4*>(sb);
+// y = LayerNorm(acc * sc + bias + residual) * gamma + beta over the 256-wide rows of a [64 x 256] accumulator
+// fragment, eps 1e-5.  r_lo: this thread's first row (the second is r_lo + 8), cp: its column offset inside an
+// 8-column group.  The statistics are two exact passes over the registers; a row's four lanes are merged with
+// shuffles in a fixed order, so the result does not depend on which CTA ran the tile.
+__device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const float* bias, const __half* res_hi,
+                                            const __half* res_lo, int ld_res, const float* gamma, const float* beta,
+                                            __half* out_hi, __half* out_lo, int ld_out, int r_lo, int M, int cp) {
+  const bool ok0 = r_lo < M, ok1 = r_lo + 8 < M;
+  float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 b = b4[i];
-    float x0 = fmaf(__uint_as_float(r[4 * i + 0]), s, b.x), x1 = fmaf(__uint_as_float(r[4 * i + 1]), s, b.y);
-    float x2 = fmaf(__uint_as_float(r[4 * i + 2]), s, b.z), x3 = fmaf(__uint_as_float(r[4 * i + 3]), s, b.w);
-    if (ACT == ACT_GELU) { gelu_fast2(x0, x1); gelu_fast2(x2, x3); }
-    if (ACT == ACT_RELU) { x0 = fmaxf(x0, 0.f); x1 = fmaxf(x1, 0.f); x2 = fmaxf(x2, 0.f); x3 = fmaxf(x3, 0.f); }
-    if (ACT == ACT_SILU) { x0 = silu_f(x0); x1 = silu_f(x1); x2 = silu_f(x2); x3 = silu_f(x3); }
-    v[4 * i + 0] = x0; v[4 * i + 1] = x1; v[4 * i + 2] = x2; v[4 * i + 3] = x3;
-  }
-}
-
-// y = (x * a + b) * gamma + beta for one parked 32-column chunk
-__device__ __forceinline__ void ln_norm_chunk(const uint32_t (&r)[32], float (&v)[32], const float* g, const float* be,
-                                              float a, float b) {
-  const float4* g4 = reinterpret_cast<const float4*>(g);
-  const float4* e4 = reinterpret_cast<const float4*>(be);
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    const float4 gg = g4[i], bb = e4[i];
-    v[4 * i + 0] = fmaf(fmaf(__uint_as_float(r[4 * i + 0]), a, b), gg.x, bb.x);
-    v[4 * i + 1] = fmaf(fmaf(__uint_as_float(r[4 * i + 1]), a, b), gg.y, bb.y);
-    v[4 * i + 2] = fmaf(fmaf(__uint_as_float(r[4 * i + 2]), a, b), gg.z, bb.z);
-    v[4 * i + 3] = fmaf(fmaf(__uint_as_float(r[4 * i + 3]), a, b), gg.w, bb.w);
-  }
-}
-// row-owner packed chunk -> SWIZZLE_64B staging pair -> two TMA bulk stores (lane 0 owns the warp's
-// bulk groups; at most PENDING older pairs still being read by the TMA engine: 1 = the caller alternates two
-// staging pairs, 0 = one pair)
-template <int PENDING = 1>
-__device__ __forceinline__ void stage_and_store(uint8_t* sb2, const uint32_t (&ph)[16], const uint32_t (&pl)[16], int lane,
-                                                const CUtensorMap* mh, const CUtensorMap* ml, int col, int row0) {
-  if constexpr (PENDING < 0) {
-    // ONE 4 KB tile used as two 2 KB halves with a bulk group per PLANE: the hi half is rewritten while the lo
-    // store of the previous chunk may still be reading its half (and vice versa).  With one group per chunk and
-    // wait_group.read 0 the warp waited for the TMA engine on every chunk (22 % of the QKV kernel's stall samples).
-    if (lane == 0) tma_store_wait_read<1>();
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(sb2 + stg_off(lane, j)) = make_uint4(ph[4 * j], ph[4 * j + 1], ph[4 * j + 2], ph[4 * j + 3]);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { tma_store_2d(mh, smem_u32(sb2), col, row0); tma_store_commit(); tma_store_wait_read<1>(); }
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      *reinterpret_cast<uint4*>(sb2 + 2048 + stg_off(lane, j)) = make_uint4(pl[4 * j], pl[4 * j + 1], pl[4 * j + 2], pl[4 * j + 3]);
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) { tma_store_2d(ml, smem_u32(sb2 + 2048), col, row0); tma_store_commit(); }
-    return;
-  }
-  if (lane == 0) tma_store_wait_read<PENDING < 0 ? 0 : PENDING>();
-  __syncwarp();
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    *reinterpret_cast<uint4*>(sb2 + stg_off(lane, j)) = make_uint4(ph[4 * j], ph[4 * j + 1], ph[4 * j + 2], ph[4 * j + 3]);
-    *reinterpret_cast<uint4*>(sb2 + 2048 + stg_off(lane, j)) = make_uint4(pl[4 * j], pl[4 * j + 1], pl[4 * j + 2], pl[4 * j + 3]);
-  }
-  fence_proxy_async_smem();
-  __syncwarp();
-  if (lane == 0) {
-    tma_store_2d(mh, smem_u32(sb2), col, row0);
-    tma_store_2d(ml, smem_u32(sb2 + 2048), col, row0);
-    tma_store_commit();
-  }
-}
-
-// ---- residual + LayerNorm of one 128 x 256 accumulator tile by SIXTEEN warps.  Warp -> TMEM lane quarter q
-// (32 rows, a thread owns one row) x column quarter cq (64 columns = two 32-column chunks).  Every thread
-// keeps one-pass statistics of its 64 values shifted by the mean of its first chunk (var = E[(x-K)^2] -
-// E[x-K]^2 does not cancel); the four quarters of a row are merged with the pairwise (Chan) update through
-// shared memory in a FIXED order, so every warp derives the same mean / rstd; the pre-norm values are parked
-// in TMEM between the passes.  The residual is loaded (coalesced pattern) before the accumulator is awaited.
-// The residual of one 32-column chunk (both planes, 2 x 2 KB) is pulled into the warp's staging tile by TMA - the
-// same SWIZZLE_64B 32 x 32 boxes the output leaves through - and read back row by row.  (As plain 16-byte loads
-// through a register transpose this was the LayerNorm epilogue's hot spot: 24 % of the out-projection kernel's stall
-// samples sat on the load instruction, most of them LG-throttle.)  One mbarrier per warp; `phase` is its parity.
-struct LnResidual { uint32_t bar; uint32_t phase; };
-// r[32] (fp32 bits) += one fp16 plane of the same 32 columns, read from this thread's row of a staging tile
-__device__ __forceinline__ void add_plane_stg(uint32_t (&r)[32], const uint8_t* stg, int lane) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const uint4 pv = *reinterpret_cast<const uint4*>(stg + stg_off(lane, i));
-    const uint32_t w[4] = {pv.x, pv.y, pv.z, pv.w};
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[j]));
-      const int e = i * 8 + j * 2;
-      r[e] = __float_as_uint(__uint_as_float(r[e]) + f.x);
-      r[e + 1] = __float_as_uint(__uint_as_float(r[e + 1]) + f.y);
-    }
-  }
-}
-// the staging tile must be idle: its TMA stores read (cp.async.bulk.wait_group.read 0 by lane 0) and this warp's
-// own reads of it done (program order + __syncwarp)
-__device__ __forceinline__ void ln16_issue_residual(const LnResidual& t, bool has_res, uint8_t* stg, const CUtensorMap* mRh,
-                                                    const CUtensorMap* mRl, int wrow0, int col, int lane) {
-  if (!has_res) return;
-  __syncwarp();
-  if (lane == 0) {
-    fence_proxy_async_smem();                        // generic-proxy reads / writes of the tile -> async-proxy writes
-    mbar_expect_tx(t.bar, 4096);
-    tma_load_2d(smem_u32(stg), mRh, t.bar, col, wrow0);          // rows >= M are zero-filled (and counted)
-    tma_load_2d(smem_u32(stg + 2048), mRl, t.bar, col, wrow0);
-  }
-}
-// trow: TMEM address of this thread's row at the tile's column cb = cq * 64.  stg: this warp's staging
-// (4 KB with WIDE_STG: both planes transposed at once and the TMA-store pair; else 2 KB).  s_vec*: bias / gamma /
-// beta of the 256 columns.  s_part: [4 quarters][mean | M2][128 rows].
-template <bool WIDE_STG>
-__device__ __forceinline__ void ln16_finish(LnResidual& t, bool has_res, const CUtensorMap* mRh, const CUtensorMap* mRl, uint32_t trow, int cq, int row, int lane, uint8_t* stg,
-                                            const float* s_bias, const float* s_gamma, const float* s_beta, float* s_part,
-                                            float sc, int wrow0, int rows_valid, bool tma_out, const CUtensorMap* mOh,
-                                            const CUtensorMap* mOl, __half* out_hi, __half* out_lo, int ld_out,
-                                            long long* tl, int& tl_n, const float* part0 = nullptr, int nparts = 0,
-                                            size_t part_stride = 0, bool defer_drain = false) {
-  const int cb = cq * 64;
-  uint32_t r[32];
-  float v[32];
-  float s1 = 0.0f, s2 = 0.0f, shiftK = 0.0f;
-#pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    tmem_ld32(trow + c * 32, r);
-    // partial accumulators of the same tile computed by other clusters (k_ffn_tc's hidden-dimension split),
-    // added in a fixed order
-    for (int pp = 0; pp < nparts; ++pp) {
-      const float4* src = reinterpret_cast<const float4*>(part0 + (size_t)pp * part_stride) + ((cq * 16 + c * 8) * 128 + row);
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float4 a[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) a[i] = __ldcg(src + (hh * 4 + i) * 128);
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int e = (hh * 4 + i) * 4;
-          r[e + 0] = __float_as_uint(__uint_as_float(r[e + 0]) + a[i].x);
-          r[e + 1] = __float_as_uint(__uint_as_float(r[e + 1]) + a[i].y);
-          r[e + 2] = __float_as_uint(__uint_as_float(r[e + 2]) + a[i].z);
-          r[e + 3] = __float_as_uint(__uint_as_float(r[e + 3]) + a[i].w);
-        }
+  for (int j = 0; j < 32; ++j) {
+    const int n = 8 * j + cp;
+    const float2 b = bias ? __ldg(reinterpret_cast<const float2*>(bias + n)) : make_float2(0.0f, 0.0f);
+    float x0 = fmaf(d[4 * j], sc, b.x), x1 = fmaf(d[4 * j + 1], sc, b.y);
+    float x2 = fmaf(d[4 * j + 2], sc, b.x), x3 = fmaf(d[4 * j + 3], sc, b.y);
+    if (res_hi) {
+      if (ok0) {
+        const int64_t o = (int64_t)r_lo * ld_res + n;
+        const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
+        const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
+        x0 = (x0 + h.x) + l.x; x1 = (x1 + h.y) + l.y;
+      }
+      if (ok1) {
+        const int64_t o = (int64_t)(r_lo + 8) * ld_res + n;
+        const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
+        const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
+        x2 = (x2 + h.x) + l.x; x3 = (x3 + h.y) + l.y;
       }
     }
-    // x = acc * sc + bias, then + residual hi plane, then + lo plane (one plane at a time: the row-owner copy
-    // of a plane is 16 registers, and 112 per thread is all there is with 576 threads)
-    const float4* b4 = reinterpret_cast<const float4*>(s_bias + cb + c * 32);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 b = b4[i];
-      r[4 * i + 0] = __float_as_uint(fmaf(__uint_as_float(r[4 * i + 0]), sc, b.x));
-      r[4 * i + 1] = __float_as_uint(fmaf(__uint_as_float(r[4 * i + 1]), sc, b.y));
-      r[4 * i + 2] = __float_as_uint(fmaf(__uint_as_float(r[4 * i + 2]), sc, b.z));
-      r[4 * i + 3] = __float_as_uint(fmaf(__uint_as_float(r[4 * i + 3]), sc, b.w));
-    }
-    if (has_res) {
-      // the first chunk was requested before (GEMM) / right after (fused FFN) the accumulator wait; the second one
-      // is requested as soon as the first has been read out of the tile and arrives under the first chunk's statistics
-      mbar_wait(t.bar, t.phase);
-      t.phase ^= 1u;
-      add_plane_stg(r, stg, lane);
-      add_plane_stg(r, stg + 2048, lane);
-      if (c == 0) ln16_issue_residual(t, true, stg, mRh, mRl, wrow0, cb + 32, lane);
-    }
-    if (c == 0) {                                  // shift: the mean of the first chunk
-      float acc = 0.0f;
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc += __uint_as_float(r[i]);
-      shiftK = acc * (1.0f / 32);
-    }
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const float d0 = __uint_as_float(r[i]) - shiftK, d1 = __uint_as_float(r[i + 1]) - shiftK;
-      s1 += d0 + d1;
-      s2 = fmaf(d0, d0, fmaf(d1, d1, s2));
-    }
-    tmem_st32(trow + c * 32, r);
+    d[4 * j] = x0; d[4 * j + 1] = x1; d[4 * j + 2] = x2; d[4 * j + 3] = x3;
+    s0 += x0 + x1; s1 += x2 + x3;
   }
-  tl_event(tl, tl_n, 7);                            // LayerNorm: statistics pass done
-  // this quarter: mean_q = K + s1/64, M2_q = s2 - s1^2/64
-  s_part[cq * 256 + row] = shiftK + s1 * (1.0f / 64);
-  s_part[cq * 256 + 128 + row] = fmaxf(s2 - s1 * s1 * (1.0f / 64), 0.0f);
-  ln_bar_sync();
-  tl_event(tl, tl_n, 17);                           // LayerNorm: quarters merged
-  const float m0 = s_part[row], m1 = s_part[256 + row], m2 = s_part[512 + row], m3 = s_part[768 + row];
-  const float mean = 0.25f * ((m0 + m1) + (m2 + m3));
-  const float d0 = m0 - mean, d1 = m1 - mean, d2 = m2 - mean, d3 = m3 - mean;
-  const float M2 = ((s_part[128 + row] + s_part[384 + row]) + (s_part[640 + row] + s_part[896 + row])) +
-                   64.0f * ((d0 * d0 + d1 * d1) + (d2 * d2 + d3 * d3));
-  const float rstd = rsqrtf(M2 * (1.0f / 256) + 1e-5f);
-  const float nb_ = -mean * rstd;                    // y = x * rstd + nb_
-#pragma unroll 1
-  for (int c = 0; c < 2; ++c) {
-    tmem_ld32(trow + c * 32, r);
-    ln_norm_chunk(r, v, s_gamma + cb + c * 32, s_beta + cb + c * 32, rstd, nb_);
-    uint32_t ph[16], pl[16];
-    pack_split(v, ph, pl);
-    if (WIDE_STG && tma_out) {
-      stage_and_store<-1>(stg, ph, pl, lane, mOh, mOl, cb + c * 32, wrow0);
-    } else {
-      const int64_t o = (int64_t)wrow0 * ld_out + cb + c * 32;
-      store_plane_coalesced(stg, ph, out_hi + o, ld_out, rows_valid, lane);
-      store_plane_coalesced(stg, pl, out_lo + o, ld_out, rows_valid, lane);
-    }
+  const float mean0 = quad_sum(s0) * (1.0f / 256), mean1 = quad_sum(s1) * (1.0f / 256);
+  float q0 = 0.0f, q1 = 0.0f;
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float a0 = d[4 * j] - mean0, a1 = d[4 * j + 1] - mean0, a2 = d[4 * j + 2] - mean1, a3 = d[4 * j + 3] - mean1;
+    q0 = fmaf(a0, a0, fmaf(a1, a1, q0));
+    q1 = fmaf(a2, a2, fmaf(a3, a3, q1));
   }
-  // the staging is the next tile's transpose buffer and s_part its statistics: the TMA engine must have read
-  // the former, every warp the latter
-  tl_event(tl, tl_n, 18);                           // LayerNorm: normalised, stores issued
-  if (defer_drain) return;                          // the caller drains (ln16_drain) before the staging is touched again
-  if (WIDE_STG && tma_out && lane == 0) tma_store_wait_read<0>();
-  ln_bar_sync();
-}
-// the drain ln16_finish leaves to the caller with defer_drain: every warp's TMA stores have read their staging tile
-// and every warp is past its partial statistics
-__device__ __forceinline__ void ln16_drain(int lane) {
-  if (lane == 0) tma_store_wait_read<0>();
-  ln_bar_sync();
-}
-
-// j-th work item of this CTA: CTA pairs (CG = 2) walk (m-pair, n) items in lockstep - CTA rank r of
-// a pair owns m-tile mp*2 + r and half of the W tile.
-__device__ __forceinline__ void decode_item(int j, const TcParams& p, int bn, int cg, int rank, int& m0, int& n0) {
-  const int t = (int)blockIdx.x / cg + j * ((int)gridDim.x / cg);
-  m0 = ((t / p.n_tiles) * cg + rank) * BM;
-  n0 = (t % p.n_tiles) * bn;
+  const float rstd0 = rsqrtf(quad_sum(q0) * (1.0f / 256) + 1e-5f), rstd1 = rsqrtf(quad_sum(q1) * (1.0f / 256) + 1e-5f);
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const int n = 8 * j + cp;
+    const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + n)), be = __ldg(reinterpret_cast<const float2*>(beta + n));
+    if (ok0)
+      store_split2(out_hi, out_lo, (int64_t)r_lo * ld_out + n, fmaf((d[4 * j] - mean0) * rstd0, g.x, be.x),
+                   fmaf((d[4 * j + 1] - mean0) * rstd0, g.y, be.y));
+    if (ok1)
+      store_split2(out_hi, out_lo, (int64_t)(r_lo + 8) * ld_out + n, fmaf((d[4 * j + 2] - mean1) * rstd1, g.x, be.x),
+                   fmaf((d[4 * j + 3] - mean1) * rstd1, g.y, be.y));
+  }
 }
 
 // ------------------------------------------------------------------------------ the kernel
-// Persistent: CTA (pair) c walks items c, c + #CTAs (pairs), ...; item t -> (m = t / n_tiles, n = t % n_tiles).
-// The accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i overlaps
-// the TMA/MMA main loop of tile i + 1.
-// EPI selects the epilogue: EPI_FAST = plain, split16 output, identity row mapping, every 32-column chunk
-// inside N (the per-layer GEMMs); EPI_LN = residual + LayerNorm; EPI_GENERIC = plain with everything else
-// (positional table, row remapping, zeroed padding rows, fp32 output, ragged N: the per-batch embedding /
-// final-layer GEMMs) kept out of the hot kernels' instruction stream.
-template <int BN, int CG, int EPI, int ACT = ACT_NONE>      // ACT: the fast epilogue's activation (NONE | GELU)
-__global__ void __launch_bounds__(EPI == EPI_LN ? LN_THREADS : NUM_THREADS, 1)
+// Persistent: CTA c walks tiles c, c + #CTAs, ...; tile t -> (m = t / n_tiles, n = t % n_tiles).
+// EPI selects the epilogue: EPI_FAST = plain, split16 output, identity row mapping, N a whole number of tiles
+// (the per-layer GEMMs); EPI_LN = residual + LayerNorm; EPI_GENERIC = plain with everything else (positional
+// table, row remapping, zeroed padding rows, fp32 output, ragged N: the per-batch embedding / final-layer
+// GEMMs) kept out of the hot kernels' instruction stream.
+template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast epilogue's activation (NONE | GELU)
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
           const __grid_constant__ CUtensorMap tmA2h, const __grid_constant__ CUtensorMap tmA2l,
-          const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl,
-          const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl,
-          const __grid_constant__ CUtensorMap tmRh, const __grid_constant__ CUtensorMap tmRl,   // residual (EPI_LN)
-          const TcParams p) {
-  constexpr bool LN = EPI == EPI_LN;
-  static_assert(!LN || BN == 256, "the LayerNorm epilogue covers a full 256-wide row");
-  using Cfg = TileCfg<BN, CG, EPI>;
+          const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const TcParams p) {
+  static_assert(EPI != EPI_LN || BN == 256, "the LayerNorm epilogue covers a full 256-wide row");
+  using Cfg = TileCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
-  constexpr bool DEEP = Cfg::DEEP;
-  constexpr int NEPI = Cfg::NEPI;                             // epilogue warps (16 with LayerNorm)
-  constexpr int EMPTY_ARRIVALS = NEPI * CG;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-B alignment by pointer arithmetic (an integer round trip would lose the shared address space
-  // and turn every staging access into a generic LD/ST)
+  // 1024-B alignment by pointer arithmetic (an integer round trip would lose the shared address space)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* aux = smem + STAGES * Cfg::STAGE_BYTES;
-  float* s_bias = reinterpret_cast<float*>(aux);              // [MAX_N]   (none of the three when DEEP)
-  float* s_gamma = s_bias + (DEEP ? 0 : MAX_N);               // [256]
-  float* s_beta = s_gamma + (DEEP ? 0 : 256);                 // [256]
-  float* s_part = s_beta + (DEEP ? 0 : 256);                  // LayerNorm partial statistics (EPI_LN only)
-  uint8_t* s_stage = reinterpret_cast<uint8_t*>(s_part) + Cfg::PART_BYTES;   // [NEPI][STG_WARP], 16B aligned
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + Cfg::STG_BYTES);
-  uint64_t* bar_full = bars;                    // [STAGES]
-  uint64_t* bar_empty = bars + STAGES;          // [STAGES]
-  uint64_t* bar_tfull = bars + 2 * STAGES;      // [2]
-  uint64_t* bar_tempty = bars + 2 * STAGES + 2; // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  uint64_t* bar_res = bars + 12;                // [LN_WARPS] residual tile landed (one per LayerNorm warp)
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);   // [STAGES] TMA tx
+  uint64_t* bar_empty = bar_full + STAGES;                                              // [STAGES] one arrival per consumer warp
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
   int tl_n = 0;                                     // debug-timeline event counter of this warp
   tl_event(p.tl, tl_n, 40);                       // kernel entry
-  const int rank = CG > 1 ? (int)cluster_ctarank() : 0;
-  const int ncl = (int)gridDim.x / CG, cid = (int)blockIdx.x / CG;          // clusters, this CTA's cluster
-  const int ngroups = ((p.m_tiles + CG - 1) / CG) * p.n_tiles;               // (m-group, n) items
-  const int nlocal = (ngroups - cid + ncl - 1) / ncl;
+  const int ntiles = p.m_tiles * p.n_tiles;
+  const int nlocal = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  auto decode = [&](int j, int& m0, int& n0) {
+    const int t = (int)blockIdx.x + j * (int)gridDim.x;
+    m0 = (t / p.n_tiles) * BM;
+    n0 = (t % p.n_tiles) * BN;
+  };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&bar_tfull[s]), 1);
-      mbar_init(smem_u32(&bar_tempty[s]), EMPTY_ARRIVALS);    // 2-SM: the leader's barrier collects both CTAs' warps
-    }
-    if (LN)
-      for (int s = 0; s < LN_WARPS; ++s) mbar_init(smem_u32(&bar_res[s]), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmA1h); tma_prefetch_desc(&tmA1l); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
   }
-  if (CG > 1) { __syncthreads(); cluster_sync_all(); }   // 2-SM TMEM allocation needs both CTAs of the pair resident
-  if (warp == 1) tmem_alloc<CG>(smem_u32(tmem_slot), Cfg::TMEM_COLS);
-  if (warp >= 2 && !DEEP) {
-    for (int i = threadIdx.x - 64; i < MAX_N; i += NEPI * 32) s_bias[i] = (p.bias && i < p.N) ? p.bias[i] : 0.0f;
-    if (LN)
-      for (int i = threadIdx.x - 64; i < 256; i += NEPI * 32) { s_gamma[i] = p.gamma[i]; s_beta[i] = p.beta[i]; }
-  }
   pdl_trigger();               // let the next kernel's prologue overlap our tail
-  tc_fence_before();
   __syncthreads();
-  if (CG > 1) cluster_sync_all();   // the peer's barriers are initialised before anyone signals them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();                  // everything below touches activations of the previous kernel
   tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
 
-  if (warp == 0) {
+  if (warp < 4) {
+    reg_dec<40>();
+    if (warp != 0) return;
     // ---------------------------------------------------------------- TMA producer
-    // The whole warp walks the loop (uniform control flow), one elected lane issues: ptxas then keeps
-    // the TMA / MMA operands in uniform registers instead of wrapping every instruction in an ELECT loop.
+    // The whole warp walks the loop (uniform control flow), one elected lane issues.
     int kbg = 0;                                   // k-block counter across tiles (ring position)
     for (int j = 0; j < nlocal; ++j) {
       int m0, n0;
-      decode_item(j, p, BN, CG, rank, m0, n0);
+      decode(j, m0, n0);
       tl_event(p.tl, tl_n, 1, j);                                    // producer: tile j begins
       for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
         const int s = kbg % STAGES;
-        const uint32_t ph = (uint32_t)(kbg / STAGES) & 1u;
-        mbar_wait(smem_u32(&bar_empty[s]), ph ^ 1u);
+        mbar_wait(smem_u32(&bar_empty[s]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
         if (elect_one()) {
           if (kb == 0 && j + 1 < nlocal) {
-            // The ring is only two or three k-blocks deep (64 KB stages): measured with the in-kernel timeline,
-            // a k-block took 2.1-2.6k cycles to arrive against 1.57k cycles of MMA work, i.e. the main loop ran
-            // at the HBM latency.  The NEXT item's activation rows are therefore pulled into L2 one whole item
-            // ahead (weights are L2-resident anyway).
+            // the ring is only two or three k-blocks deep: the NEXT tile's activation rows are pulled into L2
+            // one whole tile ahead (weights are L2-resident anyway)
             int m1, n1;
-            decode_item(j + 1, p, BN, CG, rank, m1, n1);
+            decode(j + 1, m1, n1);
             if (m1 != m0) {
               for (int k2 = 0; k2 < p.kblocks; ++k2) {
                 if (k2 < p.kb1) { tma_prefetch_2d(&tmA1h, k2 * BK, m1); tma_prefetch_2d(&tmA1l, k2 * BK, m1); }
@@ -480,619 +222,367 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
               }
             }
           }
-          uint32_t full = smem_u32(&bar_full[s]);
-          if (CG == 1) {
-            mbar_expect_tx(full, Cfg::STAGE_BYTES);
-          } else {                                   // both CTAs' boxes are counted on the leader's barrier
-            if (rank == 0) mbar_expect_tx(full, 2 * Cfg::STAGE_BYTES);
-            full = mapa_u32(full, 0);
-          }
+          const uint32_t full = smem_u32(&bar_full[s]);
+          mbar_expect_tx(full, Cfg::STAGE_BYTES);
           const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
           const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-          if (CG == 1) {
-            if (kb < p.kb1) {
-              tma_load_2d(sAh, &tmA1h, full, kb * BK, m0);
-              tma_load_2d(sAl, &tmA1l, full, kb * BK, m0);
-            } else {
-              tma_load_2d(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
-              tma_load_2d(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
-            }
-            tma_load_2d(sWh, &tmWh, full, kb * BK, n0);
-            tma_load_2d(sWl, &tmWl, full, kb * BK, n0);
+          if (kb < p.kb1) {
+            tma_load_2d(sAh, &tmA1h, full, kb * BK, m0);
+            tma_load_2d(sAl, &tmA1l, full, kb * BK, m0);
           } else {
-            // this CTA's own 128 rows of A and rows [rank*BN/2, (rank+1)*BN/2) of the W tile
-            if (kb < p.kb1) {
-              tma_load_2d_2sm(sAh, &tmA1h, full, kb * BK, m0);
-              tma_load_2d_2sm(sAl, &tmA1l, full, kb * BK, m0);
-            } else {
-              tma_load_2d_2sm(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
-              tma_load_2d_2sm(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
-            }
-            tma_load_2d_2sm(sWh, &tmWh, full, kb * BK, n0 + rank * (BN / 2));
-            tma_load_2d_2sm(sWl, &tmWl, full, kb * BK, n0 + rank * (BN / 2));
+            tma_load_2d(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
+            tma_load_2d(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
           }
+          tma_load_2d(sWh, &tmWh, full, kb * BK, n0);       // rows >= N are zero-filled (and counted)
+          tma_load_2d(sWl, &tmWl, full, kb * BK, n0);
         }
         __syncwarp();
       }
     }
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // ---------------------------------------------------------------- MMA issuer (2-SM: the leader CTA)
-      constexpr uint32_t idesc = make_idesc(BN, BM * CG);
-      int kbg = 0;
-      for (int it = 0; it < nlocal; ++it) {
-        const int as = it & 1;
-        if (CG == 1) mbar_wait(smem_u32(&bar_tempty[as]), (((uint32_t)it >> 1) & 1u) ^ 1u);   // epilogue drained it
-        else mbar_wait_cluster(smem_u32(&bar_tempty[as]), (((uint32_t)it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        tl_event(p.tl, tl_n, 2, it);                                   // MMA: accumulator stage free, tile `it` begins
-        const uint32_t tacc = tmem_base + (uint32_t)(as * BN);
-        const int nkb = p.kblocks;
-        for (int kb = 0; kb < nkb; ++kb, ++kbg) {
-          const int s = kbg % STAGES;
-          const uint32_t ph = (uint32_t)(kbg / STAGES) & 1u;
-          mbar_wait(smem_u32(&bar_full[s]), ph);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-            const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-            // descriptors of the k-block's first 16-wide slice; +2 (32 B >> 4) per further slice
-            uint64_t ah = make_desc(sAh), al = make_desc(sAl), wh = make_desc(sWh), wl = make_desc(sWl);
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk) {
-              if (CG == 1) {
-                umma(tacc, al, wh, idesc, (kb | kk) != 0 ? 1u : 0u);
-                umma(tacc, ah, wl, idesc, 1u);
-                umma(tacc, ah, wh, idesc, 1u);
-              } else {
-                umma_2sm(tacc, al, wh, idesc, (kb | kk) != 0 ? 1u : 0u);
-                umma_2sm(tacc, ah, wl, idesc, 1u);
-                umma_2sm(tacc, ah, wh, idesc, 1u);
-              }
-              ah += 2; al += 2; wh += 2; wl += 2;
-            }
-            if (CG == 1) umma_commit(smem_u32(&bar_empty[s]));      // frees the stage when these MMAs retire
-            else umma_commit_2sm(smem_u32(&bar_empty[s]));          // ... in both CTAs of the pair
-            if (kb == nkb - 1) {                                    // accumulator complete
-              if (CG == 1) umma_commit(smem_u32(&bar_tfull[as]));
-              else umma_commit_2sm(smem_u32(&bar_tfull[as]));
-            }
-          }
-          __syncwarp();
-        }
-        tl_event(p.tl, tl_n, 3, it);                                   // MMA: tile `it` issued
-      }
-    }
-  } else if constexpr (!LN) {
-    // ------------------------------------------------------------------ plain epilogues (warps 2..9)
-    const int q = warp & 3;                          // TMEM lane quarter this warp may access
-    const int hf = (warp - 2) >> 2;                  // which half of the tile's columns
-    const int row = q * 32 + lane;
-    constexpr int CH = BN / 64;                      // 32-column chunks per warp
-    uint32_t r[32];
-    float v[32];
-    int tbuf = 0;                                    // staging pair for the next TMA store
-    uint8_t* const stg = s_stage + (warp - 2) * Cfg::STG_WARP;
-    for (int it = 0; it < nlocal; ++it) {
-      const int as = it & 1;
-      int m0, n0;
-      decode_item(it, p, BN, CG, rank, m0, n0);
-      const int m = m0 + row;
-      const bool row_ok = m < p.M;
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + hf * (BN / 2));
-      const int wrow0 = m0 + q * 32;                 // first output row owned by this warp
-      const int rows_valid = min(32, p.M - wrow0);   // <= 0: nothing to write
-      mbar_wait(smem_u32(&bar_tfull[as]), ((uint32_t)it >> 1) & 1u);
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 4, it);                                     // epilogue: accumulator of tile `it` ready
-      int seq = 0, pos = m;
-      if (row_ok && p.in_group < p.M) { seq = m / p.in_group; pos = m - seq * p.in_group; }
-      const int64_t orow = (int64_t)seq * p.out_group + p.out_off + pos;
-      const bool zero = row_ok && p.zero_lengths != nullptr && pos >= p.zero_lengths[seq];
-      const float* tab = p.addtab ? p.addtab + (int64_t)(p.out_off + pos) * p.N : nullptr;
-      const float inv_scale = p.inv_scale;
-      const int act = p.act, N = p.N;
-      __half* const ohi = p.out_hi;
-      __half* const olo = p.out_lo;
-      const int64_t obase = orow * p.ld_out + p.out_col0;
-      float4 bb[8];                                  // DEEP: this chunk's bias values
-      // one 32-column chunk: accumulator registers -> bias / activation -> split16 -> global
-      auto chunk = [&](const uint32_t (&r)[32], int c) {
-        const int nb = n0 + hf * (BN / 2) + c * 32;
-        if constexpr (EPI == EPI_FAST) {
-          epi_chunk_fast<ACT>(r, v, DEEP ? reinterpret_cast<const float*>(bb) : s_bias + nb, inv_scale);
-          uint32_t ph[16], pl[16];
-          pack_split(v, ph, pl);
-          if (CG == 2 && p.tma_out) {
-            stage_and_store<DEEP ? -1 : 1>(stg + tbuf * 4096, ph, pl, lane, &tmOh, &tmOl, nb, wrow0);   // the map clips rows >= M
-            if (!DEEP) tbuf ^= 1;
-          } else {
-            const int64_t o = (int64_t)wrow0 * p.ld_out + p.out_col0 + nb;
-            store_plane_coalesced(stg, ph, ohi + o, p.ld_out, rows_valid, lane);
-            store_plane_coalesced(stg, pl, olo + o, p.ld_out, rows_valid, lane);
-          }
-        } else if (row_ok && nb < N) {
-          const bool full = nb + 32 <= N;
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            float x = __uint_as_float(r[i]) * inv_scale + s_bias[min(nb + i, MAX_N - 1)];
-            if (tab && (full || nb + i < N)) x += tab[nb + i];
-            x = apply_act(x, act);
-            v[i] = zero ? 0.0f : x;
-          }
-          if (ohi) {
-            const int64_t o = obase + nb;
-            if (full) {
-              store_split_chunk(v, ohi + o, olo + o);
-            } else {
-#pragma unroll
-              for (int i = 0; i < 32; ++i) {
-                if (nb + i < N) {
-                  __half h, l;
-                  split_f32(v[i], h, l);
-                  ohi[o + i] = h; olo[o + i] = l;
-                }
-              }
-            }
-          }
-          if (p.out_f32) {
-            float* dst = p.out_f32 + orow * p.ldc + nb;
-#pragma unroll
-            for (int i = 0; i < 32; ++i)
-              if (full || nb + i < N) dst[i] = v[i];
-          }
-        }
-        __syncwarp();
-      };
-#pragma unroll 1
-      for (int c = 0; c < CH; ++c) {
-        if (EPI == EPI_FAST && DEEP) {               // the chunk's bias (global, L1-resident) rides under the TMEM load:
-          const float4* b4 = reinterpret_cast<const float4*>(p.bias + n0 + hf * (BN / 2) + c * 32);   // read on first use it
-#pragma unroll
-          for (int i = 0; i < 8; ++i) bb[i] = __ldg(b4 + i);                                          // was 10 % of the stalls
-        }
-        tmem_ld32(trow + c * 32, r);               // warp-collective: no divergence around it
-        chunk(r, c);
-      }
-      // this warp is done reading the accumulator stage: hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      tl_event(p.tl, tl_n, 5, it);                                     // epilogue: tile `it` drained
-      if (lane == 0) { if (CG == 1) mbar_arrive(smem_u32(&bar_tempty[as])); else mbar_arrive_cluster(mapa_u32(smem_u32(&bar_tempty[as]), 0)); }
-    }
-    if (CG == 2 && lane == 0) tma_store_wait_read<0>();   // staging fully read by the TMA engine
-  } else {
-    // ------------------------------------------------------------------ LayerNorm epilogue (warps 2..9)
-    // y = LayerNorm(acc * s + bias + residual) over the 256-wide row, eps 1e-5: all sixteen warps drain one
-    // accumulator stage together (ln16_finish), the MMA warp fills the other one meanwhile.
-    const int q = warp & 3;                          // TMEM lane quarter
-    const int cq = (warp - 2) >> 2;                  // column quarter of the row
-    const int row = q * 32 + lane;
-    uint8_t* const stg = s_stage + (warp - 2) * Cfg::STG_WARP;
-    const bool has_res = p.res_hi != nullptr;        // warp-uniform
-    LnResidual t{smem_u32(&bar_res[warp - 2]), 0u};
-    for (int it = 0; it < nlocal; ++it) {
-      const int as = it & 1;
-      int m0, n0;
-      decode_item(it, p, BN, CG, rank, m0, n0);
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(as * BN + cq * 64);
-      const int wrow0 = m0 + q * 32;
-      const int rows_valid = min(32, p.M - wrow0);
-      ln16_issue_residual(t, has_res, stg, &tmRh, &tmRl, wrow0, cq * 64, lane);
-      tl_event(p.tl, tl_n, 6, it);                                     // LN epilogue: residual loads issued, waiting for tile `it`
-      mbar_wait(smem_u32(&bar_tfull[as]), ((uint32_t)it >> 1) & 1u);
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 4, it);
-      ln16_finish<CG == 2>(t, has_res, &tmRh, &tmRl, trow, cq, row, lane, stg, s_bias, s_gamma, s_beta, s_part, p.inv_scale, wrow0,
-                           rows_valid, CG == 2 && p.tma_out, &tmOh, &tmOl, p.out_hi, p.out_lo, p.ld_out, p.tl, tl_n);
-      tc_fence_before();
-      __syncwarp();
-      tl_event(p.tl, tl_n, 5, it);
-      if (lane == 0) { if (CG == 1) mbar_arrive(smem_u32(&bar_tempty[as])); else mbar_arrive_cluster(mapa_u32(smem_u32(&bar_tempty[as]), 0)); }
-    }
-    if (CG == 2 && lane == 0) tma_store_wait_read<0>();
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (CG > 1) cluster_sync_all();   // nobody exits while the peer may still signal its barriers / read its smem
+  // ------------------------------------------------------------------ consumer warpgroups
+  reg_inc<232>();
+  const int cw = (warp >> 2) - 1;                    // which 64 rows of the tile
+  const int cp = 2 * (lane & 3);                     // column offset inside an 8-column group
+  float d[BN / 2];
+  int kbg = 0;
+  for (int it = 0; it < nlocal; ++it) {
+    int m0, n0;
+    decode(it, m0, n0);
+    tl_event(p.tl, tl_n, 2, it);                                     // MMA: tile `it` begins
+    for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
+      const int s = kbg % STAGES;
+      mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
+      const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128), sAl = sAh + Cfg::A_BYTES;
+      const uint32_t sWh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
+      wg_fence();
+      kblock_ss<BN>(d, sAh, sAl, sWh, sWl, kb == 0);
+      wg_commit();
+      if (kb > 0) {                                  // the previous k-block's MMAs have retired: free its stage
+        wg_wait<1>();
+        if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+      }
+    }
+    wg_wait<0>();
+    acc_fence(d);
+    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+    tl_event(p.tl, tl_n, 4, it);                                     // epilogue: accumulator of tile `it` ready
+
+    const int r_lo = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
+    if constexpr (EPI == EPI_LN) {
+      ln_epilogue(d, p.inv_scale, p.bias, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
+                  r_lo, p.M, cp);
+    } else if constexpr (EPI == EPI_FAST) {
+      const float sc = p.inv_scale;
+      const bool ok0 = r_lo < p.M, ok1 = r_lo + 8 < p.M;
+      const int64_t o0 = (int64_t)r_lo * p.ld_out + p.out_col0 + n0 + cp, o1 = o0 + (int64_t)8 * p.ld_out;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp));
+        float x0 = fmaf(d[4 * j], sc, b.x), x1 = fmaf(d[4 * j + 1], sc, b.y);
+        float x2 = fmaf(d[4 * j + 2], sc, b.x), x3 = fmaf(d[4 * j + 3], sc, b.y);
+        if (ACT == ACT_GELU) { x0 = gelu_fast(x0); x1 = gelu_fast(x1); x2 = gelu_fast(x2); x3 = gelu_fast(x3); }
+        if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x0, x1);
+        if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x2, x3);
+      }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m = r_lo + 8 * h;
+        if (m >= p.M) continue;
+        int seq = 0, pos = m;
+        if (p.in_group < p.M) { seq = m / p.in_group; pos = m - seq * p.in_group; }
+        const int64_t orow = (int64_t)seq * p.out_group + p.out_off + pos;
+        const bool zero = p.zero_lengths != nullptr && pos >= p.zero_lengths[seq];
+        const float* tab = p.addtab ? p.addtab + (int64_t)(p.out_off + pos) * p.N : nullptr;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = n0 + 8 * j + cp + e;
+            if (n >= p.N) continue;
+            float x = d[4 * j + 2 * h + e] * p.inv_scale + (p.bias ? p.bias[n] : 0.0f);
+            if (tab) x += tab[n];
+            x = zero ? 0.0f : apply_act(x, p.act);
+            if (p.out_hi) {
+              __half hh, ll;
+              split_f32(x, hh, ll);
+              const int64_t o = orow * p.ld_out + p.out_col0 + n;
+              p.out_hi[o] = hh; p.out_lo[o] = ll;
+            }
+            if (p.out_f32) p.out_f32[orow * p.ldc + n] = x;
+          }
+        }
+      }
+    }
+    tl_event(p.tl, tl_n, 5, it);                                     // epilogue: tile `it` stored
+  }
   tl_event(p.tl, tl_n, 42);                       // kernel exit
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<CG>(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 // ------------------------------------------------------------------------------ fused FFN
 // y = LayerNorm(res + W2 gelu(W1 x + b1) + b2) for d = 256 as ONE persistent launch in which the
-// hidden activations never leave the SM (the unfused pair writes and re-reads 2 x 4 x ff bytes per
-// row through HBM, which is what bounds it).  A CTA owns 128-row m-tiles; per tile it walks the
-// hidden dimension in 128-column chunks:
-//   F1(c): acc1[c&1] (TMEM, 128 cols)  = x[128 x 256] . W1[c*128.., :]^T        (4 k-blocks)
-//   E1(c): acc1 -> *s1 + b1 -> GELU -> split16 -> Hs (shared memory, UMMA K-major SWIZZLE_128B)
-//   F2(c): acc2 (TMEM, 256 cols)      += Hs[128 x 128] . W2[:, c*128..]^T        (2 k-blocks)
-// and finishes with the residual + LayerNorm epilogue on acc2.  The MMA warp issues
-// F1(0) F1(1) F2(0) F1(2) F2(1) ... so E1(c) runs under F1(c+1); the TMA warp streams the x / W1 /
-// W2 k-blocks through one ring (2 x 64 KB; 3 x 48 KB per CTA of a pair) in exactly that order.
+// hidden activations never leave the register file (the unfused pair writes and re-reads 2 x 4 x ff
+// bytes per row through HBM, which is what bounds it).  A CTA owns 128-row m-tiles, 64 rows per
+// consumer warpgroup; the x tile (both planes, 128 KB) stays in shared memory while the warpgroup
+// walks the hidden dimension in 64-column chunks:
+//   F1(c): acc1[64 x 64]   = x[64 x 256] . W1[c*64.., :]^T                (4 k-blocks, operands in shared memory)
+//   E1(c): acc1 -> *s1 + b1 -> GELU -> split16 A fragments (the accumulator layout of 16 columns IS the
+//          register-operand layout of a 16-deep k-step, so the hidden chunk never touches shared memory)
+//   F2(c): acc2[64 x 256] += H[64 x 64] . W2[:, c*64..]^T                  (A from registers)
+// and finishes with the residual + LayerNorm epilogue on acc2.  The TMA warp streams W1 / W2 through a ring of
+// three 32 KB slots, four per chunk: W1 k-blocks 0-1, W1 k-blocks 2-3, W2 hi plane, W2 lo plane.  F2(c)'s last
+// group stays in flight under F1(c + 1); the other warpgroup's MMAs cover this one's GELU.
 struct FfnParams {
   int M, m_tiles, n_chunks;
-  // Work decomposition (see k_ffn_tc): every cluster runs `full` whole m-tile groups; the `left` groups that do
-  // not fill another round are cut along the hidden dimension into `parts` pieces, one per cluster.
+  // Work decomposition (see k_ffn_tc): every CTA runs `full` whole m-tiles; the `left` tiles that do
+  // not fill another round are cut along the hidden dimension into `parts` pieces, one per CTA.
   int full, left, parts;
-  float* scratch;              // [slot][64 column groups][128 rows][4] fp32 partial accumulators of the pieces
+  float* scratch;              // [slot][128 rows][256] fp32 partial accumulators of the pieces
   int* flags;                  // [slot] 1 = partial written (reset by the reader)
-  int reverse;                 // walk the tile groups from the last one down (snake order, see tc_attention)
+  int reverse;                 // walk the tiles from the last one down (snake order, see tc_attention)
   long long* tl;
   float inv_s1, inv_s2;
   const float* b1; const float* b2; const float* gamma; const float* beta;
   const __half* res_hi; const __half* res_lo; int ld_res;
   __half* out_hi; __half* out_lo; int ld_out;
-  int tma_out;
 };
-template <int CG>
 struct FfnCfg {
-  static constexpr int CHUNK = 128;                      // hidden columns per chunk
-  // ring slot, per CTA.  F1 k-block: xh | xl (16 KB each) | w1h | w1l (128/CG rows x 128 B each);
-  // F2 k-block: w2h | w2l (256/CG rows x 128 B each).  2-SM pairs load half of every W tile per CTA.
-  static constexpr int W1_BYTES = CHUNK / CG * 128, W2_BYTES = 256 / CG * 128;
-  static constexpr int F1_BYTES = 32768 + 2 * W1_BYTES, F2_BYTES = 2 * W2_BYTES;
-  static constexpr int STAGE_BYTES = F1_BYTES > F2_BYTES ? F1_BYTES : F2_BYTES;   // 64 KB / 48 KB
-  static constexpr int STAGES = CG == 2 ? 3 : 2;
-  static constexpr int HS_BYTES = 65536;                 // [plane][k-block][128 rows x 128 B]; also the
-                                                         // LayerNorm epilogue's staging (Hs is idle then)
-  static constexpr int TMEM_COLS = 512;                  // acc1 x 2 (128 cols each) + acc2 (256 cols)
-  static constexpr int AUX_BYTES = MAX_N * 4 + 3 * 256 * 4 + 8 * 128 * 4 + 384;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + HS_BYTES + AUX_BYTES + 1024;
+  static constexpr int CHUNK = 64;                       // hidden columns per chunk
+  static constexpr int X_BYTES = 2 * 4 * BM * 128;       // [plane][k-block][128 rows x 128 B]
+  static constexpr int STAGE_BYTES = 32768, STAGES = 3;
+  static constexpr int SMEM_BYTES = X_BYTES + STAGES * STAGE_BYTES + 256 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-// CG = 2: CTA pairs (cta_group::2).  The pair owns 256 rows (rank r: rows mp*256 + r*128); each CTA
-// stages its own x rows, its own hidden chunk (Hs) and HALF of every W1 / W2 tile, the leader issues
-// M = 256 MMAs that read both CTAs' shared memory - which halves the weight bytes every SM has to
-// pull through TMA and, more importantly, the shared-memory bandwidth the B operand costs per MMA
-// (the 3-product split scheme reads every operand byte twice; at N = 128 a 1-SM MMA needs the full
-// 128 B/clk of shared-memory bandwidth for its operands alone).
-template <int CG>
-__global__ void __launch_bounds__(LN_THREADS, 1)
+__global__ void __launch_bounds__(NUM_THREADS, 1)
 k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
          const __grid_constant__ CUtensorMap tmW1h, const __grid_constant__ CUtensorMap tmW1l,
-         const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l,
-         const __grid_constant__ CUtensorMap tmOh, const __grid_constant__ CUtensorMap tmOl,
-         const __grid_constant__ CUtensorMap tmRh, const __grid_constant__ CUtensorMap tmRl, const FfnParams p) {
-  using Cfg = FfnCfg<CG>;
+         const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l, const FfnParams p) {
+  using Cfg = FfnCfg;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint8_t* hs = smem + STAGES * Cfg::STAGE_BYTES;
-  uint8_t* aux = hs + Cfg::HS_BYTES;
-  float* s_b1 = reinterpret_cast<float*>(aux);                // [MAX_N]
-  float* s_b2 = s_b1 + MAX_N;                                 // [256]
-  float* s_gamma = s_b2 + 256;
-  float* s_beta = s_gamma + 256;
-  float* s_part = s_beta + 256;                               // [4 quarters][mean | M2][128 rows]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_part + 8 * 128);
-  uint64_t* bar_full = bars;                  // [STAGES] ring stage filled (TMA tx; 2-SM: the leader's)
-  uint64_t* bar_empty = bars + 4;             // [STAGES] ring stage consumed (MMA commit, both CTAs)
-  uint64_t* bar_a1full = bars + 8;            // [2] F1 chunk accumulated (MMA commit, both CTAs)
-  uint64_t* bar_a1empty = bars + 10;          // [2] ... and drained by the epilogue warps (2-SM: leader's)
-  uint64_t* bar_hfull = bars + 12;            // Hs written by the epilogue warps (2-SM: leader's)
-  uint64_t* bar_hempty = bars + 13;           // Hs consumed (MMA commit, both CTAs)
-  uint64_t* bar_a2full = bars + 14;           // tile's acc2 complete (MMA commit, both CTAs)
-  uint64_t* bar_a2empty = bars + 15;          // ... and drained by the LayerNorm epilogue (2-SM: leader's)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
-  uint64_t* bar_res = bars + 17;              // [LN_WARPS] residual tile landed (one per epilogue warp)
+  uint8_t* ring = smem + Cfg::X_BYTES;
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
+  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per consumer warp)
+  uint64_t* bar_xfull = bar_empty + STAGES;   // x tile landed
+  uint64_t* bar_xempty = bar_xfull + 1;       // ... and read by the tile's last F1
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
-  int tl_n = 0;                                     // debug-timeline event counter of this warp
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  int tl_n = 0;
   tl_event(p.tl, tl_n, 40);                       // kernel entry
-  const int rank = CG > 1 ? (int)cluster_ctarank() : 0;
-  const int ncl = (int)gridDim.x / CG, cid = (int)blockIdx.x / CG;
+  const int ncta = (int)gridDim.x, cid = (int)blockIdx.x;
   const int NC = p.n_chunks;
-  // Items of this cluster: `full` whole tile groups (cid, cid + ncl, ...), then - for the first left * parts
-  // clusters - one PIECE of a leftover group: hidden chunks [c0, c1) of group full * ncl + cid / parts.  Pieces
-  // 0 .. parts-2 are contributors (their raw fp32 accumulator goes to `scratch`), the last piece is the finisher
-  // (adds the contributors' accumulators in piece order, then bias + residual + LayerNorm as for a whole tile).
-  // Contributors have lower cluster ids than their finisher, so they are scheduled no later than it.
-  struct Item { int mg, c0, c1, mode, piece0; };             // mode: 0 whole tile, 1 contributor, 2 finisher
-  const int ngroups = (p.m_tiles + CG - 1) / CG;
-  auto rev = [&](int grp) { return p.reverse ? ngroups - 1 - grp : grp; };
+  // Items of this CTA: `full` whole tiles (cid, cid + ncta, ...), then - for the first left * parts CTAs - one
+  // PIECE of a leftover tile: hidden chunks [c0, c1) of tile full * ncta + cid / parts.  Pieces 0 .. parts-2 are
+  // contributors (their raw fp32 accumulator goes to `scratch`), the last piece is the finisher (adds the
+  // contributors' accumulators in piece order, then bias + residual + LayerNorm as for a whole tile).
+  // Contributors have lower CTA ids than their finisher, so they are scheduled no later than it.
+  struct Item { int mt, c0, c1, mode, piece0; };             // mode: 0 whole tile, 1 contributor, 2 finisher
+  auto rev = [&](int t) { return p.reverse ? p.m_tiles - 1 - t : t; };
   const int nlocal = p.full + (cid < p.left * p.parts ? 1 : 0);
   auto item = [&](int j) -> Item {
-    if (j < p.full) return Item{rev(cid + j * ncl), 0, NC, 0, 0};
+    if (j < p.full) return Item{rev(cid + j * ncta), 0, NC, 0, 0};
     const int t = cid / p.parts, part = cid - t * p.parts;
     const int c0 = (part * NC + p.parts - 1) / p.parts, c1 = ((part + 1) * NC + p.parts - 1) / p.parts;
-    const int slot0 = (t * (p.parts - 1)) * CG + rank;       // slot of piece k of this CTA's rows: slot0 + k * CG
-    return Item{rev(p.full * ncl + t), c0, c1, p.parts == 1 ? 0 : (part == p.parts - 1 ? 2 : 1), p.parts == 1 ? 0 : slot0 + (part == p.parts - 1 ? 0 : part * CG)};
+    const int slot0 = t * (p.parts - 1);                     // slot of piece k of this tile: slot0 + k
+    return Item{rev(p.full * ncta + t), c0, c1, p.parts == 1 ? 0 : (part == p.parts - 1 ? 2 : 1),
+                p.parts == 1 ? 0 : slot0 + (part == p.parts - 1 ? 0 : part)};
   };
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&bar_a1full[s]), 1);
-      mbar_init(smem_u32(&bar_a1empty[s]), LN_WARPS * CG);
-    }
-    mbar_init(smem_u32(bar_hfull), LN_WARPS * CG);
-    mbar_init(smem_u32(bar_hempty), 1);
-    mbar_init(smem_u32(bar_a2full), 1);
-    mbar_init(smem_u32(bar_a2empty), LN_WARPS * CG);
-    for (int s = 0; s < LN_WARPS; ++s) mbar_init(smem_u32(&bar_res[s]), 1);
+    mbar_init(smem_u32(bar_xfull), 1);
+    mbar_init(smem_u32(bar_xempty), CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmXh); tma_prefetch_desc(&tmXl); tma_prefetch_desc(&tmW1h);
     tma_prefetch_desc(&tmW1l); tma_prefetch_desc(&tmW2h); tma_prefetch_desc(&tmW2l);
   }
-  if (CG > 1) { __syncthreads(); cluster_sync_all(); }
-  if (warp == 1) tmem_alloc<CG>(smem_u32(tmem_slot), Cfg::TMEM_COLS);
-  if (warp >= 2) {
-    for (int i = threadIdx.x - 64; i < MAX_N; i += LN_WARPS * 32) s_b1[i] = (p.b1 && i < p.n_chunks * Cfg::CHUNK) ? p.b1[i] : 0.0f;
-    for (int i = threadIdx.x - 64; i < 256; i += LN_WARPS * 32) {
-      s_gamma[i] = p.gamma[i]; s_beta[i] = p.beta[i]; s_b2[i] = p.b2 ? p.b2[i] : 0.0f;
-    }
-  }
   pdl_trigger();
-  tc_fence_before();
   __syncthreads();
-  if (CG > 1) cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   pdl_wait();
   tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
 
-  // arrive on a barrier that lives in the leader CTA (2-SM) or in this CTA (1-SM)
-  auto arrive_leader = [&](uint64_t* bar) {
-    if (CG == 1) mbar_arrive(smem_u32(bar));
-    else mbar_arrive_cluster(mapa_u32(smem_u32(bar), 0));
-  };
-
-  if (warp == 0) {
-    // ---------------------------------------------------------------- TMA producer (both CTAs)
-    // whole warp walks the loop, one elected lane issues (operands stay in uniform registers)
-    int kbg = 0;
-    auto stage_begin = [&](uint32_t bytes, uint32_t& full) -> uint32_t {   // elected lane: arm the barrier
-      const int s = kbg % STAGES;
-      full = smem_u32(&bar_full[s]);
-      if (CG == 1) {
-        mbar_expect_tx(full, bytes);
-      } else {
-        if (rank == 0) mbar_expect_tx(full, 2 * bytes);  // both CTAs' boxes are counted on the leader's barrier
-        full = mapa_u32(full, 0);
-      }
-      return smem_u32(smem + s * Cfg::STAGE_BYTES);
-    };
-    auto load = [&](uint32_t dst, const CUtensorMap* map, uint32_t full, int c0, int c1) {
-      if (CG == 1) tma_load_2d(dst, map, full, c0, c1);
-      else tma_load_2d_2sm(dst, map, full, c0, c1);
-    };
+  if (warp < 4) {
+    reg_dec<40>();
+    if (warp != 0) return;
+    // ---------------------------------------------------------------- TMA producer
+    int rc = 0;                                    // ring position
+    auto slot_wait = [&]() { mbar_wait(smem_u32(&bar_empty[rc % STAGES]), (((uint32_t)(rc / STAGES)) & 1u) ^ 1u); };
     for (int j = 0; j < nlocal; ++j) {
       const Item it = item(j);
-      const int m0 = (it.mg * CG + rank) * BM, nch = it.c1 - it.c0;
-      for (int i = 0; i <= nch; ++i) {
-        if (i < nch) {
-          for (int kb = 0; kb < 4; ++kb, ++kbg) {
-            mbar_wait(smem_u32(&bar_empty[kbg % STAGES]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
-            if (elect_one()) {
-              if (i == 0 && kb == 0 && j + 1 < nlocal) {      // next tile's x rows -> L2, a whole tile ahead
-                const int m1 = (item(j + 1).mg * CG + rank) * BM;
-                for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1); }
-              }
-              uint32_t full;
-              const uint32_t dst = stage_begin(Cfg::F1_BYTES, full);
-              load(dst, &tmXh, full, kb * BK, m0);
-              load(dst + 16384, &tmXl, full, kb * BK, m0);
-              load(dst + 32768, &tmW1h, full, kb * BK, (it.c0 + i) * Cfg::CHUNK + rank * (Cfg::CHUNK / CG));
-              load(dst + 32768 + Cfg::W1_BYTES, &tmW1l, full, kb * BK, (it.c0 + i) * Cfg::CHUNK + rank * (Cfg::CHUNK / CG));
-            }
-            __syncwarp();
-          }
+      const int m0 = it.mt * BM;
+      mbar_wait(smem_u32(bar_xempty), ((uint32_t)j & 1u) ^ 1u);
+      if (elect_one()) {
+        const uint32_t full = smem_u32(bar_xfull);
+        mbar_expect_tx(full, Cfg::X_BYTES);
+        for (int kb = 0; kb < 4; ++kb) {
+          tma_load_2d(smem_u32(smem + kb * 16384), &tmXh, full, kb * BK, m0);
+          tma_load_2d(smem_u32(smem + 65536 + kb * 16384), &tmXl, full, kb * BK, m0);
         }
-        if (i >= 1) {
-          for (int kb = 0; kb < 2; ++kb, ++kbg) {
-            mbar_wait(smem_u32(&bar_empty[kbg % STAGES]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
-            if (elect_one()) {
-              uint32_t full;
-              const uint32_t dst = stage_begin(Cfg::F2_BYTES, full);
-              load(dst, &tmW2h, full, (it.c0 + i - 1) * Cfg::CHUNK + kb * BK, rank * (256 / CG));
-              load(dst + Cfg::W2_BYTES, &tmW2l, full, (it.c0 + i - 1) * Cfg::CHUNK + kb * BK, rank * (256 / CG));
-            }
-            __syncwarp();
-          }
+        if (j + 1 < nlocal) {                      // next tile's x rows -> L2, a whole tile ahead
+          const int m1 = item(j + 1).mt * BM;
+          for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1); }
         }
       }
-    }
-  } else if (warp == 1) {
-    if (rank == 0) {
-      // ---------------------------------------------------------------- MMA issuer (2-SM: the leader)
-      // The whole warp walks the loop (uniform control flow); one elected lane issues each k-block.
-      constexpr uint32_t idesc1 = make_idesc(Cfg::CHUNK, BM * CG), idesc2 = make_idesc(256, BM * CG);
-      const uint32_t hs_u = smem_u32(hs);
-      // one k-block (64 deep): 4 x (A_lo.W_hi + A_hi.W_lo + A_hi.W_hi), then release the ring slot
-      auto kblock = [&](uint32_t tacc, uint32_t sAh, uint32_t sAl, uint32_t sWh, uint32_t sWl, uint32_t idesc,
-                        bool first, uint64_t* slot_bar, uint64_t* bar2, uint64_t* bar3) {
-        if (elect_one()) {
-          uint64_t ah = make_desc(sAh), al = make_desc(sAl), wh = make_desc(sWh), wl = make_desc(sWl);
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint32_t acc = (first && kk == 0) ? 0u : 1u;
-            if (CG == 1) {
-              umma(tacc, al, wh, idesc, acc); umma(tacc, ah, wl, idesc, 1u); umma(tacc, ah, wh, idesc, 1u);
-            } else {
-              umma_2sm(tacc, al, wh, idesc, acc); umma_2sm(tacc, ah, wl, idesc, 1u); umma_2sm(tacc, ah, wh, idesc, 1u);
-            }
-            ah += 2; al += 2; wh += 2; wl += 2;        // next 16-wide slice: +32 B (>> 4)
-          }
-          for (uint64_t* bar : {slot_bar, bar2, bar3})
-            if (bar) { if (CG == 1) umma_commit(smem_u32(bar)); else umma_commit_2sm(smem_u32(bar)); }
-        }
-        __syncwarp();
-      };
-      auto wait_epi = [&](uint64_t* bar, uint32_t parity) {     // barriers the epilogue warps arrive on
-        if (CG == 1) mbar_wait(smem_u32(bar), parity); else mbar_wait_cluster(smem_u32(bar), parity);
-      };
-      int kbg = 0, g1 = 0, g2 = 0;                 // ring position, F1 chunks issued, F2 chunks issued
-      for (int j = 0; j < nlocal; ++j) {
-        const Item it = item(j);
-        const int nch = it.c1 - it.c0;             // hidden chunks of this item
-        for (int i = 0; i <= nch; ++i) {
-          if (i < nch) {                           // F1(i)
-            const int b = g1 & 1;
-            wait_epi(&bar_a1empty[b], (((uint32_t)g1 >> 1) & 1u) ^ 1u);
-            tc_fence_after();
-            tl_event(p.tl, tl_n, 10, i);                             // MMA: F1(i) may start (acc1 buffer free)
-            const uint32_t tacc = tmem_base + (uint32_t)(b * Cfg::CHUNK);
-            for (int kb = 0; kb < 4; ++kb, ++kbg) {
-              const int s = kbg % STAGES;
-              mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
-              tc_fence_after();
-              const uint32_t sXh = smem_u32(smem + s * Cfg::STAGE_BYTES);
-              kblock(tacc, sXh, sXh + 16384, sXh + 32768, sXh + 32768 + Cfg::W1_BYTES, idesc1, kb == 0,
-                     &bar_empty[s], kb == 3 ? &bar_a1full[b] : nullptr, nullptr);
-            }
-            ++g1;
-          }
-          if (i >= 1) {                            // F2(i - 1)
-            if (i == 1) {                          // the previous tile's LayerNorm epilogue has drained acc2
-              wait_epi(bar_a2empty, ((uint32_t)j & 1u) ^ 1u);
-              tc_fence_after();
-            }
-            tl_event(p.tl, tl_n, 11, i - 1);                         // MMA: F1 chain issued, waiting for Hs(i - 1)
-            wait_epi(bar_hfull, (uint32_t)g2 & 1u);
-            tc_fence_after();
-            tl_event(p.tl, tl_n, 12, i - 1);                         // MMA: F2(i - 1) starts
-            const uint32_t tacc = tmem_base + 2u * Cfg::CHUNK;
-            for (int kb = 0; kb < 2; ++kb, ++kbg) {
-              const int s = kbg % STAGES;
-              mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
-              tc_fence_after();
-              const uint32_t sWh = smem_u32(smem + s * Cfg::STAGE_BYTES);
-              kblock(tacc, hs_u + kb * 16384, hs_u + 32768 + kb * 16384, sWh, sWh + Cfg::W2_BYTES, idesc2,
-                     i == 1 && kb == 0, &bar_empty[s], kb == 1 ? bar_hempty : nullptr,
-                     (kb == 1 && i == nch) ? bar_a2full : nullptr);
-            }
-            ++g2;
-          }
-        }
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps 2..17
-    const int q = warp & 3;                          // TMEM lane quarter
-    const int cq = (warp - 2) >> 2;                  // column quarter: 32 of a chunk's 128 hidden columns (E1),
-                                                     // 64 of the 256 output columns (LayerNorm)
-    const int row = q * 32 + lane;
-    uint8_t* const stg = hs + (warp - 2) * 4096;     // LayerNorm staging lives in the (then idle) Hs buffer
-    uint32_t r[32];
-    float v[32];
-    const bool has_res = p.res_hi != nullptr;
-    LnResidual t{smem_u32(&bar_res[warp - 2]), 0u};
-    bool drain_pending = false;                      // the last LayerNorm tail's staging drain is still owed
-    int g = 0;                                       // hidden chunks handled so far
-    for (int j = 0; j < nlocal; ++j) {
-      const Item it = item(j);
-      const int m0 = (it.mg * CG + rank) * BM;
-      // ---- E1: hidden chunks -> Hs
-      for (int c = it.c0; c < it.c1; ++c, ++g) {
-        const int b = g & 1;
-        mbar_wait(smem_u32(&bar_a1full[b]), ((uint32_t)g >> 1) & 1u);
-        tc_fence_after();
-        tl_event(p.tl, tl_n, 13, c);                                 // E1(c): acc1 ready
-        uint32_t PH[16], PL[16];
-        tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(b * Cfg::CHUNK + cq * 32), r);
-        epi_chunk_fast<ACT_GELU>(r, v, s_b1 + c * Cfg::CHUNK + cq * 32, p.inv_s1);
-        pack_split(v, PH, PL);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) arrive_leader(&bar_a1empty[b]);
-        mbar_wait(smem_u32(bar_hempty), ((uint32_t)g & 1u) ^ 1u);     // F2(g - 1) has read Hs
-        // Hs doubles as the LayerNorm staging: the previous tile's output stores must have read it.  That drain
-        // (~2.7k cycles) is taken here, under this chunk's TMEM load and GELU, instead of at the end of the tail.
-        if (drain_pending) { ln16_drain(lane); drain_pending = false; }
-        // this thread's row of k-block cq / 2, 64-byte half cq % 2: 4 x 16 B per plane, 16-B index XOR (row & 7)
-        // (SWIZZLE_128B)
-        uint8_t* const hrow = hs + (cq >> 1) * 16384 + row * 128;
-#pragma unroll
-        for (int jj = 0; jj < 4; ++jj) {
-          const int sl = (((cq & 1) * 4 + jj) ^ (row & 7)) << 4;
-          *reinterpret_cast<uint4*>(hrow + sl) = make_uint4(PH[4 * jj], PH[4 * jj + 1], PH[4 * jj + 2], PH[4 * jj + 3]);
-          *reinterpret_cast<uint4*>(hrow + 32768 + sl) = make_uint4(PL[4 * jj], PL[4 * jj + 1], PL[4 * jj + 2], PL[4 * jj + 3]);
-        }
-        fence_proxy_async_smem();                    // generic-proxy writes -> tcgen05.mma reads
-        __syncwarp();
-        tl_event(p.tl, tl_n, 14, c);                                 // E1(c): Hs written
-        if (lane == 0) arrive_leader(bar_hfull);
-      }
-      const uint32_t trow2 = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(2 * Cfg::CHUNK + cq * 64);
-      if (it.mode == 1) {
-        // ---- contributor piece: the raw fp32 accumulator -> scratch ([column group of 4][row][4]: a warp's
-        // 32 rows are 512 contiguous bytes per store), then the flag
-        mbar_wait(smem_u32(bar_a2full), (uint32_t)j & 1u);
-        tc_fence_after();
-        tl_event(p.tl, tl_n, 15, j);
-        float4* const dst = reinterpret_cast<float4*>(p.scratch + (size_t)it.piece0 * (BM * 256));
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          tmem_ld32(trow2 + c * 32, r);
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            dst[(cq * 16 + c * 8 + i) * 128 + row] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]),
-                                                                  __uint_as_float(r[4 * i + 2]), __uint_as_float(r[4 * i + 3]));
-        }
-        __threadfence();
-        ln_bar_sync();
-        if (threadIdx.x == 64) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.flags + it.piece0), "r"(1) : "memory");
-        tc_fence_before();
-        __syncwarp();
-        tl_event(p.tl, tl_n, 16, j);
-        if (lane == 0) arrive_leader(bar_a2empty);
-        continue;
-      }
-      // ---- residual + LayerNorm on acc2 (ln16_finish: sixteen warps, a row's four column quarters merged
-      // through shared memory); the first residual chunk is requested before the accumulator is awaited
-      const int wrow0 = m0 + q * 32;
-      const int rows_valid = min(32, p.M - wrow0);
-      mbar_wait(smem_u32(bar_a2full), (uint32_t)j & 1u);      // all F2 MMAs retired: acc2 complete, Hs idle
-      tc_fence_after();
-      tl_event(p.tl, tl_n, 15, j);                                   // LN tail: acc2 ready
-      // the residual tile lands in Hs (this warp's staging), which the F2 chain has only now finished reading
-      ln16_issue_residual(t, has_res, stg, &tmRh, &tmRl, wrow0, cq * 64, lane);
-      const int nparts = it.mode == 2 ? p.parts - 1 : 0;
-      if (nparts > 0) {                                      // finisher: the contributors' partials must have landed
-        if (lane == 0) {
-          for (int pp = 0; pp < nparts; ++pp) {
-            const int* f = p.flags + it.piece0 + pp * CG;
-            uint32_t v = 0;
-            long long t_end = clock64() + 4000000000ll;      // ~2 s: a lost contributor is a bug, trap instead of hanging
-            do {
-              asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-              if (v == 0 && clock64() > t_end) __trap();
-            } while (v == 0);
-          }
-        }
-        __syncwarp();
-      }
-      ln16_finish<true>(t, has_res, &tmRh, &tmRl, trow2, cq, row, lane, stg,
-                        s_b2, s_gamma, s_beta, s_part, p.inv_s2, wrow0, rows_valid, p.tma_out != 0, &tmOh, &tmOl,
-                        p.out_hi, p.out_lo, p.ld_out, p.tl, tl_n,
-                        nparts > 0 ? p.scratch + (size_t)it.piece0 * (BM * 256) : nullptr, nparts, (size_t)CG * (BM * 256),
-                        /*defer_drain=*/nparts == 0);
-      drain_pending = nparts == 0;
-      if (nparts > 0 && threadIdx.x == 64)                   // everyone is past its partial loads: re-arm the flags
-        for (int pp = 0; pp < nparts; ++pp) p.flags[it.piece0 + pp * CG] = 0;
-      // (the staging drain + barrier that frees Hs for the next E1 is deferred to that E1's first Hs write)
-      tc_fence_before();
       __syncwarp();
-      tl_event(p.tl, tl_n, 16, j);                                   // LN tail done
-      if (lane == 0) arrive_leader(bar_a2empty);
+      for (int c = it.c0; c < it.c1; ++c) {
+        for (int half = 0; half < 2; ++half, ++rc) {           // W1 rows [c*64, +64): k-blocks 2*half, 2*half + 1, hi then lo
+          slot_wait();
+          if (elect_one()) {
+            const uint32_t full = smem_u32(&bar_full[rc % STAGES]);
+            const uint32_t dst = smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES);
+            mbar_expect_tx(full, Cfg::STAGE_BYTES);
+            for (int k = 0; k < 2; ++k) {
+              tma_load_2d(dst + k * 8192, &tmW1h, full, (2 * half + k) * BK, c * Cfg::CHUNK);
+              tma_load_2d(dst + 16384 + k * 8192, &tmW1l, full, (2 * half + k) * BK, c * Cfg::CHUNK);
+            }
+          }
+          __syncwarp();
+        }
+        for (int pl = 0; pl < 2; ++pl, ++rc) {                 // W2[:, c*64 .. +64): hi plane, then lo plane
+          slot_wait();
+          if (elect_one()) {
+            const uint32_t full = smem_u32(&bar_full[rc % STAGES]);
+            mbar_expect_tx(full, Cfg::STAGE_BYTES);
+            tma_load_2d(smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES), pl ? &tmW2l : &tmW2h, full, c * Cfg::CHUNK, 0);
+          }
+          __syncwarp();
+        }
+      }
     }
-    if (drain_pending && lane == 0) tma_store_wait_read<0>();   // the last tile's stores still read this CTA's shared memory
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (CG > 1) cluster_sync_all();
+  // ------------------------------------------------------------------ consumer warpgroups
+  reg_inc<232>();
+  const int cw = (warp >> 2) - 1;
+  const int cp = 2 * (lane & 3);
+  const uint32_t sX = smem_u32(smem) + cw * (64 * 128);
+  float acc2[128];
+  float acc1[32];
+  uint32_t hh[4][4], hl[4][4];                     // the hidden chunk as A fragments: [16-deep k-step][register]
+  int rc = 0;
+  auto slot_full = [&](int r) { mbar_wait(smem_u32(&bar_full[r % STAGES]), ((uint32_t)(r / STAGES)) & 1u); };
+  auto slot_free = [&](int r) { if (lane == 0) mbar_arrive(smem_u32(&bar_empty[r % STAGES])); };
+  for (int j = 0; j < nlocal; ++j) {
+    const Item it = item(j);
+    const int m0 = it.mt * BM;
+    mbar_wait(smem_u32(bar_xfull), (uint32_t)j & 1u);
+    tl_event(p.tl, tl_n, 2, j);                                      // x tile landed
+    int pend = -1;                                   // ring position of the F2 group still in flight
+    for (int c = it.c0; c < it.c1; ++c) {
+      // ---- F1(c)
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        slot_full(rc + half);
+        const uint32_t w = smem_u32(ring + ((rc + half) % STAGES) * Cfg::STAGE_BYTES);
+        wg_fence();
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const uint32_t xh = sX + (2 * half + k) * 16384;
+          kblock_ss<64>(acc1, xh, xh + 65536, w + k * 8192, w + 16384 + k * 8192, half == 0 && k == 0);
+        }
+        wg_commit();
+      }
+      wg_wait<0>();
+      acc_fence(acc1);
+      if (pend >= 0) slot_free(pend);
+      slot_free(rc); slot_free(rc + 1);
+      rc += 2;
+      if (c == it.c1 - 1 && lane == 0) mbar_arrive(smem_u32(bar_xempty));     // the x tile may be overwritten
+      // ---- E1(c): bias + GELU -> split16 A fragments
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+#pragma unroll
+        for (int g = 0; g < 2; ++g) {
+          const int jj = 2 * ks + g, n = c * Cfg::CHUNK + 8 * jj + cp;
+          const float2 b = p.b1 ? __ldg(reinterpret_cast<const float2*>(p.b1 + n)) : make_float2(0.0f, 0.0f);
+          split2(gelu_fast(fmaf(acc1[4 * jj], p.inv_s1, b.x)), gelu_fast(fmaf(acc1[4 * jj + 1], p.inv_s1, b.y)),
+                 hh[ks][2 * g], hl[ks][2 * g]);
+          split2(gelu_fast(fmaf(acc1[4 * jj + 2], p.inv_s1, b.x)), gelu_fast(fmaf(acc1[4 * jj + 3], p.inv_s1, b.y)),
+                 hh[ks][2 * g + 1], hl[ks][2 * g + 1]);
+        }
+      }
+      // ---- F2(c): H_lo.W2_hi + H_hi.W2_hi on the hi slot, H_hi.W2_lo on the lo slot
+      slot_full(rc);
+      wg_fence();
+      {
+        const uint64_t wd = make_desc(smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES));
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          wgmma_rs_n256(acc2, hl[ks], wd + 2 * ks, (c == it.c0 && ks == 0) ? 0u : 1u);
+          wgmma_rs_n256(acc2, hh[ks], wd + 2 * ks, 1u);
+        }
+      }
+      wg_commit();
+      slot_full(rc + 1);
+      {
+        const uint64_t wd = make_desc(smem_u32(ring + ((rc + 1) % STAGES) * Cfg::STAGE_BYTES));
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) wgmma_rs_n256(acc2, hh[ks], wd + 2 * ks, 1u);
+      }
+      wg_commit();
+      wg_wait<1>();
+      slot_free(rc);
+      pend = rc + 1;
+      rc += 2;
+    }
+    wg_wait<0>();
+    acc_fence(acc2);
+    if (pend >= 0) slot_free(pend);
+    tl_event(p.tl, tl_n, 4, j);                                      // acc2 complete
+    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first row inside the tile
+    if (it.mode == 1) {
+      // ---- contributor piece: the raw fp32 accumulator -> scratch, then the flag
+      float* const dst = p.scratch + (size_t)it.piece0 * (BM * 256);
+#pragma unroll
+      for (int jj = 0; jj < 32; ++jj) {
+        *reinterpret_cast<float2*>(dst + rl * 256 + 8 * jj + cp) = make_float2(acc2[4 * jj], acc2[4 * jj + 1]);
+        *reinterpret_cast<float2*>(dst + (rl + 8) * 256 + 8 * jj + cp) = make_float2(acc2[4 * jj + 2], acc2[4 * jj + 3]);
+      }
+      __threadfence();
+      named_bar_sync(1, CONSUMER_WARPS * 32);
+      if (threadIdx.x == 128) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.flags + it.piece0), "r"(1) : "memory");
+      continue;
+    }
+    const int nparts = it.mode == 2 ? p.parts - 1 : 0;
+    if (nparts > 0) {
+      // ---- finisher: the contributors' partials must have landed; they are added in piece order
+      if (lane == 0) {
+        for (int pp = 0; pp < nparts; ++pp) {
+          const int* f = p.flags + it.piece0 + pp;
+          uint32_t v = 0;
+          long long t_end = clock64() + 4000000000ll;      // ~2 s: a lost contributor is a bug, trap instead of hanging
+          do {
+            asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
+            if (v == 0 && clock64() > t_end) __trap();
+          } while (v == 0);
+        }
+      }
+      __syncwarp();
+      for (int pp = 0; pp < nparts; ++pp) {
+        const float* src = p.scratch + (size_t)(it.piece0 + pp) * (BM * 256);
+#pragma unroll
+        for (int jj = 0; jj < 32; ++jj) {
+          const float2 a = __ldcg(reinterpret_cast<const float2*>(src + rl * 256 + 8 * jj + cp));
+          const float2 b = __ldcg(reinterpret_cast<const float2*>(src + (rl + 8) * 256 + 8 * jj + cp));
+          acc2[4 * jj] += a.x; acc2[4 * jj + 1] += a.y; acc2[4 * jj + 2] += b.x; acc2[4 * jj + 3] += b.y;
+        }
+      }
+      named_bar_sync(1, CONSUMER_WARPS * 32);                // everyone is past its partial loads: re-arm the flags
+      if (threadIdx.x == 128)
+        for (int pp = 0; pp < nparts; ++pp) p.flags[it.piece0 + pp] = 0;
+    }
+    ln_epilogue(acc2, p.inv_s2, p.b2, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
+                m0 + rl, p.M, cp);
+    tl_event(p.tl, tl_n, 5, j);                                      // LN tail done
+  }
   tl_event(p.tl, tl_n, 42);                       // kernel exit
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<CG>(tmem_base, Cfg::TMEM_COLS);
-  }
 }
 
 }  // namespace
@@ -1100,9 +590,9 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
 // ------------------------------------------------------------------------------ host side
 struct TcCtx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   int ffn_fused = 1;          // FFN1 + GELU + FFN2 + residual + LayerNorm as one launch (option ffn_fused)
-  int ffn_split = 1;          // cut the leftover tile groups of the fused FFN along the hidden dimension (option ffn_split)
+  int ffn_split = 1;          // cut the leftover tiles of the fused FFN along the hidden dimension (option ffn_split)
   tc::PFN_tmapEncodeTiled encode = nullptr;
 };
 
@@ -1123,14 +613,11 @@ TcCtx* tc_create(int device) {
   auto opt_in = [&](auto kernel, int bytes) {
     if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
   };
-  opt_in(k_gemm_tc<256, 1, EPI_FAST>, TileCfg<256, 1, EPI_FAST>::SMEM_BYTES); opt_in(k_gemm_tc<128, 1, EPI_FAST>, TileCfg<128, 1, EPI_FAST>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 2, EPI_FAST>, TileCfg<256, 2, EPI_FAST>::SMEM_BYTES); opt_in(k_gemm_tc<128, 2, EPI_FAST>, TileCfg<128, 2, EPI_FAST>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 1, EPI_FAST, ACT_GELU>, TileCfg<256, 1, EPI_FAST>::SMEM_BYTES); opt_in(k_gemm_tc<128, 1, EPI_FAST, ACT_GELU>, TileCfg<128, 1, EPI_FAST>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 2, EPI_FAST, ACT_GELU>, TileCfg<256, 2, EPI_FAST>::SMEM_BYTES); opt_in(k_gemm_tc<128, 2, EPI_FAST, ACT_GELU>, TileCfg<128, 2, EPI_FAST>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 1, EPI_GENERIC>, TileCfg<256, 1, EPI_GENERIC>::SMEM_BYTES); opt_in(k_gemm_tc<128, 1, EPI_GENERIC>, TileCfg<128, 1, EPI_GENERIC>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 2, EPI_GENERIC>, TileCfg<256, 2, EPI_GENERIC>::SMEM_BYTES); opt_in(k_gemm_tc<128, 2, EPI_GENERIC>, TileCfg<128, 2, EPI_GENERIC>::SMEM_BYTES);
-  opt_in(k_gemm_tc<256, 2, EPI_LN>, TileCfg<256, 2, EPI_LN>::SMEM_BYTES);
-  opt_in(k_ffn_tc<1>, FfnCfg<1>::SMEM_BYTES); opt_in(k_ffn_tc<2>, FfnCfg<2>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_FAST>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_FAST, ACT_GELU>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST, ACT_GELU>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_GENERIC>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_GENERIC>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_LN>, TileCfg<256>::SMEM_BYTES);
+  opt_in(k_ffn_tc, FfnCfg::SMEM_BYTES);
   if (e != cudaSuccess) {
     mldb_set_err(std::string("cudaFuncSetAttribute(k_gemm_tc): ") + cudaGetErrorString(e));
     delete c;
@@ -1153,24 +640,6 @@ static bool make_map(const TcCtx* c, CUtensorMap* m, const __half* base, int row
   return r == CUDA_SUCCESS;
 }
 
-// output map for the TMA-store epilogue: fp16 plane [rows, cols] with row pitch ld, 32 x 32 boxes whose
-// shared-memory image is SWIZZLE_64B (= stg_off); rows / columns beyond the extents are clipped
-static bool make_map_out(const TcCtx* c, CUtensorMap* m, const __half* base, int rows, int cols, int ld) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * sizeof(__half)};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = c->encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B,
-                         CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
-template <int EPI, int ACT = ACT_NONE>
-static constexpr int threads_of() { return EPI == EPI_LN ? LN_THREADS : NUM_THREADS; }
-template <int BN, int CG, int EPI, int ACT = ACT_NONE>
-static constexpr int smem_of() { return TileCfg<BN, CG, EPI>::SMEM_BYTES; }
-
 static int pick_bn(const GemmArgs& g) { return (g.w.N % 256 == 0) ? 256 : 128; }
 
 bool tc_gemm_supported(const TcCtx* c, const GemmArgs& g) {
@@ -1185,7 +654,7 @@ bool tc_gemm_supported(const TcCtx* c, const GemmArgs& g) {
 }
 
 bool tc_gemm_ln_supported(const TcCtx* c, const GemmArgs& g, const LnArgs& l) {
-  if (!tc_gemm_supported(c, g) || c->sm_count % 2) return false;
+  if (!tc_gemm_supported(c, g)) return false;
   if (g.w.N != 256 || l.d != 256 || g.act != ACT_NONE) return false;
   if (l.in_group != 0 || l.c != nullptr || l.out_f32 != nullptr || !l.out.hi) return false;
   if (l.out.cols != 256 || (l.res.hi && l.res.cols != 256)) return false;
@@ -1226,46 +695,24 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   bool ok = make_map(c, &mA1h, g.a1.hi, g.M, g.K1, BM) && make_map(c, &mA1l, g.a1.lo(), g.M, g.K1, BM);
   if (g.K2 > 0) ok = ok && make_map(c, &mA2h, g.a2.hi, g.M, g.K2, BM) && make_map(c, &mA2l, g.a2.lo(), g.M, g.K2, BM);
   else { mA2h = mA1h; mA2l = mA1l; }
-  const int m_tiles_ = (g.M + BM - 1) / BM;
-  // small problems: no pairs.  The LayerNorm epilogue exists for pairs only (its 16-warp staging does not fit
-  // next to a full-width W stage) - tc_gemm_ln_supported() has checked that the SM count is even.
-  const int cl = ((m_tiles_ >= 4 || ln) && c->sm_count % 2 == 0) ? 2 : 1;
-  ok = ok && make_map(c, &mWh, g.w.w, g.w.N, g.w.K, bn / cl) &&
-       make_map(c, &mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, bn / cl);
+  ok = ok && make_map(c, &mWh, g.w.w, g.w.N, g.w.K, bn) && make_map(c, &mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, bn);
   if (!ok) return map_fail("gemm", g.M, g.w.N, g.w.K);
   TcParams p;
   fill_params(g, ln, bn, &p);
-  CUtensorMap mOh = mA1h, mOl = mA1l;
   // the fast plain epilogue: split16 output, identity row mapping, N a whole number of tiles
   const bool fast = !ln && g.out.hi && !g.out_f32 && !g.addtab && !g.zero_lengths && g.in_group >= g.M &&
                     g.out_group == 0 && g.out_off == 0 && g.w.N % bn == 0 && g.w.bias != nullptr &&
                     (g.act == ACT_NONE || g.act == ACT_GELU);
-  CUtensorMap mRh = mA1h, mRl = mA1l;             // residual of the LayerNorm epilogue: same 32 x 32 SWIZZLE_64B boxes
-  if (cl == 2 && ln) {
-    if (!make_map_out(c, &mOh, ln->out.hi, g.M, 256, ln->out.cols) || !make_map_out(c, &mOl, ln->out.lo(), g.M, 256, ln->out.cols))
-      return map_fail("gemm ln out", g.M, g.w.N, g.w.K);
-    if (ln->res.hi && (!make_map_out(c, &mRh, ln->res.hi, g.M, 256, ln->res.cols) ||
-                       !make_map_out(c, &mRl, ln->res.lo(), g.M, 256, ln->res.cols)))
-      return map_fail("gemm ln residual", g.M, g.w.N, g.w.K);
-    p.tma_out = 1;
-  } else if (cl == 2 && fast) {
-    if (!make_map_out(c, &mOh, g.out.hi + g.out_col0, g.M, g.w.N, g.out.cols) ||
-        !make_map_out(c, &mOl, g.out.lo() + g.out_col0, g.M, g.w.N, g.out.cols))
-      return map_fail("gemm out", g.M, g.w.N, g.w.K);
-    p.tma_out = 1;
-  }
-  const int ngroups = ((p.m_tiles + cl - 1) / cl) * p.n_tiles;
-  const int ncl = ngroups < c->sm_count / cl ? ngroups : c->sm_count / cl;
-  dim3 grid(ncl * cl);
-#define MLDB_LAUNCH(BN_, CL_, ...)                                                                                       \
-  launch_pdl_cluster(k_gemm_tc<BN_, CL_, __VA_ARGS__>, grid, dim3(threads_of<__VA_ARGS__>()), smem_of<BN_, CL_, __VA_ARGS__>(), st, CL_, \
-                     mA1h, mA1l, mA2h, mA2l, mWh, mWl, mOh, mOl, mRh, mRl, p)
-#define MLDB_LAUNCH_SHAPE(...)                                                                        \
-  do {                                                                                                \
-    if (bn == 256) { if (cl == 2) MLDB_LAUNCH(256, 2, __VA_ARGS__); else MLDB_LAUNCH(256, 1, __VA_ARGS__); } \
-    else           { if (cl == 2) MLDB_LAUNCH(128, 2, __VA_ARGS__); else MLDB_LAUNCH(128, 1, __VA_ARGS__); } \
+  const int ntiles = p.m_tiles * p.n_tiles;
+  dim3 grid(ntiles < c->sm_count ? ntiles : c->sm_count);
+#define MLDB_LAUNCH(BN_, ...)                                                                                      \
+  launch_pdl(k_gemm_tc<BN_, __VA_ARGS__>, grid, dim3(NUM_THREADS), TileCfg<BN_>::SMEM_BYTES, st, mA1h, mA1l, mA2h, \
+             mA2l, mWh, mWl, p)
+#define MLDB_LAUNCH_SHAPE(...)                                                       \
+  do {                                                                               \
+    if (bn == 256) MLDB_LAUNCH(256, __VA_ARGS__); else MLDB_LAUNCH(128, __VA_ARGS__); \
   } while (0)
-  if (ln)                           { if (cl != 2) return map_fail("gemm ln needs CTA pairs", g.M, g.w.N, g.w.K); MLDB_LAUNCH(256, 2, EPI_LN); }
+  if (ln)                             MLDB_LAUNCH(256, EPI_LN);
   else if (fast && g.act == ACT_GELU) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_GELU);
   else if (fast)                      MLDB_LAUNCH_SHAPE(EPI_FAST);
   else                                MLDB_LAUNCH_SHAPE(EPI_GENERIC);
@@ -1291,53 +738,40 @@ bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, co
   if (!c || !c->ffn_fused) return false;
   if (!tc_gemm_supported(c, g1) || !tc_gemm_ln_supported(c, g2, l2)) return false;
   if (g1.K1 != 256 || g1.K2 > 0 || g2.K2 > 0 || g1.M != g2.M) return false;
-  if (g1.w.N % FfnCfg<1>::CHUNK || g1.w.N > MAX_N || g1.w.N != g2.K1) return false;
+  if (g1.w.N % FfnCfg::CHUNK || g1.w.N > MAX_N || g1.w.N != g2.K1) return false;
   if (g1.act != ACT_GELU || g1.out_f32 || g1.addtab || g1.zero_lengths) return false;
   if (g1.in_group < g1.M || g1.out_group != 0 || g1.out_off != 0) return false;
   return true;
 }
 bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* scratch, int* flags, cudaStream_t st) {
-  CUtensorMap mXh, mXl, mW1h, mW1l, mW2h, mW2l, mOh, mOl, mRh, mRl;
+  CUtensorMap mXh, mXl, mW1h, mW1l, mW2h, mW2l;
   const int m_tiles = (g1.M + BM - 1) / BM;
-  const int cg = (m_tiles >= 2 && c->sm_count % 2 == 0) ? 2 : 1;
   const bool ok = make_map(c, &mXh, g1.a1.hi, g1.M, g1.K1, BM) && make_map(c, &mXl, g1.a1.lo(), g1.M, g1.K1, BM) &&
-                  make_map(c, &mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg<1>::CHUNK / cg) &&
-                  make_map(c, &mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg<1>::CHUNK / cg) &&
-                  make_map(c, &mW2h, g2.w.w, g2.w.N, g2.w.K, 256 / cg) &&
-                  make_map(c, &mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256 / cg) &&
-                  make_map_out(c, &mOh, l2.out.hi, g1.M, 256, l2.out.cols) &&
-                  make_map_out(c, &mOl, l2.out.lo(), g1.M, 256, l2.out.cols);
+                  make_map(c, &mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+                  make_map(c, &mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+                  make_map(c, &mW2h, g2.w.w, g2.w.N, g2.w.K, 256) &&
+                  make_map(c, &mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256);
   if (!ok) return map_fail("ffn", g1.M, g1.w.N, g1.w.K);
-  mRh = mOh; mRl = mOl;
-  if (l2.res.hi && (!make_map_out(c, &mRh, l2.res.hi, g1.M, 256, l2.res.cols) || !make_map_out(c, &mRl, l2.res.lo(), g1.M, 256, l2.res.cols)))
-    return map_fail("ffn residual", g1.M, g1.w.N, g1.w.K);
   FfnParams p{};
-  p.M = g1.M; p.m_tiles = m_tiles; p.n_chunks = g1.w.N / FfnCfg<1>::CHUNK;
+  p.M = g1.M; p.m_tiles = m_tiles; p.n_chunks = g1.w.N / FfnCfg::CHUNK;
   p.tl = tc::mldb_timeline_buffer();
   p.inv_s1 = g1.w.inv_scale; p.inv_s2 = g2.w.inv_scale;
   p.b1 = g1.w.bias; p.b2 = g2.w.bias; p.gamma = l2.gamma; p.beta = l2.beta;
   p.res_hi = l2.res.hi; p.res_lo = l2.res.hi ? l2.res.lo() : nullptr; p.ld_res = l2.res.cols;
   p.out_hi = l2.out.hi; p.out_lo = l2.out.lo(); p.ld_out = l2.out.cols;
-  p.tma_out = 1;
-  const int groups = (m_tiles + cg - 1) / cg;
-  const int ncl_max = c->sm_count / cg;
-  // whole rounds of tile groups, then the leftover groups cut along the hidden dimension so that the last
-  // round uses (nearly) every cluster instead of `left` of them (FfnParams).  scratch == nullptr, a knob
-  // (MLDB_FFN_SPLIT=0) or left * 2 > clusters: the leftover groups run as whole tiles.
-  p.full = groups / ncl_max; p.left = groups % ncl_max; p.parts = 1;
+  const int ncta_max = c->sm_count;
+  // whole rounds of tiles, then the leftover tiles cut along the hidden dimension so that the last round
+  // uses (nearly) every SM instead of `left` of them (FfnParams).  scratch == nullptr, the ffn_split option
+  // off or left * 2 > SMs: the leftover tiles run as whole tiles.
+  p.full = m_tiles / ncta_max; p.left = m_tiles % ncta_max; p.parts = 1;
   p.scratch = scratch; p.flags = flags;
   if (p.left > 0 && scratch && flags && c->ffn_split) {
-    const int parts = std::min(p.n_chunks, ncl_max / p.left);
-    if (parts >= 2 && (size_t)p.left * (parts - 1) * cg * (BM * 256 * 4) <= TC_FFN_SCRATCH_BYTES) p.parts = parts;
+    const int parts = std::min(p.n_chunks, ncta_max / p.left);
+    if (parts >= 2 && (size_t)p.left * (parts - 1) * (BM * 256 * 4) <= TC_FFN_SCRATCH_BYTES) p.parts = parts;
   }
-  const int ncl = p.full > 0 ? ncl_max : p.left * p.parts;
+  const int ncta = p.full > 0 ? ncta_max : p.left * p.parts;
   static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
   p.reverse = snake;
-  if (cg == 2)
-    launch_pdl_cluster(k_ffn_tc<2>, dim3(ncl * 2), dim3(LN_THREADS), FfnCfg<2>::SMEM_BYTES, st, 2, mXh, mXl, mW1h, mW1l,
-                       mW2h, mW2l, mOh, mOl, mRh, mRl, p);
-  else
-    launch_pdl(k_ffn_tc<1>, dim3(ncl), dim3(LN_THREADS), FfnCfg<1>::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l,
-               mOh, mOl, mRh, mRl, p);
+  launch_pdl(k_ffn_tc, dim3(ncta), dim3(NUM_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
   return true;
 }

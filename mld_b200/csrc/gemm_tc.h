@@ -1,4 +1,4 @@
-// tcgen05 (5th-gen tensor core) split-fp16 GEMM with fused epilogues - interface.
+// wgmma (Hopper warpgroup MMA) split-fp16 GEMM with fused epilogues - interface.
 #pragma once
 #include "ops.cuh"
 
@@ -12,7 +12,7 @@ bool tc_gemm_ln_supported(const TcCtx* c, const GemmArgs& g, const LnArgs& l);
 // enqueue; ln == nullptr for the plain epilogue.  false: tensor-map encoding failed, nothing was
 // launched and mldb_last_error() says why.
 bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st);
-// FFN block linear1 + GELU + linear2 + residual + LayerNorm as one launch (hidden stays on the SM)
+// FFN block linear1 + GELU + linear2 + residual + LayerNorm as one launch (hidden stays in registers)
 bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2);
 // scratch / flags: TC_FFN_SCRATCH_BYTES / TC_FFN_FLAG_BYTES of device memory owned by the caller, one pair per stream
 // that may run tc_ffn concurrently (flags zeroed once); nullptr = no hidden-dimension split of leftover tiles

@@ -1,4 +1,4 @@
-// Operator argument blocks shared by the tensor-core (tcgen05) and SIMT implementations.
+// Operator argument blocks shared by the tensor-core (wgmma) and SIMT implementations.
 #pragma once
 #include "common.cuh"
 
@@ -71,10 +71,10 @@ void simt_attention(const AttnArgs& a, cudaStream_t st);
 bool mma_attention_supported(const AttnArgs& a);
 void mma_attention_init();
 void mma_attention(const AttnArgs& a, cudaStream_t st);
-// attn_tc.cu: tcgen05 attention core (Lq, Lk <= 256, head_dim 64 / 128)
+// attn_tc.cu: wgmma attention core (Lk <= 256, head_dim 64 / 128)
 bool tc_attention_init(int device);                       // once per process, outside stream capture
 bool tc_attention_supported(const AttnArgs& a);
 bool tc_attention(const AttnArgs& a, cudaStream_t st);    // false: tensor-map encoding failed, nothing launched
 void simt_init();
-// --- tcgen05 implementations (gemm_tc.cu) ---
+// --- wgmma implementations (gemm_tc.cu) ---
 struct TcCtx;

@@ -1,5 +1,5 @@
 // CUDA-core (fp32 FFMA) implementations of the path's operators.  These are the on-device
-// reference for the tcgen05 kernels (engine option gemm=simt) and serve the GEMMs whose
+// reference for the wgmma kernels (engine option gemm=simt) and serve the GEMMs whose
 // shapes do not fit a tensor-core tile (odd K such as 263/150 motion features, tiny M).
 #include "ops.cuh"
 

@@ -6,7 +6,7 @@
   lengths equal, else the reference raises) and a ``.txt`` with every prompt of every replication, one per line
   (demo.py:195-214).
 
-What is B200-native here is how the joints reach the host: :class:`PinnedJointsReader` copies each finished batch
+What is H100-native here is how the joints reach the host: :class:`PinnedJointsReader` copies each finished batch
 device -> pinned host memory on a side stream and hands the file writing to the caller while the NEXT
 replication is already sampling, instead of the reference's synchronous ``.cpu()`` per motion.
 """

@@ -29,7 +29,7 @@ class Engine:
         self._h = None
         self.lib = _lib.lib()
         if not torch.cuda.is_available():
-            raise RuntimeError("mld_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise RuntimeError("mld_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         dev = torch.device(device) if not isinstance(device, int) else torch.device("cuda", device)
         self.device = dev
         self.cfg = cfg
@@ -100,7 +100,7 @@ class Engine:
 
     def debug_ffn(self, X, W1, b1, W2, b2, gamma, beta, mode=2):
         """Kernel unit-test hook (mldb_debug_ffn): LayerNorm(X + W2 gelu(W1 X + b1) + b2); mode 0 CUDA-core,
-        1 tcgen05 GEMMs (two launches), 2 fused tcgen05 FFN kernel.  X [M,d] (device), the rest host."""
+        1 wgmma GEMMs (two launches), 2 fused wgmma FFN kernel.  X [M,d] (device), the rest host."""
         X = _f32c(X, self.device)
         host = [t.detach().float().contiguous().cpu() for t in (W1, b1, W2, b2, gamma, beta)]
         M, d = X.shape
@@ -113,7 +113,7 @@ class Engine:
     def debug_attention(self, q, nseq, Lq, heads, lengths=None, mode=2, kv=None, Lk=None, kv_prefix=0):
         """Kernel unit-test hook (mldb_debug_attention).  ``kv is None``: ``q`` is a packed qkv
         [nseq*Lq, 3*heads*hd] tensor (self-attention, the layout the stacks use); else ``q`` [nseq*Lq, d] and
-        ``kv`` [nseq*Lk, 2*d] (cross-attention).  mode 0 CUDA-core, 1 mma.sync, 2 tcgen05 (product).
+        ``kv`` [nseq*Lk, 2*d] (cross-attention).  mode 0 CUDA-core, 1 mma.sync, 2 wgmma (product).
         Returns [nseq*Lq, heads*hd]."""
         q = _f32c(q, self.device)
         kvd = None if kv is None else _f32c(kv, self.device)

@@ -56,7 +56,7 @@ class _EngineModule(nn.Module):
     def engine(self) -> Engine:
         dev = next(self.parameters()).device
         if dev.type != "cuda":
-            raise RuntimeError(f"{type(self).__name__} runs on a B200 only: move it with .cuda() "
+            raise RuntimeError(f"{type(self).__name__} runs on a H100 only: move it with .cuda() "
                                "(no CPU/PyTorch fallback exists)")
         if self._engine is None or self._engine_epoch != self._weights_epoch or self._engine.device != dev:
             eng = Engine(self._make_config(), dev)

@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz by running the REFERENCE's own modules (TEST INFRASTRUCTURE).
 
-Run in the build container only (``/root/reference`` does not exist on the GPU box):
+Run in the build container only (``/root/reference`` does not exist ):
 
     python -m oracle.make_golden
 

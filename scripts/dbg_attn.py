@@ -1,4 +1,4 @@
-"""Bring-up aid for the tcgen05 attention kernel: every shape in its own process (a device trap poisons the
+"""Bring-up aid for the wgmma attention kernel: every shape in its own process (a device trap poisons the
 context), with an error breakdown by head / query-row block / which key blocks seem to contribute.
 usage: python scripts/dbg_attn.py            (all cases)      python scripts/dbg_attn.py one nseq Lq Lk hd masked"""
 import os, subprocess, sys

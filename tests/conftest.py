@@ -9,12 +9,12 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
 def built_lib():
-    """The in-tree C-ABI library (compiled by nvcc here, prebuilt on the GPU box)."""
+    """The in-tree C-ABI library (compiled by nvcc on first use)."""
     import __graft_entry__ as g
     g.build()
     from mld_b200 import _lib

@@ -1,4 +1,4 @@
-"""GPU kernel unit tests (pytest -m gpu): each GEMM epilogue of the tcgen05 kernel against a
+"""GPU kernel unit tests (pytest -m gpu): each GEMM epilogue of the wgmma kernel against a
 float64 torch reference of the same op, and against the CUDA-core kernel, through the C ABI's
 debug hook.  Tolerance 5e-6 relative-to-max: the split-fp16 3-product scheme keeps ~22 bits."""
 import pytest
@@ -54,11 +54,11 @@ def test_tc_gemm_epilogues(eng, M, N, K, K1, act, ln):
     y_cc = eng.debug_gemm(A, W, bias, K1=K1, act=act, use_tc=False, **kw)
     assert torch.isfinite(y_tc).all()
     assert _rel(y_cc, ref) < 5e-6, "CUDA-core kernel vs float64 reference"
-    assert _rel(y_tc, ref) < 5e-6, "tcgen05 kernel vs float64 reference"
+    assert _rel(y_tc, ref) < 5e-6, "wgmma kernel vs float64 reference"
     if not ln and N % 8 == 0:
         # the production epilogue: split16 planes (TMA bulk stores on the CTA-pair kernels)
         y_sp = eng.debug_gemm(A, W, bias, K1=K1, act=act, use_tc=True, split_out=True)
-        assert _rel(y_sp, ref) < 5e-6, "tcgen05 kernel, split16 output"
+        assert _rel(y_sp, ref) < 5e-6, "wgmma kernel, split16 output"
 
 
 @pytest.mark.parametrize("M,ff", [(100, 1024), (128 * 3 + 5, 1024), (148 * 128 * 2 + 777, 1024), (1000, 512),
@@ -186,7 +186,7 @@ SELF_ATTN_CASES = [
     (3, 60, 64, True),           # ActorVae
     (6, 196, 128, False),        # no-VAE denoiser (d = 512): two 64-wide slices of the head, one Q buffer
     (3, 79, 128, True),
-    (2, 256, 64, False),         # the largest key count the score row fits (256 TMEM columns)
+    (2, 256, 64, False),         # the largest key count the score row fits (the score row lives in registers)
     (256, 196, 64, True),        # VAE decode at the benchmark batch: many items per CTA on ONE score buffer
     (90, 196, 128, False),       # ... and with head_dim 128
     (400, 130, 64, True),        # three key blocks on two score buffers
@@ -195,7 +195,7 @@ SELF_ATTN_CASES = [
 
 @pytest.mark.parametrize("nseq,L,hd,masked", SELF_ATTN_CASES)
 def test_self_attention_kernels(eng, nseq, L, hd, masked):
-    """The attention cores in isolation on the packed q|k|v layout of the stacks, against float64: tcgen05
+    """The attention cores in isolation on the packed q|k|v layout of the stacks, against float64: wgmma
     (product), mma.sync and CUDA cores.  5e-6 relative-to-max: the split-fp16 scheme keeps ~22 bits."""
     heads = 4
     d = heads * hd
@@ -203,7 +203,7 @@ def test_self_attention_kernels(eng, nseq, L, hd, masked):
     qkv = torch.randn(nseq * L, 3 * d, generator=g)
     lengths = [max(1, (7 * i + 5) % L) for i in range(nseq)] if masked else None
     ref = _attention_ref(qkv[:, :d], qkv[:, d:2 * d], qkv[:, 2 * d:], nseq, L, L, heads, lengths)
-    for mode, name in ((2, "tcgen05"), (1, "mma.sync"), (0, "cuda-core")):
+    for mode, name in ((2, "wgmma"), (1, "mma.sync"), (0, "cuda-core")):
         if mode == 1 and (hd == 128 and L > 128 or L < 8):
             continue                       # outside the mma.sync kernel's shared-memory budget / tile shape
         y = eng.debug_attention(qkv, nseq, L, heads, lengths, mode=mode).cpu().double()
@@ -231,7 +231,7 @@ def test_cross_attention_kernels(eng, nseq, Lq, Lk, hd, prefix, masked):
     lengths = [max(1, (11 * i + 3) % (Lk - prefix)) for i in range(nseq)] if masked else None
     nk = None if lengths is None else [min(Lk, prefix + n) for n in lengths]
     ref = _attention_ref(q, kv[:, :d], kv[:, d:], nseq, Lq, Lk, heads, nk)
-    for mode, name in ((2, "tcgen05"), (0, "cuda-core")):
+    for mode, name in ((2, "wgmma"), (0, "cuda-core")):
         y = eng.debug_attention(q, nseq, Lq, heads, lengths, mode=mode, kv=kv, Lk=Lk, kv_prefix=prefix).cpu().double()
         assert torch.isfinite(y).all(), name
         assert _rel(y, ref) < 5e-6, name
@@ -239,8 +239,8 @@ def test_cross_attention_kernels(eng, nseq, Lq, Lk, hd, prefix, masked):
 
 def test_product_path_runs_on_tcgen05(built_lib):
     """Kernel-choice introspection (mldb_kernel_stats): the text-to-motion path enqueues its GEMMs, FFN blocks
-    and attention on the tcgen05 kernels - no CUDA-core attention, no LayerNorm split off a GEMM - and the
-    CTA-pair variants the benchmark runs are the ones a medium batch exercises."""
+    and attention on the tensor-core kernels (wgmma on this architecture; the test keeps its first name) - no
+    CUDA-core attention, no LayerNorm split off a GEMM."""
     from mld_b200 import synth
     from mld_b200.engine import Engine, make_config
     eng = Engine(make_config(), 0)

@@ -352,7 +352,7 @@ def test_novae_full_shape_vs_reference_golden_and_oracle(novae):
     """configs[4] shape: 196 frames x 263 features, d = 512 (head_dim 128), ragged lengths.  Single forward
     against the reference module's output, then 4 guided DDPM steps with injected noise against the oracle;
     the kernel statistics must show every attention (196 x 196 self-attention, 2-token cross-attention) on
-    the tcgen05 kernel and every stack GEMM on the tensor cores."""
+    the wgmma kernel and every stack GEMM on the tensor cores."""
     eng, nsd = novae
     g = golden("denoiser_novae_T196.npz")
     lengths = [196, 132]
