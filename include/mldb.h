@@ -233,7 +233,10 @@ int mldb_debug_timeline(int32_t enable, int64_t* out, int32_t cap, int32_t* coun
  * given, through the engine's GEMM operators (use_tc: 1 = wgmma path, 0 = CUDA-core path).
  * A [M,K], R [M,N], out [M,N]: fp32 DEVICE; W [N,K], bias/gamma/beta [N]: fp32 HOST.  0 < K1 < K feeds
  * A as two concatenated sources (the skip-connection GEMM).  split_out != 0: the plain epilogue writes
- * split16 planes (the production path; N % 8 == 0) which are then widened to fp32.  Synchronous. */
+ * split16 planes (the production path; N % 8 == 0) which are then widened to fp32.  Synchronous.
+ * R given without gamma selects the residual-add epilogue out = A W^T + b + R (fp32 output, act must be 0 on
+ * the wgmma path; R == out runs it in place, as the text tower does).  act: 0 none, 1 GELU, 2 ReLU, 3 SiLU,
+ * 4 quick-GELU x * sigmoid(1.702 x) (CLIP).  N up to 4096 runs on the wgmma kernel here. */
 int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float* bias, const float* gamma,
                     const float* beta, const float* R, int32_t M, int32_t N, int32_t K, int32_t K1,
                     int32_t act, int32_t use_tc, int32_t split_out, float* out, void* stream);
@@ -257,6 +260,45 @@ int mldb_debug_attention(mldb_handle* h, const float* Q, const float* KV, const 
                          int32_t nseq, int32_t Lq, int32_t Lk, int32_t heads, int32_t hd, int32_t mode, float* out,
                          void* stream);
 
+/* Debug aid: mldb_debug_attention with a causal mask (query i attends to keys j <= i; self-attention only:
+ * KV must be NULL, Lq == Lk).  mode 1 (mma.sync) has no causal mask and returns MLDB_ERR_UNSUPPORTED. */
+int mldb_debug_attention_causal(mldb_handle* h, const float* Q, const float* KV, const int32_t* lengths,
+                                int32_t kv_prefix, int32_t nseq, int32_t Lq, int32_t Lk, int32_t heads, int32_t hd,
+                                int32_t mode, float* out, void* stream);
+
+/* ---- CLIP text encoder (MldTextEncoder, mld/models/architectures/mld_clip.py): token ids -> the denoiser's context.
+ * The CLIP ViT-L/14 text tower: token + position embedding, `layers` pre-norm blocks (LN1 -> causal self-attention
+ * -> + residual, LN2 -> fc1 -> quick-GELU -> fc2 -> + residual), final LayerNorm; pooled mode adds the eos-row
+ * gather and text_projection.  The tokenizer stays on the host (Hugging Face's); this path starts at int64 ids. */
+#define MLDB_TEXT_ABI_VERSION 1
+#define MLDB_TEXT_HIDDEN 0   /* "clip_hidden": text_model(ids).last_hidden_state            [n, L, hidden] */
+#define MLDB_TEXT_POOLED 1   /* "clip": get_text_features(ids) (the shipped config)            [n, projection_dim] */
+typedef struct mldb_text_config {
+  int32_t abi_version;       /* must be MLDB_TEXT_ABI_VERSION */
+  int32_t vocab_size;        /* 49408 */
+  int32_t max_positions;     /* 77 */
+  int32_t hidden;            /* 768 (a multiple of 128, <= 1024) */
+  int32_t heads;             /* 12 (head_dim hidden / heads must be 64 or 128 for the wgmma attention) */
+  int32_t layers;            /* 12 */
+  int32_t ff;                /* 3072 */
+  int32_t projection_dim;    /* 768 */
+  int32_t eos_token_id;      /* 49407; 2 selects the legacy argmax(ids) pooling rule */
+  float   ln_eps;            /* 1e-5 */
+} mldb_text_config;
+void mldb_default_text_config(mldb_text_config* cfg);
+/* Add the text tower's keys to the strict key spec; call after mldb_create, before mldb_finalize_weights.  Keys are
+ * "text_encoder." + MldTextEncoder.state_dict() keys of the text tower ("text_encoder.text_model.text_model.encoder.
+ * layers.0.self_attn.q_proj.weight", "text_encoder.text_model.text_projection.weight", ...); the position_ids buffer
+ * of older checkpoints is not one of them.  q/k/v_proj are packed into one [3 * hidden, hidden] operand at finalize. */
+int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg);
+/* Replaces: MldTextEncoder.forward after the tokenizer (mld_clip.py:53-97).
+ *   ids  device int64 [n, L], 1 <= L <= max_positions; an id outside [0, vocab_size) yields a NaN row
+ *   out  MLDB_TEXT_HIDDEN: [n, L, hidden]; MLDB_TEXT_POOLED: [n, projection_dim]
+ * Enqueued eagerly on `stream` (no graph); the workspace grows on demand (outside any capture: synchronises the
+ * device when it does).  The GEMMs and the attention count under MLDB_KSTAT_GEMM_TC / ATTN_TC (or the *_SIMT
+ * indices with gemm=simt / attn=simt), the row LayerNorms under MLDB_KSTAT_TEXT_LN. */
+int mldb_text_encode(mldb_handle* h, const int64_t* ids, int32_t n, int32_t L, int32_t mode, float* out, void* stream);
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);
@@ -275,7 +317,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
 #define MLDB_KSTAT_LN_SIMT 7      /* k_ln stand-alone LayerNorm (stack-final norms, cross-attention collapse) */
 #define MLDB_KSTAT_LN_UNFUSED 8   /* k_ln behind a GEMM whose LayerNorm could NOT be fused (a fallback) */
 #define MLDB_KSTAT_MISC 9         /* token assembly, scheduler step, feats2joints, ... */
-#define MLDB_KSTAT_COUNT 10
+#define MLDB_KSTAT_TEXT_LN 10     /* k_text_ln: the text tower's row LayerNorm (+ embedding / eos gather) */
+#define MLDB_KSTAT_COUNT 11
 int mldb_kernel_stats(const mldb_handle* h, int64_t* out, int32_t n);
 int mldb_reset_kernel_stats(mldb_handle* h);
 

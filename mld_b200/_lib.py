@@ -20,7 +20,10 @@ SCHED_DDIM, SCHED_DDPM = 0, 1
 DTYPE_F32 = 0
 # mldb_kernel_stats indices (MLDB_KSTAT_* in include/mldb.h)
 KSTAT_NAMES = ("gemm_tc", "gemm_ln_tc", "ffn_tc", "attn_tc", "attn_mma", "attn_simt", "gemm_simt", "ln_simt",
-               "ln_unfused", "misc")
+               "ln_unfused", "misc", "text_ln")
+# CLIP text tower (mldb_text_config, mldb_text_encode)
+MLDB_TEXT_ABI_VERSION = 1
+TEXT_HIDDEN, TEXT_POOLED = 0, 1
 
 
 class MldbConfig(C.Structure):
@@ -37,6 +40,15 @@ class MldbConfig(C.Structure):
         ("sched_kind", C.c_int32), ("num_train_timesteps", C.c_int32),
         ("beta_start", C.c_double), ("beta_end", C.c_double), ("steps_offset", C.c_int32),
         ("set_alpha_to_one", C.c_int32), ("eta", C.c_float), ("njoints", C.c_int32),
+    ]
+
+
+class MldbTextConfig(C.Structure):
+    """``mldb_text_config`` (include/mldb.h)."""
+    _fields_ = [
+        ("abi_version", C.c_int32), ("vocab_size", C.c_int32), ("max_positions", C.c_int32),
+        ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32), ("ff", C.c_int32),
+        ("projection_dim", C.c_int32), ("eos_token_id", C.c_int32), ("ln_eps", C.c_float),
     ]
 
 
@@ -68,6 +80,11 @@ _SIGNATURES = {
     "mldb_debug_ffn": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_debug_attention": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, _P, _P]),
+    "mldb_debug_attention_causal": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                              C.c_int32, C.c_int32, _P, _P]),
+    "mldb_default_text_config": (None, [C.POINTER(MldbTextConfig)]),
+    "mldb_text_configure": (C.c_int, [_P, C.POINTER(MldbTextConfig)]),
+    "mldb_text_encode": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
@@ -114,4 +131,10 @@ def check(status: int, what: str = "mldb"):
 def default_config() -> MldbConfig:
     cfg = MldbConfig()
     lib().mldb_default_config(C.byref(cfg))
+    return cfg
+
+
+def default_text_config() -> MldbTextConfig:
+    cfg = MldbTextConfig()
+    lib().mldb_default_text_config(C.byref(cfg))
     return cfg

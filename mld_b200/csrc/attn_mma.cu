@@ -244,6 +244,7 @@ size_t attn_smem(const AttnArgs& a) {
 bool mma_attention_supported(const AttnArgs& a) {
   if (a.hd != 64 && a.hd != 128) return false;
   if (a.Lk < 8) return false;                                  // 1-2 memory tokens: CUDA-core kernel
+  if (a.causal) return false;                                  // no causal mask here: wgmma or CUDA-core kernel
   if ((a.q.cols % 8) || (a.kv.cols % 8) || (a.q_col0 % 8) || (a.k_col0 % 8) || (a.v_col0 % 8)) return false;
   const size_t smem = a.hd == 64 ? attn_smem<64>(a) : attn_smem<128>(a);
   return smem <= 227 * 1024;

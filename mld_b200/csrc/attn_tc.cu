@@ -2,7 +2,8 @@
 // Replaces the attention core of nn.MultiheadAttention (cross_attention.py:264-266, 330-338):
 // scores scaled by 1/sqrt(head_dim), padded keys masked (-inf), softmax over keys, P @ V - for
 // every shape the sampling path uses: Lq in 1.., Lk in 1..256 (denoiser 79 / 3 tokens, VAE 196 / 198
-// frames, 1-2 memory tokens), head_dim 64 or 128.
+// frames, 1-2 memory tokens), head_dim 64 or 128.  Causal self-attention (the CLIP text tower): query i sees
+// keys j <= i; the key blocks that lie wholly above a query tile's diagonal are neither loaded nor multiplied.
 //
 // Work item = (sequence, head, 64-row query tile) = one warpgroup's MMA height.  A CTA (one per SM,
 // persistent) runs TWO independent pipelines, each a consumer warpgroup with its own Q buffer and
@@ -49,6 +50,11 @@ struct AtcParams {
 };
 
 struct Item { int s, h, qt; };
+// key blocks item `it` needs: all of them, or (causal) the blocks up to its query tile's diagonal (KBLK == QROWS)
+template <bool CAUSAL>
+__device__ __forceinline__ int item_kblocks(const Item& it, int nkb) {
+  return CAUSAL ? min(nkb, it.qt + 1) : nkb;
+}
 __device__ __forceinline__ Item decode_item(int item, const AtcParams& p) {
   Item it;
   if (p.reverse) item = p.items - 1 - item;
@@ -70,7 +76,8 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-template <int HD>
+// CAUSAL is a template parameter so that the non-causal instantiations (the sampling path) carry no mask state
+template <int HD, bool CAUSAL>
 __global__ void __launch_bounds__(ATC_THREADS, 1)
 k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
           const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,    // 64-row boxes
@@ -90,7 +97,6 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   int tl_n = 0;                                       // debug-timeline event counter of this warp
   tl_event(p.tl, tl_n, 40);                       // kernel entry
   const int nkb = p.nkb;
-
   if (threadIdx.x == 0) {
     for (int g = 0; g < 2; ++g) {
       uint64_t* b = bars + g * (2 + 2 * MAX_RS);
@@ -125,6 +131,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     int rc = 0;                                       // ring position (K and V blocks, all items)
     for (int j = 0; j < nlocal; ++j) {
       const Item it = decode_item(pid + j * npipes, p);
+      const int nkb_i = item_kblocks<CAUSAL>(it, nkb);
       mbar_wait(smem_u32(q_empty), ((uint32_t)j & 1u) ^ 1u);
       tl_event(p.tl, tl_n, 20, j);                                     // producer: Q buffer free, loads issued
       if (elect_one()) {
@@ -141,7 +148,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
       __syncwarp();
       for (int kv = 0; kv < 2; ++kv) {
         const int col0 = (kv ? p.v_col0 : p.k_col0) + it.h * HD;
-        for (int kb = 0; kb < nkb; ++kb, ++rc) {
+        for (int kb = 0; kb < nkb_i; ++kb, ++rc) {
           const int sl_i = rc % RS;
           mbar_wait(smem_u32(&r_empty[sl_i]), (((uint32_t)(rc / RS)) & 1u) ^ 1u);
           if (elect_one()) {
@@ -173,15 +180,19 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   int rc = 0;
   for (int j = 0; j < nlocal; ++j) {
     const Item it = decode_item(pid + j * npipes, p);
+    const int nkb_i = item_kblocks<CAUSAL>(it, nkb);
     int nk = p.Lk;
     if (p.lengths) nk = min(p.Lk, p.kv_prefix + p.lengths[p.len_mod > 0 ? (p.seq0 + it.s) % p.len_mod : it.s]);
+    // valid keys of this thread's two query rows (causal: keys j <= i)
+    const int q0 = it.qt * QROWS + row;
+    const int nk0 = CAUSAL ? min(nk, q0 + 1) : nk, nk1 = CAUSAL ? min(nk, q0 + 9) : nk;
     mbar_wait(smem_u32(q_full), (uint32_t)j & 1u);
     tl_event(p.tl, tl_n, 22, j);                                       // Q(j) landed
     // ---- S = Q K^T, block by block; a block's ring slot is freed when the NEXT block's MMAs have been issued
     const uint32_t qbase = smem_u32(sQ);
 #pragma unroll
     for (int kb = 0; kb < MAX_KB; ++kb) {
-      if (kb < nkb) {
+      if (kb < nkb_i) {
         const int sl_i = (rc + kb) % RS;
         mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
         const uint32_t kbase = smem_u32(sR + sl_i * SLOT_BYTES);
@@ -207,26 +218,26 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     }
     wg_wait<0>();
     if (lane == 0) {
-      mbar_arrive(smem_u32(&r_empty[(rc + nkb - 1) % RS]));
+      mbar_arrive(smem_u32(&r_empty[(rc + nkb_i - 1) % RS]));
       mbar_arrive(smem_u32(q_empty));                 // Q only feeds the scores
     }
-    rc += nkb;
+    rc += nkb_i;
 #pragma unroll
     for (int kb = 0; kb < MAX_KB; ++kb)
-      if (kb < nkb) acc_fence(S[kb]);
+      if (kb < nkb_i) acc_fence(S[kb]);
     tl_event(p.tl, tl_n, 31, j);                                       // softmax: S(j) ready
     // ---- pass 1: row maxima over the valid keys (a row is spread over the 4 lanes of a quad)
     float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
     for (int kb = 0; kb < MAX_KB; ++kb) {
-      if (kb < nkb) {
+      if (kb < nkb_i) {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const bool valid = kb * KBLK + 8 * jj + cp + e < nk;
-            mx0 = fmaxf(mx0, valid ? S[kb][4 * jj + e] : -INFINITY);
-            mx1 = fmaxf(mx1, valid ? S[kb][4 * jj + 2 + e] : -INFINITY);
+            const int key = kb * KBLK + 8 * jj + cp + e;
+            mx0 = fmaxf(mx0, key < nk0 ? S[kb][4 * jj + e] : -INFINITY);
+            mx1 = fmaxf(mx1, key < nk1 ? S[kb][4 * jj + 2 + e] : -INFINITY);
           }
         }
       }
@@ -237,17 +248,17 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     float sum0 = 0.0f, sum1 = 0.0f;
 #pragma unroll
     for (int kb = 0; kb < MAX_KB; ++kb) {
-      if (kb < nkb) {
+      if (kb < nkb_i) {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
-            const bool valid = kb * KBLK + 8 * jj + cp + e < nk;
+            const int key = kb * KBLK + 8 * jj + cp + e;
             float e0, e1;
             asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e0) : "f"(fmaf(S[kb][4 * jj + e], sc, -mc0)));
             asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e1) : "f"(fmaf(S[kb][4 * jj + 2 + e], sc, -mc1)));
-            e0 = valid ? e0 : 0.0f;
-            e1 = valid ? e1 : 0.0f;
+            e0 = key < nk0 ? e0 : 0.0f;
+            e1 = key < nk1 ? e1 : 0.0f;
             S[kb][4 * jj + e] = e0; S[kb][4 * jj + 2 + e] = e1;
             sum0 += e0; sum1 += e1;
           }
@@ -259,7 +270,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     // ---- O = P V, block by block: P re-split to hi / lo fp16 A fragments, 16 keys per k-step
 #pragma unroll
     for (int kb = 0; kb < MAX_KB; ++kb) {
-      if (kb < nkb) {
+      if (kb < nkb_i) {
         uint32_t ph[4][4], pl[4][4];
 #pragma unroll
         for (int ks = 0; ks < 4; ++ks)
@@ -288,7 +299,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
         if (lane == 0) mbar_arrive(smem_u32(&r_empty[sl_i]));
       }
     }
-    rc += nkb;
+    rc += nkb_i;
 #pragma unroll
     for (int sl = 0; sl < NS; ++sl) acc_fence(O[sl]);
     tl_event(p.tl, tl_n, 34, j);                                       // O(j) ready
@@ -353,8 +364,10 @@ bool tc_attention_init(int device) {
     return false;
   g_encode = (PFN_tmapEncodeTiled)fn;
   cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, device);
-  if (cudaFuncSetAttribute(k_attn_tc<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(k_attn_tc<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
+  if (cudaFuncSetAttribute(k_attn_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+      cudaFuncSetAttribute(k_attn_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+      cudaFuncSetAttribute(k_attn_tc<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
+      cudaFuncSetAttribute(k_attn_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
     return false;
   g_ready = true;
   return true;
@@ -362,6 +375,7 @@ bool tc_attention_init(int device) {
 
 bool tc_attention_supported(const AttnArgs& a) {
   if (!g_ready || (a.hd != 64 && a.hd != 128) || a.Lq < 1 || a.Lk < 1 || a.Lk > 256 || a.nseq < 1) return false;
+  if (a.causal && a.Lq != a.Lk) return false;
   if ((a.q.cols % 8) || (a.kv.cols % 8) || (a.q_col0 % 8) || (a.k_col0 % 8) || (a.v_col0 % 8)) return false;
   if ((a.out.cols % 8) || ((uintptr_t)a.q.hi & 15) || ((uintptr_t)a.kv.hi & 15) || ((uintptr_t)a.out.hi & 15)) return false;
   if ((a.q.plane_stride % 8) || (a.kv.plane_stride % 8) || (a.out.plane_stride % 8)) return false;
@@ -393,9 +407,8 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   for (int k = 0; k < 8; ++k) if ((1 << k) == p.heads) p.heads_log2 = k;
   const int pairs = (p.items + 1) / 2;                 // two pipelines per CTA
   const int grid = pairs < g_sm_count ? pairs : g_sm_count;
-  if (a.hd == 64)
-    launch_pdl(k_attn_tc<64>, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
-  else
-    launch_pdl(k_attn_tc<128>, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
+  auto kernel = a.hd == 64 ? (a.causal ? k_attn_tc<64, true> : k_attn_tc<64, false>)
+                           : (a.causal ? k_attn_tc<128, true> : k_attn_tc<128, false>);
+  launch_pdl(kernel, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
   return true;
 }

@@ -48,6 +48,8 @@ __device__ __forceinline__ float gelu_fast(float x) {
   return 0.5f * x * (1.0f + copysignf(erf_abs, x));
 }
 __device__ __forceinline__ float silu_f(float x) { return x / (1.0f + expf(-x)); }
+// CLIP's quick-GELU x * sigmoid(1.702 x) (transformers ACT2FN["quick_gelu"])
+__device__ __forceinline__ float quick_gelu_f(float x) { return x / (1.0f + expf(-1.702f * x)); }
 
 // Programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization
 // attribute may begin (prologue: barrier init, descriptor prefetch) while its predecessor
@@ -84,13 +86,14 @@ static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 #endif
 
-enum ActKind { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3 };
+enum ActKind { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3, ACT_QUICKGELU = 4 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
   switch (act) {
     case ACT_GELU: return gelu_erf(v);
     case ACT_RELU: return fmaxf(v, 0.0f);
     case ACT_SILU: return silu_f(v);
+    case ACT_QUICKGELU: return quick_gelu_f(v);
     default: return v;
   }
 }

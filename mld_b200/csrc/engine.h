@@ -32,6 +32,27 @@ struct StackW {
   LnW norm;                // final norm (g == nullptr: none, ActorVae)
 };
 
+// CLIP text tower (mldb_text_configure): pre-norm layers, fused q|k|v operand
+struct TextLayerW {
+  LinW qkv, out, fc1, fc2;
+  LnW ln1, ln2;
+};
+struct TextW {
+  bool on = false;
+  mldb_text_config cfg{};
+  std::vector<TextLayerW> layers;
+  LnW final_ln;
+  LinW proj;                      // text_projection, no bias
+  float* tok = nullptr;           // token_embedding [vocab, hidden] fp32
+  float* pos = nullptr;           // position_embedding [max_positions, hidden] fp32
+  // workspace for `rows` tokens (grown on demand by mldb_text_encode)
+  int rows = 0, seqs = 0;
+  float* x = nullptr;             // [rows, hidden] fp32 residual stream
+  ActBuf a{}, qkv{}, att{}, h{};  // LN output, q|k|v, attention output, fc1 output (split16)
+  ActBuf pooled{};                // [seqs, hidden] final LN of the eos rows (split16, A of text_projection)
+  std::vector<void*> ws_allocs;
+};
+
 struct RawTensor {
   std::vector<float> host;
   std::vector<int64_t> shape;
@@ -101,6 +122,7 @@ struct mldb_handle {
   float* vae_enc_pe = nullptr;
   float* global_token = nullptr;     // [2*n_lat, d]
   float* mean = nullptr; float* stdv = nullptr; int nstat = 0;
+  TextW text;          // CLIP text tower (mldb_text_configure)
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;

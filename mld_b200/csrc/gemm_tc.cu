@@ -17,6 +17,7 @@
 //   generic:   + positional table, row remapping, zeroed padding rows, fp32 output, ragged N
 //   LayerNorm: BN == N == 256, so a quad owns COMPLETE rows: bias + residual, exact two-pass
 //              statistics over the registers with quad shuffles, normalise -> split16.
+//   residual:  bias + fp32 residual R -> fp32 (may run in place, out == R: the text tower's residual stream).
 #include "gemm_tc.h"
 
 #include <stdio.h>
@@ -37,6 +38,7 @@ constexpr int BM = 128, BK = 64;
 constexpr int NUM_THREADS = 384;                     // producer warpgroup + two consumer warpgroups
 constexpr int CONSUMER_WARPS = 8;
 constexpr int MAX_N = 1024;
+constexpr int MAX_N_WIDE = 4096;                     // GemmArgs::wide_n
 
 // ------------------------------------------------------------------------------ parameters
 struct TcParams {
@@ -48,6 +50,7 @@ struct TcParams {
   int act;
   __half* out_hi; __half* out_lo; int ld_out, out_col0;
   float* out_f32; int ldc;
+  const float* res_f32;                              // EPI_RES: [M, N] fp32, leading dimension ldc (may alias out_f32)
   int in_group, out_group, out_off;
   const int32_t* zero_lengths;
   // residual + LayerNorm epilogue
@@ -56,7 +59,7 @@ struct TcParams {
   long long* tl; // debug timeline (nullptr normally)
 };
 
-enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2 };     // epilogue variants of k_gemm_tc (see the kernel)
+enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2, EPI_RES = 3 };     // epilogue variants of k_gemm_tc (see the kernel)
 
 template <int BN>
 struct TileCfg {
@@ -157,8 +160,8 @@ __device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const flo
 // EPI selects the epilogue: EPI_FAST = plain, split16 output, identity row mapping, N a whole number of tiles
 // (the per-layer GEMMs); EPI_LN = residual + LayerNorm; EPI_GENERIC = plain with everything else (positional
 // table, row remapping, zeroed padding rows, fp32 output, ragged N: the per-batch embedding / final-layer
-// GEMMs) kept out of the hot kernels' instruction stream.
-template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast epilogue's activation (NONE | GELU)
+// GEMMs) kept out of the hot kernels' instruction stream; EPI_RES = bias + fp32 residual -> fp32, N even.
+template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast epilogue's activation (NONE | GELU | QUICKGELU)
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
           const __grid_constant__ CUtensorMap tmA2h, const __grid_constant__ CUtensorMap tmA2l,
@@ -283,8 +286,28 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
         float x0 = fmaf(d[4 * j], sc, b.x), x1 = fmaf(d[4 * j + 1], sc, b.y);
         float x2 = fmaf(d[4 * j + 2], sc, b.x), x3 = fmaf(d[4 * j + 3], sc, b.y);
         if (ACT == ACT_GELU) { x0 = gelu_fast(x0); x1 = gelu_fast(x1); x2 = gelu_fast(x2); x3 = gelu_fast(x3); }
+        if (ACT == ACT_QUICKGELU) {
+          x0 = quick_gelu_f(x0); x1 = quick_gelu_f(x1); x2 = quick_gelu_f(x2); x3 = quick_gelu_f(x3);
+        }
         if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x0, x1);
         if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x2, x3);
+      }
+    } else if constexpr (EPI == EPI_RES) {
+      // each element of R is read and then overwritten by the same thread: in place is safe (plain loads, no __ldg)
+      const float sc = p.inv_scale;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + cp;
+        if (n >= p.N) continue;                        // N even: a column pair is in or out together
+        const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (r_lo + 8 * h >= p.M) continue;
+          const int64_t o = (int64_t)(r_lo + 8 * h) * p.ldc + n;
+          const float2 r = *reinterpret_cast<const float2*>(p.res_f32 + o);
+          *reinterpret_cast<float2*>(p.out_f32 + o) =
+              make_float2(fmaf(d[4 * j + 2 * h], sc, b.x) + r.x, fmaf(d[4 * j + 2 * h + 1], sc, b.y) + r.y);
+        }
       }
     } else {
 #pragma unroll
@@ -616,6 +639,9 @@ TcCtx* tc_create(int device) {
   opt_in(k_gemm_tc<256, EPI_FAST>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_FAST, ACT_GELU>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST, ACT_GELU>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_GENERIC>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_GENERIC>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_FAST, ACT_QUICKGELU>, TileCfg<256>::SMEM_BYTES);
+  opt_in(k_gemm_tc<128, EPI_FAST, ACT_QUICKGELU>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_RES>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_RES>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_LN>, TileCfg<256>::SMEM_BYTES);
   opt_in(k_ffn_tc, FfnCfg::SMEM_BYTES);
   if (e != cudaSuccess) {
@@ -644,12 +670,16 @@ static int pick_bn(const GemmArgs& g) { return (g.w.N % 256 == 0) ? 256 : 128; }
 
 bool tc_gemm_supported(const TcCtx* c, const GemmArgs& g) {
   if (!c) return false;
-  if (g.a_kind != A_SPLIT || g.M < 1 || g.w.N > MAX_N) return false;
+  if (g.a_kind != A_SPLIT || g.M < 1 || g.w.N > (g.wide_n ? MAX_N_WIDE : MAX_N)) return false;
   if (g.K1 <= 0 || g.K1 % BK || g.K2 % BK || g.a1.cols != g.K1) return false;
   if (g.K2 > 0 && g.a2.cols != g.K2) return false;
   if (g.w.K != g.K1 + g.K2) return false;
   if (((uintptr_t)g.a1.hi & 15) || ((uintptr_t)g.w.w & 15)) return false;
   if (g.out.hi && ((g.out.cols % 8) || (g.out_col0 % 8))) return false;
+  if (g.res_f32 && (!g.out_f32 || g.out.hi || g.act != ACT_NONE || g.addtab || g.zero_lengths || g.in_group < g.M ||
+                    g.out_group != 0 || g.out_off != 0 || (g.w.N % 2) || (g.ldc % 2) || ((uintptr_t)g.out_f32 & 7) ||
+                    ((uintptr_t)g.res_f32 & 7)))
+    return false;
   return true;
 }
 
@@ -674,7 +704,7 @@ static void fill_params(const GemmArgs& g, const LnArgs* ln, int bn, TcParams* o
     p.gamma = ln->gamma; p.beta = ln->beta;
   } else {
     p.out_hi = g.out.hi; p.out_lo = g.out.hi ? g.out.lo() : nullptr; p.ld_out = g.out.cols; p.out_col0 = g.out_col0;
-    p.out_f32 = g.out_f32; p.ldc = g.ldc;
+    p.out_f32 = g.out_f32; p.ldc = g.ldc; p.res_f32 = g.res_f32;
   }
   p.m_tiles = (g.M + BM - 1) / BM;
   p.n_tiles = (g.w.N + bn - 1) / bn;
@@ -702,7 +732,7 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   // the fast plain epilogue: split16 output, identity row mapping, N a whole number of tiles
   const bool fast = !ln && g.out.hi && !g.out_f32 && !g.addtab && !g.zero_lengths && g.in_group >= g.M &&
                     g.out_group == 0 && g.out_off == 0 && g.w.N % bn == 0 && g.w.bias != nullptr &&
-                    (g.act == ACT_NONE || g.act == ACT_GELU);
+                    (g.act == ACT_NONE || g.act == ACT_GELU || g.act == ACT_QUICKGELU);
   const int ntiles = p.m_tiles * p.n_tiles;
   dim3 grid(ntiles < c->sm_count ? ntiles : c->sm_count);
 #define MLDB_LAUNCH(BN_, ...)                                                                                      \
@@ -713,7 +743,9 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
     if (bn == 256) MLDB_LAUNCH(256, __VA_ARGS__); else MLDB_LAUNCH(128, __VA_ARGS__); \
   } while (0)
   if (ln)                             MLDB_LAUNCH(256, EPI_LN);
+  else if (g.res_f32)                 MLDB_LAUNCH_SHAPE(EPI_RES);
   else if (fast && g.act == ACT_GELU) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_GELU);
+  else if (fast && g.act == ACT_QUICKGELU) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_QUICKGELU);
   else if (fast)                      MLDB_LAUNCH_SHAPE(EPI_FAST);
   else                                MLDB_LAUNCH_SHAPE(EPI_GENERIC);
 #undef MLDB_LAUNCH_SHAPE

@@ -34,6 +34,11 @@ struct GemmArgs {
   int in_group = 1 << 30, out_group = 0, out_off = 0;
   const float* addtab = nullptr;        // [*, N]: row (out_off + r % in_group)
   const int32_t* zero_lengths = nullptr;  // zero rows with (r % in_group) >= zero_lengths[r / in_group]
+  // residual add: out_f32[r, n] = act(...) + res_f32[r * ldc + n] (fp32 [M, N], leading dimension ldc; may alias
+  // out_f32, which is how the CLIP text tower updates its fp32 residual stream in place)
+  const float* res_f32 = nullptr;
+  int wide_n = 0;                       // 1: the wgmma kernel may take N up to 4096 (the text tower's 2304 / 3072);
+                                        // the sampling path keeps its N <= 1024 kernel selection
 };
 
 // y = LayerNorm(c + res + rowvec[r / rv_group]) * gamma + beta, eps 1e-5; optional second LN
@@ -60,6 +65,7 @@ struct AttnArgs {
   int kv_prefix = 0;
   int len_mod = 0;                    // lengths index = (seq0 + s) % len_mod when len_mod > 0
   int seq0 = 0;                       // global index of this launch's first sequence (chunked launches)
+  int causal = 0;                     // 1: query i attends to keys j <= i only (self-attention, Lq == Lk)
   ActBuf out{};                       // [nseq*Lq, heads*hd]
 };
 
@@ -76,5 +82,24 @@ bool tc_attention_init(int device);                       // once per process, o
 bool tc_attention_supported(const AttnArgs& a);
 bool tc_attention(const AttnArgs& a, cudaStream_t st);    // false: tensor-map encoding failed, nothing launched
 void simt_init();
+// --- CLIP text tower row kernels (text_ln.cu) ---
+// One warp per row, d a multiple of 128 up to 1024, exact two-pass statistics, no shared memory.
+//   TEXT_LN_ROWS:  out = LN(x[r])                                   (pre-norm LN1 / LN2, final LN of every row)
+//   TEXT_LN_EMBED: x[r] = tok[ids[r]] + pos[r % L]; out = LN(x[r])  (layer 0; an id outside [0, vocab) -> NaN row)
+//   TEXT_LN_EOS:   out[s] = LN(x[s * L + eos_pos(ids[s, :])])       (pooled mode: only the gathered rows)
+enum TextLnMode { TEXT_LN_ROWS = 0, TEXT_LN_EMBED = 1, TEXT_LN_EOS = 2 };
+struct TextLnArgs {
+  int mode = TEXT_LN_ROWS;
+  float* x = nullptr;                 // fp32 residual stream [rows, d] (written in TEXT_LN_EMBED, read otherwise)
+  const int64_t* ids = nullptr; int L = 0;
+  const float* tok = nullptr; const float* pos = nullptr; int vocab = 0;
+  int eos_id = 0;                     // eos_id == 2: eos_pos = argmax(ids) (legacy configs); else first id == eos_id, or 0
+  const float* gamma = nullptr; const float* beta = nullptr; float eps = 1e-5f;
+  int M = 0, d = 0;                   // output rows (TEXT_LN_EOS: sequences)
+  ActBuf out{};                       // split16 output (nullable)
+  float* out_f32 = nullptr;           // fp32 output [M, d] (nullable)
+};
+bool text_ln_supported(int d);
+void text_ln(const TextLnArgs& a, cudaStream_t st);
 // --- wgmma implementations (gemm_tc.cu) ---
 struct TcCtx;

@@ -86,6 +86,7 @@ __global__ void __launch_bounds__(256) k_gemm_simt(const GemmArgs a) {
       if (a.addtab) v += a.addtab[(int64_t)(a.out_off + pos) * N + n];
       v = apply_act(v, a.act);
       if (zero) v = 0.0f;
+      if (a.res_f32) v += a.res_f32[orow * a.ldc + n];   // the same thread reads and writes: may run in place
       if (a.out.hi) {
         __half h, l;
         split_f32(v, h, l);
@@ -176,7 +177,8 @@ __global__ void __launch_bounds__(256) k_ln(const LnArgs a) {
 // ------------------------------------------------------------------------------- attention
 // One block per (sequence, head).  K (padded rows) and V live in shared memory as fp32; each
 // warp owns query rows q = warp, warp + nwarps, ...  Softmax over the valid keys only (the
-// reference masks padded keys with -inf: cross_attention.py:264-266, mld_vae.py:226-232).
+// reference masks padded keys with -inf: cross_attention.py:264-266, mld_vae.py:226-232); with a.causal set,
+// query qi sees keys 0..qi only (CLIP's causal mask).
 constexpr int ATT_WARPS = 8;
 
 __global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) {
@@ -214,8 +216,9 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) 
       qv[d] = join_f32(a.q.hi[o], a.q.lo()[o]) * scale;
     }
     __syncwarp();
+    const int nkq = a.causal ? min(nk, qi + 1) : nk;   // causal: keys j <= qi
     float mx = -INFINITY;
-    for (int t = lane; t < nk; t += 32) {
+    for (int t = lane; t < nkq; t += 32) {
       const float* kr = Ks + t * (hd + 1);
       float acc = 0.0f;
 #pragma unroll 8
@@ -225,7 +228,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) 
     }
     mx = warp_max(mx);
     float sum = 0.0f;
-    for (int t = lane; t < nk; t += 32) {
+    for (int t = lane; t < nkq; t += 32) {
       float e = expf(pv[t] - mx);
       pv[t] = e;
       sum += e;
@@ -235,7 +238,7 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) 
     __syncwarp();
     for (int d = lane; d < hd; d += 32) {
       float acc = 0.0f;
-      for (int t = 0; t < nk; ++t) acc = fmaf(pv[t], Vs[t * hd + d], acc);
+      for (int t = 0; t < nkq; ++t) acc = fmaf(pv[t], Vs[t * hd + d], acc);
       acc *= inv;
       __half hh, ll;
       split_f32(acc, hh, ll);

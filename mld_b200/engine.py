@@ -84,8 +84,10 @@ class Engine:
         check(self.lib.mldb_profile_steps(self._h, _ptr(c), _ptr(z0), B, S, ms), "mldb_profile_steps")
         return [float(v) for v in ms]
 
-    def debug_gemm(self, A, W, bias=None, gamma=None, beta=None, R=None, K1=0, act=0, use_tc=True, split_out=False):
-        """Kernel unit-test hook (mldb_debug_gemm): A [M,K] (device), W [N,K] / bias / gamma / beta (host)."""
+    def debug_gemm(self, A, W, bias=None, gamma=None, beta=None, R=None, K1=0, act=0, use_tc=True, split_out=False,
+                   in_place=False):
+        """Kernel unit-test hook (mldb_debug_gemm): A [M,K] (device), W [N,K] / bias / gamma / beta (host).
+        ``R`` without ``gamma``: the residual-add epilogue A W^T + b + R; ``in_place`` runs it with out == R."""
         A = _f32c(A, self.device)
         Wc = W.detach().float().contiguous().cpu()
         host = [None if t is None else t.detach().float().contiguous().cpu() for t in (bias, gamma, beta)]
@@ -93,6 +95,10 @@ class Engine:
         M, K = A.shape
         N = Wc.shape[0]
         out = torch.empty((M, N), dtype=torch.float32, device=self.device)
+        if in_place:
+            if Rd is None or gamma is not None:
+                raise ValueError("in_place needs R and no gamma (the residual-add epilogue)")
+            out = Rd = Rd.clone()
         check(self.lib.mldb_debug_gemm(self._h, _ptr(A), _ptr(Wc), _ptr(host[0]), _ptr(host[1]), _ptr(host[2]),
                                        _ptr(Rd), M, N, K, K1, act, int(use_tc), int(split_out), _ptr(out), self._stream()),
               "mldb_debug_gemm")
@@ -110,10 +116,12 @@ class Engine:
                                       self._stream()), "mldb_debug_ffn")
         return out
 
-    def debug_attention(self, q, nseq, Lq, heads, lengths=None, mode=2, kv=None, Lk=None, kv_prefix=0):
+    def debug_attention(self, q, nseq, Lq, heads, lengths=None, mode=2, kv=None, Lk=None, kv_prefix=0,
+                        causal=False):
         """Kernel unit-test hook (mldb_debug_attention).  ``kv is None``: ``q`` is a packed qkv
         [nseq*Lq, 3*heads*hd] tensor (self-attention, the layout the stacks use); else ``q`` [nseq*Lq, d] and
         ``kv`` [nseq*Lk, 2*d] (cross-attention).  mode 0 CUDA-core, 1 mma.sync, 2 wgmma (product).
+        ``causal``: query i attends to keys j <= i (mldb_debug_attention_causal; self-attention only).
         Returns [nseq*Lq, heads*hd]."""
         q = _f32c(q, self.device)
         kvd = None if kv is None else _f32c(kv, self.device)
@@ -123,8 +131,33 @@ class Engine:
             raise ValueError("debug_attention: shape mismatch")
         ln = None if lengths is None else torch.as_tensor(lengths, dtype=torch.int32, device=self.device).contiguous()
         out = torch.empty((nseq * Lq, d), dtype=torch.float32, device=self.device)
-        check(self.lib.mldb_debug_attention(self._h, _ptr(q), _ptr(kvd), _ptr(ln), int(kv_prefix), nseq, Lq, Lk, heads,
-                                            d // heads, int(mode), _ptr(out), self._stream()), "mldb_debug_attention")
+        fn = self.lib.mldb_debug_attention_causal if causal else self.lib.mldb_debug_attention
+        check(fn(self._h, _ptr(q), _ptr(kvd), _ptr(ln), int(kv_prefix), nseq, Lq, Lk, heads, d // heads, int(mode),
+                 _ptr(out), self._stream()), "mldb_debug_attention")
+        return out
+
+    # ------------------------------------------------------------------ CLIP text tower
+    def text_configure(self, tcfg):
+        """Add the text tower's keys (``text_encoder.`` prefix) to the strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_text_configure(self._h, C.byref(tcfg)), "mldb_text_configure")
+        self.text_cfg = tcfg
+
+    def text_encode(self, ids: torch.Tensor, mode: int = _lib.TEXT_POOLED) -> torch.Tensor:
+        """int64 token ids [n, L] -> last_hidden_state [n, L, hidden] (TEXT_HIDDEN) or get_text_features [n, proj]
+        (TEXT_POOLED), on the current stream.  Ids outside the vocabulary are rejected here, before the launch."""
+        tc = getattr(self, "text_cfg", None)
+        if tc is None:
+            raise RuntimeError("text_configure() was not called before finalize()")
+        if ids.dim() != 2 or ids.shape[0] < 1 or not 1 <= ids.shape[1] <= tc.max_positions:
+            raise ValueError(f"ids must be [n, L] with 1 <= L <= {tc.max_positions}, got {tuple(ids.shape)}")
+        if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= tc.vocab_size):
+            raise ValueError(f"token ids must lie in [0, {tc.vocab_size})")
+        d_ids = ids.to(device=self.device, dtype=torch.int64).contiguous()
+        n, L = d_ids.shape
+        shape = (n, L, tc.hidden) if mode == _lib.TEXT_HIDDEN else (n, tc.projection_dim)
+        out = torch.empty(shape, dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_text_encode(self._h, _ptr(d_ids), n, L, int(mode), _ptr(out), self._stream()),
+              "mldb_text_encode")
         return out
 
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:

@@ -45,6 +45,9 @@ class _EngineModule(nn.Module):
     def _make_config(self):
         raise NotImplementedError
 
+    def _configure_engine(self, eng: Engine):
+        """Hook between mldb_create and the weight upload (the text encoder adds its key spec here)."""
+
     def _load_from_state_dict(self, *args, **kwargs):   # weights changed -> rebuild engine
         self._weights_epoch += 1
         return super()._load_from_state_dict(*args, **kwargs)
@@ -60,6 +63,7 @@ class _EngineModule(nn.Module):
                                "(no CPU/PyTorch fallback exists)")
         if self._engine is None or self._engine_epoch != self._weights_epoch or self._engine.device != dev:
             eng = Engine(self._make_config(), dev)
+            self._configure_engine(eng)
             eng.load_state_dict(self.state_dict(), self._prefix)
             eng.finalize()
             self._engine, self._engine_epoch = eng, self._weights_epoch

@@ -9,8 +9,8 @@ and a scheduler object with the diffusers surface the reference touches
 (``init_noise_sigma``, ``set_timesteps``, ``timesteps``, ``step(...).prev_sample``,
 ``config.num_train_timesteps``; mld.py:310-320,345).
 
-The text encoder is NOT part of this path (frozen CLIP, SURVEY.md section 8f): pass any callable
-``text_encoder(List[str]) -> Tensor[2B, S, 768]`` (e.g. the reference's ``MldTextEncoder``).
+The text encoder is a separate callable ``text_encoder(List[str]) -> Tensor[2B, S, 768]``: the native
+``mld_b200.text.B200TextEncoder`` (CLIP on this library's kernels) or the reference's ``MldTextEncoder``.
 """
 from __future__ import annotations
 

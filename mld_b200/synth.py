@@ -197,3 +197,42 @@ def mean_std(nfeats: int = 263, seed: int = 5):
         mean[4:4 + n_ric] = torch.randn(n_ric, generator=g) * 0.3
         std[4:4 + n_ric] = 0.1 + 0.2 * torch.rand(n_ric, generator=g)
     return mean, std
+
+
+def clip_text_state_dict(seed: int = 4242, vocab_size: int = 49408, max_positions: int = 77, hidden: int = 768,
+                         layers: int = 12, ff: int = 3072, projection_dim: int = 768, **_unused) -> Dict[str, Tensor]:
+    """State dict of the CLIP text tower as ``MldTextEncoder.state_dict()`` names it (mld_clip.py:26-27: its
+    ``text_model`` is a ``CLIPModel``): ``text_model.text_model.*`` and ``text_model.text_projection.weight``.
+    Stripping the leading ``text_model.`` gives the keys of transformers' ``CLIPTextModelWithProjection``.  The
+    default shape is CLIP ViT-L/14's text tower; smaller shapes are for fast tests (``heads`` does not change the
+    weights and is accepted for symmetry with the text config)."""
+    g, sd = _Gen(seed), {}
+    p = "text_model.text_model."
+    sd[p + "embeddings.token_embedding.weight"] = g.normal(vocab_size, hidden, std=0.02)
+    sd[p + "embeddings.position_embedding.weight"] = g.normal(max_positions, hidden, std=0.01)
+    for i in range(layers):
+        q = f"{p}encoder.layers.{i}."
+        for name in ("k_proj", "v_proj", "q_proj", "out_proj"):
+            sd[f"{q}self_attn.{name}.weight"] = g.xavier(hidden, hidden)
+            sd[f"{q}self_attn.{name}.bias"] = g.normal(hidden, std=0.02)
+        _ln(sd, g, q + "layer_norm1.", hidden)
+        sd[q + "mlp.fc1.weight"] = g.xavier(ff, hidden)
+        sd[q + "mlp.fc1.bias"] = g.normal(ff, std=0.02)
+        sd[q + "mlp.fc2.weight"] = g.xavier(hidden, ff)
+        sd[q + "mlp.fc2.bias"] = g.normal(hidden, std=0.02)
+        _ln(sd, g, q + "layer_norm2.", hidden)
+    _ln(sd, g, p + "final_layer_norm.", hidden)
+    sd["text_model.text_projection.weight"] = g.xavier(projection_dim, hidden)
+    return sd
+
+
+def clip_text_ids(n: int, L: int = 77, seed: int = 7, eos_lo: int = 8, eos_hi: int = 30, vocab_size: int = 49408,
+                  bos: int = 49406, eos: int = 49407) -> Tensor:
+    """Tokenizer-shaped id rows ``[n, L]`` (int64): bos, random word ids, eos at a seeded position in
+    [eos_lo, eos_hi], then eos padding (CLIP's pad token is its eos token)."""
+    g = torch.Generator().manual_seed(seed)
+    ids = torch.randint(0, min(bos, vocab_size), (n, L), generator=g)
+    pos = torch.randint(eos_lo, eos_hi + 1, (n,), generator=g).clamp(max=L - 1)
+    ids[:, 0] = bos
+    ids[torch.arange(L).expand(n, L) >= pos[:, None]] = eos
+    return ids
