@@ -381,7 +381,10 @@ static void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st) {
     mma_attention(a, st);
     kcount(h, MLDB_KSTAT_ATTN_MMA);
   } else {
-    simt_attention(a, st);
+    if (!simt_attention(a, st)) {
+      mldb_set_err("CUDA-core attention: head_dim " + std::to_string(a.hd) + " does not fit shared memory");
+      h->op_failed = true;
+    }
     kcount(h, MLDB_KSTAT_ATTN_SIMT);
   }
 }
@@ -615,6 +618,10 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   if (cfg->abi_version != MLDB_ABI_VERSION) FAIL(MLDB_ERR_INVALID, "abi_version mismatch");
   if (cfg->latent_dim % cfg->num_heads || cfg->latent_dim % 32) FAIL(MLDB_ERR_INVALID, "latent_dim must be a multiple of 32 and of num_heads");
   if (cfg->latent_dim > 1024) FAIL(MLDB_ERR_UNSUPPORTED, "latent_dim > 1024");
+  // every attention shape must have a kernel: the CUDA-core core takes any length, but not any head width
+  for (int heads : {cfg->num_heads, cfg->vae_heads})
+    if (heads > 0 && !simt_attention_supported(cfg->latent_dim / heads))
+      FAIL(MLDB_ERR_UNSUPPORTED, "head_dim %d is too wide for the attention kernels", cfg->latent_dim / heads);
   if (cfg->arch == MLDB_ARCH_TRANS_ENC && cfg->num_layers > 0 && cfg->num_layers % 2 != 1) FAIL(MLDB_ERR_INVALID, "skip encoder needs an odd layer count");
   if (cfg->arch == MLDB_ARCH_TRANS_ENC && cfg->diffusion_only) FAIL(MLDB_ERR_UNSUPPORTED, "diffusion_only requires arch trans_dec");
   if (cfg->vae_kind == MLDB_VAE_MLD && cfg->vae_layers % 2 != 1) FAIL(MLDB_ERR_INVALID, "MldVae needs an odd layer count");
@@ -765,6 +772,8 @@ extern "C" int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg) 
     FAIL(MLDB_ERR_INVALID, "bad text config");
   if (!text_ln_supported(c.hidden) || c.hidden % c.heads)
     FAIL(MLDB_ERR_UNSUPPORTED, "text hidden size %d: must be a multiple of 128 (<= 1024) and of heads", c.hidden);
+  if (!simt_attention_supported(c.hidden / c.heads))
+    FAIL(MLDB_ERR_UNSUPPORTED, "text head_dim %d is too wide for the attention kernels", c.hidden / c.heads);
   if (c.max_positions < 1 || c.max_positions > 256) FAIL(MLDB_ERR_UNSUPPORTED, "max_positions must lie in [1, 256]");
   const std::string T = kTextPrefix, M = T + "text_model.";
   const int d = c.hidden;
@@ -1017,7 +1026,10 @@ static int run_graphed(mldb_handle* h, Plan* p, cudaStream_t st, F record) {
       e = cudaStreamEndCapture(h->cap_stream, &graph);
     }
     h->capturing = false;
-    if (e != cudaSuccess) FAIL(MLDB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+    if (e != cudaSuccess) {
+      (void)cudaGetLastError();   // the launch error that broke the capture must not fail the next, unrelated call
+      FAIL(MLDB_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
+    }
     if (h->op_failed) { cudaGraphDestroy(graph); return check_ops(h); }
     e = cudaGraphInstantiate(&p->exec, graph, 0);
     cudaGraphDestroy(graph);
@@ -1542,7 +1554,7 @@ static int run_f2j(mldb_handle* h, const float* feats, int B, int T, float* join
   const int F = c.vae_kind != MLDB_VAE_NONE ? c.vae_nfeats : c.nfeats;
   if (!h->mean || h->nstat != F) FAIL(MLDB_ERR_STATE, "call mldb_set_mean_std with %d features first", F);
   if (F < 4 + (c.njoints - 1) * 3) FAIL(MLDB_ERR_UNSUPPORTED, "feats2joints needs the HumanML3D/KIT layout");
-  k_feats2joints<<<B, 256, (size_t)4 * T * sizeof(float), st>>>(feats, h->mean, h->stdv, T, F, c.njoints, joints);
+  k_feats2joints<<<B, 256, 0, st>>>(feats, h->mean, h->stdv, T, F, c.njoints, joints);
   kcount(h, MLDB_KSTAT_MISC);
   CK(cudaGetLastError());
   return MLDB_OK;
@@ -1952,7 +1964,7 @@ static int debug_attention(mldb_handle* h, const float* Q, const float* KV, cons
   a.nseq = nseq; a.heads = heads; a.hd = hd; a.lengths = lengths; a.kv_prefix = kv_prefix; a.out = o;
   a.causal = causal;
   int rc = MLDB_OK;
-  if (mode == 0) simt_attention(a, st);
+  if (mode == 0 && simt_attention_supported(hd)) { if (!simt_attention(a, st)) rc = MLDB_ERR_UNSUPPORTED; }
   else if (mode == 1 && mma_attention_supported(a)) mma_attention(a, st);
   else if (mode == 2 && tc_attention_supported(a)) { if (!tc_attention(a, st)) rc = MLDB_ERR_CUDA; }
   else rc = MLDB_ERR_UNSUPPORTED;

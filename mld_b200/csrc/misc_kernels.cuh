@@ -196,74 +196,81 @@ static __global__ void k_sched_step(const float* __restrict__ eps, const float* 
 }
 
 // feats2joints (mld/data/HumanML3D.py:41-45 -> motion_process.py:415-431, 362-381;
-// quaternion.py:16-20, 54-73).  One block per motion.  Thread 0 performs the two sequential
-// fp32 prefix sums in the reference's order (torch.cumsum on CPU is a serial sum), all threads
-// then rotate the rotation-invariant joint coordinates into the global frame.
+// quaternion.py:16-20, 54-73).  One block per motion, frames in chunks of F2J_CHUNK.  Per chunk,
+// thread 0 continues the two sequential fp32 prefix sums in the reference's order (torch.cumsum on CPU
+// is a serial sum), then all threads rotate the chunk's rotation-invariant joint coordinates into the
+// global frame.  The chunking bounds the shared memory at any motion length.
 //   feats [B, T, F] normalised; joints [B, T, J, 3]
+constexpr int F2J_CHUNK = 1024;
 static __global__ void __launch_bounds__(256) k_feats2joints(const float* __restrict__ feats,
                                                       const float* __restrict__ mean,
                                                       const float* __restrict__ stdv, int T, int F,
                                                       int J, float* __restrict__ joints) {
-  extern __shared__ float sm[];
-  float* cs = sm;           // cos(angle)[T]
-  float* sn = cs + T;       // sin(angle)[T]
-  float* px = sn + T;       // root x [T]
-  float* pz = px + T;       // root z [T]
+  __shared__ float cs[F2J_CHUNK];   // cos(angle)
+  __shared__ float sn[F2J_CHUNK];   // sin(angle)
+  __shared__ float px[F2J_CHUNK];   // root x
+  __shared__ float pz[F2J_CHUNK];   // root z
   const int b = blockIdx.x;
   const float* f = feats + (int64_t)b * T * F;
-  if (threadIdx.x == 0) {
-    // r_rot_ang[t] = sum_{u<t} rot_vel[u]; quaternion q = (cos, 0, sin, 0); r_pos accumulates
-    // qrot(qinv(q[t]), (vx[t-1], 0, vz[t-1])).
-    float ang = 0.0f, ax = 0.0f, az = 0.0f;
-    for (int t = 0; t < T; ++t) {
-      float vx = 0.0f, vz = 0.0f;
-      if (t > 0) {
-        const float* fp = f + (int64_t)(t - 1) * F;
-        ang = __fadd_rn(ang, __fadd_rn(__fmul_rn(fp[0], stdv[0]), mean[0]));
-        vx = __fadd_rn(__fmul_rn(fp[1], stdv[1]), mean[1]);
-        vz = __fadd_rn(__fmul_rn(fp[2], stdv[2]), mean[2]);
-      }
-      const float c = cosf(ang), s = sinf(ang);
-      cs[t] = c;
-      sn[t] = s;
-      // qrot with q = (w=c, x=0, y=-s, z=0) on v=(vx,0,vz):
-      //   uv = cross(qvec, v) = (-s*vz, 0, s*vx); uuv = cross(qvec, uv) = (-s*s*vx, 0, -s*s*vz)
-      //   out = v + 2*(w*uv + uuv)
-      const float uvx = -s * vz, uvz = s * vx;
-      const float uuvx = -s * uvz, uuvz = s * uvx;
-      const float rx = vx + 2.0f * (c * uvx + uuvx);
-      const float rz = vz + 2.0f * (c * uvz + uuvz);
-      ax = __fadd_rn(ax, rx);
-      az = __fadd_rn(az, rz);
-      px[t] = ax;
-      pz[t] = az;
-    }
-  }
-  __syncthreads();
   float* out = joints + (int64_t)b * T * J * 3;
-  for (int i = threadIdx.x; i < T * J; i += blockDim.x) {
-    const int t = i / J, j = i - t * J;
-    const float* fp = f + (int64_t)t * F;
-    float x, y, z;
-    if (j == 0) {
-      x = px[t];
-      y = fp[3] * stdv[3] + mean[3];
-      z = pz[t];
-    } else {
-      const int o = 4 + (j - 1) * 3;
-      const float vx = fp[o] * stdv[o] + mean[o];
-      const float vy = fp[o + 1] * stdv[o + 1] + mean[o + 1];
-      const float vz = fp[o + 2] * stdv[o + 2] + mean[o + 2];
-      const float c = cs[t], s = sn[t];
-      // qvec = (0, -s, 0): uv = cross(qvec, v) = (-s*vz, 0, s*vx)
-      const float uvx = -s * vz, uvz = s * vx;
-      const float uuvx = -s * uvz, uuvz = s * uvx;
-      x = vx + 2.0f * (c * uvx + uuvx) + px[t];
-      y = vy;
-      z = vz + 2.0f * (c * uvz + uuvz) + pz[t];
+  float ang = 0.0f, ax = 0.0f, az = 0.0f;   // thread 0's running sums across chunks
+  for (int t0 = 0; t0 < T; t0 += F2J_CHUNK) {
+    const int n = min(F2J_CHUNK, T - t0);
+    if (threadIdx.x == 0) {
+      // r_rot_ang[t] = sum_{u<t} rot_vel[u]; quaternion q = (cos, 0, sin, 0); r_pos accumulates
+      // qrot(qinv(q[t]), (vx[t-1], 0, vz[t-1])).
+      for (int u = 0; u < n; ++u) {
+        const int t = t0 + u;
+        float vx = 0.0f, vz = 0.0f;
+        if (t > 0) {
+          const float* fp = f + (int64_t)(t - 1) * F;
+          ang = __fadd_rn(ang, __fadd_rn(__fmul_rn(fp[0], stdv[0]), mean[0]));
+          vx = __fadd_rn(__fmul_rn(fp[1], stdv[1]), mean[1]);
+          vz = __fadd_rn(__fmul_rn(fp[2], stdv[2]), mean[2]);
+        }
+        const float c = cosf(ang), s = sinf(ang);
+        cs[u] = c;
+        sn[u] = s;
+        // qrot with q = (w=c, x=0, y=-s, z=0) on v=(vx,0,vz):
+        //   uv = cross(qvec, v) = (-s*vz, 0, s*vx); uuv = cross(qvec, uv) = (-s*s*vx, 0, -s*s*vz)
+        //   out = v + 2*(w*uv + uuv)
+        const float uvx = -s * vz, uvz = s * vx;
+        const float uuvx = -s * uvz, uuvz = s * uvx;
+        const float rx = vx + 2.0f * (c * uvx + uuvx);
+        const float rz = vz + 2.0f * (c * uvz + uuvz);
+        ax = __fadd_rn(ax, rx);
+        az = __fadd_rn(az, rz);
+        px[u] = ax;
+        pz[u] = az;
+      }
     }
-    out[(int64_t)i * 3 + 0] = x;
-    out[(int64_t)i * 3 + 1] = y;
-    out[(int64_t)i * 3 + 2] = z;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n * J; i += blockDim.x) {
+      const int u = i / J, j = i - u * J;
+      const float* fp = f + (int64_t)(t0 + u) * F;
+      float x, y, z;
+      if (j == 0) {
+        x = px[u];
+        y = fp[3] * stdv[3] + mean[3];
+        z = pz[u];
+      } else {
+        const int o = 4 + (j - 1) * 3;
+        const float vx = fp[o] * stdv[o] + mean[o];
+        const float vy = fp[o + 1] * stdv[o + 1] + mean[o + 1];
+        const float vz = fp[o + 2] * stdv[o + 2] + mean[o + 2];
+        const float c = cs[u], s = sn[u];
+        // qvec = (0, -s, 0): uv = cross(qvec, v) = (-s*vz, 0, s*vx)
+        const float uvx = -s * vz, uvz = s * vx;
+        const float uuvx = -s * uvz, uuvz = s * uvx;
+        x = vx + 2.0f * (c * uvx + uuvx) + px[u];
+        y = vy;
+        z = vz + 2.0f * (c * uvz + uuvz) + pz[u];
+      }
+      const int64_t oi = (int64_t)t0 * J + i;
+      out[oi * 3 + 0] = x;
+      out[oi * 3 + 1] = y;
+      out[oi * 3 + 2] = z;
+    }
+    __syncthreads();                        // the next chunk overwrites the tables
   }
 }

@@ -72,7 +72,10 @@ struct AttnArgs {
 // --- SIMT implementations (simt.cu) ---
 void simt_gemm(const GemmArgs& a, cudaStream_t st);
 void simt_ln(const LnArgs& a, cudaStream_t st);
-void simt_attention(const AttnArgs& a, cudaStream_t st);
+// CUDA-core attention: any Lq / Lk (K and V stream through shared memory in key chunks).  false: the head is too
+// wide for the shared memory (simt_attention_supported), nothing launched.
+bool simt_attention(const AttnArgs& a, cudaStream_t st);
+bool simt_attention_supported(int hd);
 // --- mma.sync tensor-core attention (attn_mma.cu) ---
 bool mma_attention_supported(const AttnArgs& a);
 void mma_attention_init();

@@ -175,13 +175,19 @@ __global__ void __launch_bounds__(256) k_ln(const LnArgs a) {
 }
 
 // ------------------------------------------------------------------------------- attention
-// One block per (sequence, head).  K (padded rows) and V live in shared memory as fp32; each
-// warp owns query rows q = warp, warp + nwarps, ...  Softmax over the valid keys only (the
-// reference masks padded keys with -inf: cross_attention.py:264-266, mld_vae.py:226-232); with a.causal set,
-// query qi sees keys 0..qi only (CLIP's causal mask).
+// One block per (sequence, head); each warp owns query rows q = warp, warp + nwarps, ...  Softmax over
+// the valid keys only (the reference masks padded keys with -inf: cross_attention.py:264-266,
+// mld_vae.py:226-232); with a.causal set, query qi sees keys 0..qi only (CLIP's causal mask).
+// K and V pass through shared memory as fp32 in chunks of kc keys.  When every valid key fits one chunk
+// (kc >= nk, the common case) K and V are loaded once and the scores of pass 1 are kept for pass 2.
+// Otherwise the warps step through their query rows together, one row per warp at a time, and stream
+// the chunks twice: pass 1 takes the row maximum, pass 2 recomputes the scores, exponentiates and
+// accumulates P V.  The per-warp output row lives in shared memory between chunks.  Both ways give the
+// same exact two-pass softmax, summed in the same order.
 constexpr int ATT_WARPS = 8;
+constexpr size_t ATT_SMEM_MAX = 227 * 1024;   // the opt-in set in simt_init
 
-__global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) {
+__global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a, const int kc) {
   extern __shared__ float sm[];
   const int s = blockIdx.x / a.heads, h = blockIdx.x % a.heads;
   const int hd = a.hd, Lk = a.Lk, Lq = a.Lq;
@@ -190,63 +196,106 @@ __global__ void __launch_bounds__(ATT_WARPS * 32) k_attn_simt(const AttnArgs a) 
     const int li = a.len_mod > 0 ? (a.seq0 + s) % a.len_mod : s;
     nk = min(Lk, a.kv_prefix + a.lengths[li]);
   }
-  float* Ks = sm;                          // [Lk][hd+1]
-  float* Vs = Ks + (size_t)Lk * (hd + 1);  // [Lk][hd]
-  float* Qs = Vs + (size_t)Lk * hd;        // [ATT_WARPS][hd]
-  float* Ps = Qs + ATT_WARPS * hd;         // [ATT_WARPS][Lk]
+  float* Ks = sm;                          // [kc][hd+1]
+  float* Vs = Ks + (size_t)kc * (hd + 1);  // [kc][hd]
+  float* Qs = Vs + (size_t)kc * hd;        // [ATT_WARPS][hd]
+  float* Ps = Qs + ATT_WARPS * hd;         // [ATT_WARPS][kc]
+  float* Os = Ps + ATT_WARPS * kc;         // [ATT_WARPS][hd], only when kc < Lk
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const __half* khi = a.kv.hi;
   const __half* klo = a.kv.lo();
-  for (int i = tid; i < nk * hd; i += blockDim.x) {
-    const int t = i / hd, d = i - t * hd;
-    const int64_t row = (int64_t)s * Lk + t;
-    int64_t ok = row * a.kv.cols + a.k_col0 + h * hd + d;
-    int64_t ov = row * a.kv.cols + a.v_col0 + h * hd + d;
-    Ks[t * (hd + 1) + d] = join_f32(khi[ok], klo[ok]);
-    Vs[t * hd + d] = join_f32(khi[ov], klo[ov]);
+  auto load = [&](int c0, int c1, bool with_v) {   // keys [c0, c1) -> chunk rows [0, c1 - c0)
+    for (int i = tid; i < (c1 - c0) * hd; i += blockDim.x) {
+      const int t = i / hd, d = i - t * hd;
+      const int64_t row = (int64_t)s * Lk + c0 + t;
+      int64_t ok = row * a.kv.cols + a.k_col0 + h * hd + d;
+      Ks[t * (hd + 1) + d] = join_f32(khi[ok], klo[ok]);
+      if (with_v) {
+        int64_t ov = row * a.kv.cols + a.v_col0 + h * hd + d;
+        Vs[t * hd + d] = join_f32(khi[ov], klo[ov]);
+      }
+    }
+  };
+  const bool resident = nk <= kc;
+  if (resident) {
+    load(0, nk, true);
+    __syncthreads();
   }
-  __syncthreads();
   const float scale = rsqrtf((float)hd);
   float* qv = Qs + warp * hd;
-  float* pv = Ps + warp * Lk;
-  for (int qi = warp; qi < Lq; qi += ATT_WARPS) {
+  float* pv = Ps + warp * kc;
+  float* ov = Os + warp * hd;
+  // block-uniform trip counts: every warp reaches every __syncthreads of the streamed chunks
+  for (int q0 = 0; q0 < Lq; q0 += ATT_WARPS) {
+    const int qi = q0 + warp;
+    const bool active = qi < Lq;
     const int64_t qrow = (int64_t)s * Lq + qi;
-    for (int d = lane; d < hd; d += 32) {
-      int64_t o = qrow * a.q.cols + a.q_col0 + h * hd + d;
-      qv[d] = join_f32(a.q.hi[o], a.q.lo()[o]) * scale;
+    if (active) {
+      for (int d = lane; d < hd; d += 32) {
+        int64_t o = qrow * a.q.cols + a.q_col0 + h * hd + d;
+        qv[d] = join_f32(a.q.hi[o], a.q.lo()[o]) * scale;
+      }
     }
     __syncwarp();
-    const int nkq = a.causal ? min(nk, qi + 1) : nk;   // causal: keys j <= qi
-    float mx = -INFINITY;
-    for (int t = lane; t < nkq; t += 32) {
-      const float* kr = Ks + t * (hd + 1);
+    const int nkq = !active ? 0 : (a.causal ? min(nk, qi + 1) : nk);   // causal: keys j <= qi
+    // keys any warp of the block needs; at least one chunk, so a row without valid keys is still written (NaN)
+    const int nkb = max(1, a.causal ? min(nk, min(q0 + ATT_WARPS, Lq)) : nk);
+    auto score = [&](int t, int c0) {
+      const float* kr = Ks + (t - c0) * (hd + 1);
       float acc = 0.0f;
 #pragma unroll 8
       for (int d = 0; d < hd; ++d) acc = fmaf(qv[d], kr[d], acc);
-      pv[t] = acc;
-      mx = fmaxf(mx, acc);
+      return acc;
+    };
+    float mx = -INFINITY;
+    for (int c0 = 0; c0 < nkb; c0 += kc) {
+      const int c1 = min(c0 + kc, nkb);
+      if (!resident) {
+        __syncthreads();
+        load(c0, c1, false);
+        __syncthreads();
+      }
+      for (int t = c0 + lane; t < min(c1, nkq); t += 32) {
+        const float acc = score(t, c0);
+        if (resident) pv[t] = acc;
+        mx = fmaxf(mx, acc);
+      }
     }
     mx = warp_max(mx);
     float sum = 0.0f;
-    for (int t = lane; t < nkq; t += 32) {
-      float e = expf(pv[t] - mx);
-      pv[t] = e;
-      sum += e;
+    for (int c0 = 0; c0 < nkb; c0 += kc) {
+      const int c1 = min(c0 + kc, nkb), ce = min(c1, nkq);
+      if (!resident) {
+        __syncthreads();
+        load(c0, c1, true);
+        __syncthreads();
+      }
+      for (int t = c0 + lane; t < ce; t += 32) {
+        float e = expf((resident ? pv[t - c0] : score(t, c0)) - mx);
+        pv[t - c0] = e;
+        sum += e;
+      }
+      const bool last = c1 == nkb;
+      const float inv = last ? 1.0f / warp_sum(sum) : 0.0f;
+      __syncwarp();
+      if (active) {
+        for (int d = lane; d < hd; d += 32) {
+          float acc = c0 == 0 ? 0.0f : ov[d];
+          for (int t = c0; t < ce; ++t) acc = fmaf(pv[t - c0], Vs[(t - c0) * hd + d], acc);
+          if (!last) {
+            ov[d] = acc;
+            continue;
+          }
+          acc *= inv;
+          __half hh, ll;
+          split_f32(acc, hh, ll);
+          int64_t o = qrow * a.out.cols + h * hd + d;
+          a.out.hi[o] = hh;
+          a.out.lo()[o] = ll;
+        }
+      }
+      __syncwarp();
     }
-    sum = warp_sum(sum);
-    const float inv = 1.0f / sum;
-    __syncwarp();
-    for (int d = lane; d < hd; d += 32) {
-      float acc = 0.0f;
-      for (int t = 0; t < nkq; ++t) acc = fmaf(pv[t], Vs[t * hd + d], acc);
-      acc *= inv;
-      __half hh, ll;
-      split_f32(acc, hh, ll);
-      int64_t o = qrow * a.out.cols + h * hd + d;
-      a.out.hi[o] = hh;
-      a.out.lo()[o] = ll;
-    }
-    __syncwarp();
   }
 }
 
@@ -369,19 +418,37 @@ void simt_ln(const LnArgs& a, cudaStream_t st) {
   else launch_pdl(k_ln<32>, grid, dim3(256), 0, st, a);
 }
 
-size_t simt_attention_smem(const AttnArgs& a) {
-  return ((size_t)a.Lk * (2 * a.hd + 1) + (size_t)ATT_WARPS * (a.hd + a.Lk)) * sizeof(float);
+// shared memory of k_attn_simt for kc keys per chunk (the output rows only when the keys do not fit one chunk)
+static size_t attn_smem(int hd, int Lk, int kc) {
+  size_t f = (size_t)kc * (2 * hd + 1) + (size_t)ATT_WARPS * (hd + kc);
+  if (kc < Lk) f += (size_t)ATT_WARPS * hd;
+  return f * sizeof(float);
 }
+
+// Keys per chunk: all Lk when they fit (K and V loaded once), else the most that fit, in whole warps of keys.
+// 0: not even one key fits beside the query and output rows (head_dim above ~3200).
+static int attn_chunk(int hd, int Lk) {
+  if (attn_smem(hd, Lk, Lk) <= ATT_SMEM_MAX) return Lk;
+  const size_t fixed = attn_smem(hd, Lk, 0), per_key = (size_t)(2 * hd + 1 + ATT_WARPS) * sizeof(float);
+  if (fixed + per_key > ATT_SMEM_MAX) return 0;
+  const int kc = (int)((ATT_SMEM_MAX - fixed) / per_key);
+  return kc >= 32 ? kc & ~31 : kc;
+}
+
+bool simt_attention_supported(int hd) { return hd >= 1 && attn_chunk(hd, 1 << 30) > 0; }
 
 int g_mldb_pdl = 1;
 
 void simt_init() {
   if (const char* e = getenv("MLDB_PDL")) g_mldb_pdl = atoi(e) != 0;
   // opt in to the full 227 KB once (not during stream capture)
-  cudaFuncSetAttribute(k_attn_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  cudaFuncSetAttribute(k_attn_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM_MAX);
 }
 
-void simt_attention(const AttnArgs& a, cudaStream_t st) {
-  const size_t smem = simt_attention_smem(a);
-  k_attn_simt<<<a.nseq * a.heads, ATT_WARPS * 32, smem, st>>>(a);
+bool simt_attention(const AttnArgs& a, cudaStream_t st) {
+  const int kc = attn_chunk(a.hd, a.Lk);
+  const size_t smem = kc > 0 ? attn_smem(a.hd, a.Lk, kc) : 0;
+  if (kc <= 0 || smem > ATT_SMEM_MAX) return false;       // never launch above the opt-in
+  k_attn_simt<<<a.nseq * a.heads, ATT_WARPS * 32, smem, st>>>(a, kc);
+  return true;
 }

@@ -59,10 +59,14 @@ def _causal_ref(qkv, nseq, L, heads):
     return (torch.softmax(s, -1) @ v).transpose(1, 2).reshape(nseq * L, d)
 
 
-@pytest.mark.parametrize("L", [1, 20, 77, 130])
-def test_causal_attention(eng, L):
-    nseq, heads, hd = 5, 12, 64
-    g = torch.Generator().manual_seed(L)
+@pytest.mark.parametrize("L,heads,hd", [pytest.param(L, 12, 64, id=str(L)) for L in (1, 20, 77, 130)] + [
+    # head_dim 128 around the 64-row query tiles and key blocks, up to the wgmma core's 256 keys; power-of-two and
+    # other head counts take the two head-decode branches of the wgmma kernel
+    pytest.param(L, heads, 128, id=f"hd128-h{heads}-{L}") for L, heads in
+    ((64, 8), (65, 12), (128, 16), (129, 8), (256, 12), (256, 16))])
+def test_causal_attention(eng, L, heads, hd):
+    nseq = 5
+    g = torch.Generator().manual_seed(L * heads + hd)
     qkv = torch.randn(nseq * L, 3 * heads * hd, generator=g)
     ref = _causal_ref(qkv, nseq, L, heads)
     for mode in (0, 2):
@@ -73,7 +77,8 @@ def test_causal_attention(eng, L):
         eng.debug_attention(qkv, nseq, L, heads, mode=1, causal=True)
 
 
-@pytest.mark.parametrize("M,N,K", [(385, 768, 768), (333, 768, 3072), (1000, 768, 2304)])
+@pytest.mark.parametrize("M,N,K", [(385, 768, 768), (333, 768, 3072), (1000, 768, 2304),
+                                   (200, 512, 4096), (129, 1024, 4096)])     # CLIP-B fc2 width, CLIP-H fc2 (K = 4096)
 def test_residual_add_epilogue(eng, M, N, K):
     g = torch.Generator().manual_seed(M + N + K)
     A, R = torch.randn(M, K, generator=g), torch.randn(M, N, generator=g)
@@ -85,7 +90,8 @@ def test_residual_add_epilogue(eng, M, N, K):
             assert _rel(y, ref) < (_tc_tol(K) if tc else 5e-6), (tc, in_place)
 
 
-@pytest.mark.parametrize("M,N,K", [(385, 3072, 768), (1000, 2304, 768), (129, 768, 3072)])
+@pytest.mark.parametrize("M,N,K", [(385, 3072, 768), (1000, 2304, 768), (129, 768, 3072),
+                                   (300, 1000, 256)])                         # N not a whole number of tiles
 def test_quick_gelu_epilogue(eng, M, N, K):
     g = torch.Generator().manual_seed(M * 3 + N)
     A = torch.randn(M, K, generator=g)
