@@ -76,8 +76,11 @@ __device__ __forceinline__ float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// CAUSAL is a template parameter so that the non-causal instantiations (the sampling path) carry no mask state
-template <int HD, bool CAUSAL>
+// CAUSAL is a template parameter so that the non-causal instantiations (the sampling path) carry no mask state.
+// KB (2 or 4) sizes the score row held in registers: S[KB][32] is 32 * KB registers per thread, and the consumer
+// warpgroup has 168 (three warpgroups per CTA), so the <= 128-key shapes (the denoiser's 79 tokens, the text
+// tower's 77) compile without spills or serialised MMAs only when the row is sized for them.
+template <int HD, bool CAUSAL, int KB>
 __global__ void __launch_bounds__(ATC_THREADS, 1)
 k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
           const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,    // 64-row boxes
@@ -88,6 +91,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   constexpr int SLOT_BYTES = 2 * NS * TILE;           // [plane][slice] tiles of one key block; the Q tile has the same shape
   constexpr int SL_PLANE = NS * TILE;                 // plane stride inside a slot
   constexpr int RS = PIPE_BYTES / SLOT_BYTES - 1;     // ring slots next to the Q tile
+  static_assert(KB >= 1 && KB <= MAX_KB, "score row");
   static_assert(RS >= 2 && RS <= MAX_RS, "ring depth");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -175,7 +179,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   const int cp = 2 * (lane & 3);                      // column offset inside an 8-column group
   const int row = (warp & 3) * 16 + (lane >> 2);      // this thread's first query row (the second is row + 8)
   const float sc = p.scale_log2e;
-  float S[MAX_KB][32];                                // the score row: [key block][accumulator fragment of 64 keys]
+  float S[KB][32];                                    // the score row: [key block][accumulator fragment of 64 keys]
   float O[NS][32];
   int rc = 0;
   for (int j = 0; j < nlocal; ++j) {
@@ -191,7 +195,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     // ---- S = Q K^T, block by block; a block's ring slot is freed when the NEXT block's MMAs have been issued
     const uint32_t qbase = smem_u32(sQ);
 #pragma unroll
-    for (int kb = 0; kb < MAX_KB; ++kb) {
+    for (int kb = 0; kb < KB; ++kb) {
       if (kb < nkb_i) {
         const int sl_i = (rc + kb) % RS;
         mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
@@ -223,13 +227,13 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     }
     rc += nkb_i;
 #pragma unroll
-    for (int kb = 0; kb < MAX_KB; ++kb)
+    for (int kb = 0; kb < KB; ++kb)
       if (kb < nkb_i) acc_fence(S[kb]);
     tl_event(p.tl, tl_n, 31, j);                                       // softmax: S(j) ready
     // ---- pass 1: row maxima over the valid keys (a row is spread over the 4 lanes of a quad)
     float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-    for (int kb = 0; kb < MAX_KB; ++kb) {
+    for (int kb = 0; kb < KB; ++kb) {
       if (kb < nkb_i) {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
@@ -247,7 +251,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     // ---- pass 2: P = exp2(sc * s - sc * max) (unnormalised, in place), fp32 row sums
     float sum0 = 0.0f, sum1 = 0.0f;
 #pragma unroll
-    for (int kb = 0; kb < MAX_KB; ++kb) {
+    for (int kb = 0; kb < KB; ++kb) {
       if (kb < nkb_i) {
 #pragma unroll
         for (int jj = 0; jj < 8; ++jj) {
@@ -267,9 +271,11 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     }
     sum0 = quad_sum(sum0); sum1 = quad_sum(sum1);
     tl_event(p.tl, tl_n, 33, j);                                       // softmax: pass 2 done
-    // ---- O = P V, block by block: P re-split to hi / lo fp16 A fragments, 16 keys per k-step
+    // ---- O = P V, block by block: P re-split to hi / lo fp16 A fragments, 16 keys per k-step.  Each block waits for
+    // its MMAs before the next block's split: keeping a block in flight holds its A fragments live across the next
+    // split, which at 168 registers makes ptxas serialise every wgmma of the kernel.
 #pragma unroll
-    for (int kb = 0; kb < MAX_KB; ++kb) {
+    for (int kb = 0; kb < KB; ++kb) {
       if (kb < nkb_i) {
         uint32_t ph[4][4], pl[4][4];
 #pragma unroll
@@ -353,6 +359,10 @@ bool plan_shape(const AttnArgs& a, AtcParams* p) {
   return p->nkb <= MAX_KB;
 }
 
+// the score row sized for the shape: up to 128 keys (the denoiser, the text tower) in KB = 2, longer rows in KB = 4
+template <int HD, bool CAUSAL>
+auto pick_kernel(int nkb) { return nkb <= 2 ? k_attn_tc<HD, CAUSAL, 2> : k_attn_tc<HD, CAUSAL, MAX_KB>; }
+
 }  // namespace
 
 bool tc_attention_init(int device) {
@@ -364,11 +374,11 @@ bool tc_attention_init(int device) {
     return false;
   g_encode = (PFN_tmapEncodeTiled)fn;
   cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, device);
-  if (cudaFuncSetAttribute(k_attn_tc<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(k_attn_tc<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(k_attn_tc<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess ||
-      cudaFuncSetAttribute(k_attn_tc<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
-    return false;
+  using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, AtcParams);
+  const Kernel kernels[] = {k_attn_tc<64, false, 2>, k_attn_tc<64, false, 4>, k_attn_tc<64, true, 2>, k_attn_tc<64, true, 4>,
+                            k_attn_tc<128, false, 2>, k_attn_tc<128, false, 4>, k_attn_tc<128, true, 2>, k_attn_tc<128, true, 4>};
+  for (Kernel k : kernels)
+    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) return false;
   g_ready = true;
   return true;
 }
@@ -407,8 +417,8 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   for (int k = 0; k < 8; ++k) if ((1 << k) == p.heads) p.heads_log2 = k;
   const int pairs = (p.items + 1) / 2;                 // two pipelines per CTA
   const int grid = pairs < g_sm_count ? pairs : g_sm_count;
-  auto kernel = a.hd == 64 ? (a.causal ? k_attn_tc<64, true> : k_attn_tc<64, false>)
-                           : (a.causal ? k_attn_tc<128, true> : k_attn_tc<128, false>);
+  auto kernel = a.hd == 64 ? (a.causal ? pick_kernel<64, true>(p.nkb) : pick_kernel<64, false>(p.nkb))
+                           : (a.causal ? pick_kernel<128, true>(p.nkb) : pick_kernel<128, false>(p.nkb));
   launch_pdl(kernel, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
   return true;
 }

@@ -138,6 +138,7 @@ __device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const flo
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     const float a0 = d[4 * j] - mean0, a1 = d[4 * j + 1] - mean0, a2 = d[4 * j + 2] - mean1, a3 = d[4 * j + 3] - mean1;
+    d[4 * j] = a0; d[4 * j + 1] = a1; d[4 * j + 2] = a2; d[4 * j + 3] = a3;
     q0 = fmaf(a0, a0, fmaf(a1, a1, q0));
     q1 = fmaf(a2, a2, fmaf(a3, a3, q1));
   }
@@ -147,11 +148,11 @@ __device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const flo
     const int n = 8 * j + cp;
     const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + n)), be = __ldg(reinterpret_cast<const float2*>(beta + n));
     if (ok0)
-      store_split2(out_hi, out_lo, (int64_t)r_lo * ld_out + n, fmaf((d[4 * j] - mean0) * rstd0, g.x, be.x),
-                   fmaf((d[4 * j + 1] - mean0) * rstd0, g.y, be.y));
+      store_split2(out_hi, out_lo, (int64_t)r_lo * ld_out + n, fmaf(d[4 * j] * rstd0, g.x, be.x),
+                   fmaf(d[4 * j + 1] * rstd0, g.y, be.y));
     if (ok1)
-      store_split2(out_hi, out_lo, (int64_t)(r_lo + 8) * ld_out + n, fmaf((d[4 * j + 2] - mean1) * rstd1, g.x, be.x),
-                   fmaf((d[4 * j + 3] - mean1) * rstd1, g.y, be.y));
+      store_split2(out_hi, out_lo, (int64_t)(r_lo + 8) * ld_out + n, fmaf(d[4 * j + 2] * rstd1, g.x, be.x),
+                   fmaf(d[4 * j + 3] * rstd1, g.y, be.y));
   }
 }
 
