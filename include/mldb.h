@@ -35,7 +35,7 @@ extern "C" {
 #define MLDB_ERR_STATE 3     /* call out of order (weights not finalized, ...) */
 #define MLDB_ERR_UNSUPPORTED 4
 
-#define MLDB_ABI_VERSION 3
+#define MLDB_ABI_VERSION 4
 
 typedef struct mldb_handle mldb_handle;
 
@@ -52,6 +52,10 @@ typedef struct mldb_handle mldb_handle;
 /* scheduler kinds (diffusers; configs/modules/scheduler.yaml) */
 #define MLDB_SCHED_DDIM 0
 #define MLDB_SCHED_DDPM 1
+/* beta schedules (diffusers beta_schedule) */
+#define MLDB_BETA_SCALED_LINEAR 0       /* linspace(sqrt(beta_start), sqrt(beta_end), T, fp32) ** 2 */
+#define MLDB_BETA_LINEAR 1              /* linspace(beta_start, beta_end, T, fp32) */
+#define MLDB_BETA_SQUAREDCOS_CAP_V2 2   /* betas_for_alpha_bar: cosine alpha_bar, double math, max_beta 0.999 */
 /* tensor dtypes for mldb_load_tensor */
 #define MLDB_DTYPE_F32 0
 
@@ -85,11 +89,15 @@ typedef struct mldb_config {
   int32_t sched_kind;         /* MLDB_SCHED_* */
   int32_t num_train_timesteps;/* 1000 */
   double  beta_start;         /* 0.00085 (double: diffusers takes the Python float's sqrt) */
-  double  beta_end;           /* 0.012  (beta_schedule is scaled_linear) */
+  double  beta_end;           /* 0.012 */
   int32_t steps_offset;       /* DDIM: 1 */
   int32_t set_alpha_to_one;   /* DDIM: 0 */
-  float   eta;                /* DDIM: 0.0 (only eta == 0 is supported: no step noise) */
+  float   eta;                /* DDIM: 0.0, in [0, 1].  eta > 0 adds std_dev_t * N(0,1) at every step; the
+                                 caller passes those draws as step_noise (the library draws no random numbers).
+                                 DDPM ignores it (its steps at t > 0 always add noise). */
   int32_t njoints;            /* 22 (HumanML3D) for feats2joints */
+  int32_t beta_schedule;      /* MLDB_BETA_*: scaled_linear (0, the shipped config) */
+  int32_t clip_sample;        /* 0; != 0 clamps the predicted x0 to [-1, 1] (DDIM and DDPM) */
 } mldb_config;
 
 /* Fill cfg with the shipped text-to-motion defaults (configs/modules/{denoiser,motion_vae,
@@ -127,9 +135,10 @@ int mldb_scheduler_timesteps(const mldb_config* cfg, int32_t n, int64_t* out);
  * diffusers: DDIM (arange(n)*(T/n))[::-1]+steps_offset, DDPM arange(0,T,T/n)[::-1]. */
 int mldb_scheduler_set_timesteps(mldb_handle* h, int32_t n, int64_t* timesteps_out);
 
-/* Replaces: scheduler.step(model_output, t, sample, eta=0).prev_sample (mld.py:345).
- * `noise` is the injected N(0,1) tensor for DDPM when t > 0 (NULL for DDIM).
- * count = number of floats in sample. */
+/* Replaces: scheduler.step(model_output, t, sample, eta=cfg.eta).prev_sample (mld.py:345), with the
+ * configured beta_schedule and clip_sample.  `noise` is the injected N(0,1) tensor (diffusers' variance_noise,
+ * count floats), required when the step adds noise: DDIM with eta > 0, DDPM at t > 0; else it may be NULL
+ * and is not read.  count = number of floats in sample. */
 int mldb_scheduler_step(mldb_handle* h, const float* model_output, int64_t timestep,
                         const float* sample, const float* noise, int64_t count,
                         float* prev_sample, void* stream);
@@ -150,8 +159,10 @@ int mldb_denoise(mldb_handle* h, const float* sample, int64_t timestep, const vo
  *   cond        [2B, S_ctx, text_dim] uncond half first (mld.py:225-230) when guidance > 1,
  *               else [B, ...]; int64 [2B,1] for the action model
  *   init_noise  [B, n_lat, d] (or [B, T, nfeats] when diffusion_only)
- *   step_noise  DDPM only (required then): the N(0,1) draws of scheduler.step, [n_steps, B, n_lat, d]
- *               (or [n_steps, B, T, nfeats] when diffusion_only); NULL for DDIM
+ *   step_noise  the N(0,1) draws of scheduler.step, [n_steps, B, n_lat, d] (or [n_steps, B, T, nfeats] when
+ *               diffusion_only), slice i for step i.  Required when some step adds noise (DDIM with eta > 0,
+ *               DDPM); then only the slices of steps that add noise are read (DDPM: not the last, t == 0).
+ *               May be NULL, and is ignored, when no step adds noise (DDIM with eta == 0)
  *   latents_out [n_lat, B, d]  (mld.py:359)  (or [T, B, nfeats])
  * The n scheduler steps are replayed from one CUDA graph per (B, S_ctx, T) shape (the no-VAE model: one
  * captured step, replayed n times with a device-side step counter). */
@@ -177,19 +188,20 @@ int mldb_feats2joints(mldb_handle* h, const float* feats, int32_t B, int32_t T,
 
 /* Replaces: MLD.forward(batch) after the text encoder (mld.py:232-264): reverse diffusion ->
  * vae.decode -> feats2joints, replayed as one CUDA graph.  Buffers as above; feats_out and
- * joints_out may each be NULL when not wanted. */
+ * joints_out may each be NULL when not wanted.  step_noise as for mldb_diffusion_reverse. */
 int mldb_sample(mldb_handle* h, const void* cond, const float* init_noise,
                 const int32_t* lengths, int32_t B, int32_t S_ctx, int32_t T,
-                float* latents_out, float* feats_out, float* joints_out, void* stream);
+                float* latents_out, float* feats_out, float* joints_out, void* stream,
+                const float* step_noise);
 
 /* Same as mldb_sample but through HOST buffers (pinned or pageable): copies cond/noise/
- * lengths host->device, runs, copies joints device->host, all on `stream`; returns after
- * enqueue (synchronise the stream before reading joints_host).  This is the call the
+ * lengths (and step_noise_host when given) host->device, runs, copies joints device->host, all on `stream`;
+ * returns after enqueue (synchronise the stream before reading joints_host).  This is the call the
  * end-to-end benchmark times.  With a communicator attached joints_host receives the GATHERED motions
  * [nranks * B, T, njoints, 3]. */
 int mldb_sample_host(mldb_handle* h, const void* cond_host, const float* init_noise_host,
                      const int32_t* lengths_host, int32_t B, int32_t S_ctx, int32_t T,
-                     float* joints_host, void* stream);
+                     float* joints_host, void* stream, const float* step_noise_host);
 
 /* ---- multi-GPU: batch-sharded replicas + ONE all-gather of the finished motions (SURVEY.md section 8e).
  * One process (handle) per GPU; NCCL is bound at run time (dlopen libnccl.so.2).  Either build the
@@ -205,9 +217,11 @@ int mldb_allgather(mldb_handle* h, const float* local, float* global, int64_t co
 /* mldb_sample on this rank's shard, the joints of all ranks gathered into joints_global
  * [nranks * B, T, njoints, 3]: this rank's joints are written straight into its slot and the in-place
  * all-gather runs on a side stream, overlapping whatever is enqueued next on `stream`.  Alternate two
- * joints_global buffers between consecutive calls; mldb_gather_wait makes `stream` wait for the last gather. */
+ * joints_global buffers between consecutive calls; mldb_gather_wait makes `stream` wait for the last gather.
+ * step_noise is this rank's shard [n_steps, B, n_lat, d] of the global per-step draws (or NULL, as for mldb_sample). */
 int mldb_sample_gather(mldb_handle* h, const void* cond, const float* init_noise, const int32_t* lengths,
-                       int32_t B, int32_t S_ctx, int32_t T, float* joints_global, void* stream);
+                       int32_t B, int32_t S_ctx, int32_t T, float* joints_global, void* stream,
+                       const float* step_noise);
 int mldb_gather_wait(mldb_handle* h, void* stream);
 
 /* Profiling aid used by bench.py's roofline leg: time one operator of denoiser layer 0 in

@@ -12,11 +12,13 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libmldb200.so")
 
-MLDB_ABI_VERSION = 3
+MLDB_ABI_VERSION = 4
 COND_TEXT, COND_ACTION = 0, 1
 ARCH_TRANS_ENC, ARCH_TRANS_DEC = 0, 1
 VAE_NONE, VAE_MLD, VAE_ACTOR = 0, 1, 2
 SCHED_DDIM, SCHED_DDPM = 0, 1
+# diffusers beta_schedule names -> MLDB_BETA_*
+BETA_SCHEDULES = {"scaled_linear": 0, "linear": 1, "squaredcos_cap_v2": 2}
 DTYPE_F32 = 0
 # mldb_kernel_stats indices (MLDB_KSTAT_* in include/mldb.h)
 KSTAT_NAMES = ("gemm_tc", "gemm_ln_tc", "ffn_tc", "attn_tc", "attn_mma", "attn_simt", "gemm_simt", "ln_simt",
@@ -40,6 +42,7 @@ class MldbConfig(C.Structure):
         ("sched_kind", C.c_int32), ("num_train_timesteps", C.c_int32),
         ("beta_start", C.c_double), ("beta_end", C.c_double), ("steps_offset", C.c_int32),
         ("set_alpha_to_one", C.c_int32), ("eta", C.c_float), ("njoints", C.c_int32),
+        ("beta_schedule", C.c_int32), ("clip_sample", C.c_int32),
     ]
 
 
@@ -70,8 +73,8 @@ _SIGNATURES = {
     "mldb_vae_decode": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
     "mldb_vae_encode": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     "mldb_feats2joints": (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P, _P]),
-    "mldb_sample": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P]),
-    "mldb_sample_host": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_sample": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P, _P, _P]),
+    "mldb_sample_host": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P]),
     "mldb_profile_op": (C.c_int, [_P, C.c_char_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_float)]),
     "mldb_profile_steps": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P]),
     "mldb_debug_timeline": (C.c_int, [C.c_int32, _P, C.c_int32, C.POINTER(C.c_int32)]),
@@ -90,7 +93,7 @@ _SIGNATURES = {
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_info": (C.c_int, [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "mldb_allgather": (C.c_int, [_P, _P, _P, C.c_int64, _P]),
-    "mldb_sample_gather": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_sample_gather": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P, _P]),
     "mldb_gather_wait": (C.c_int, [_P, _P]),
     "mldb_kernel_stats": (C.c_int, [_P, _P, C.c_int32]),
     "mldb_reset_kernel_stats": (C.c_int, [_P]),

@@ -73,6 +73,7 @@ extern "C" void mldb_default_config(mldb_config* c) {
   c->sched_kind = MLDB_SCHED_DDIM; c->num_train_timesteps = 1000;
   c->beta_start = 0.00085; c->beta_end = 0.012; c->steps_offset = 1; c->set_alpha_to_one = 0;
   c->eta = 0.0f; c->njoints = 22;
+  c->beta_schedule = MLDB_BETA_SCALED_LINEAR; c->clip_sample = 0;
 }
 
 // ----------------------------------------------------------------------------- tensor spec
@@ -283,20 +284,44 @@ static int upload_pe(mldb_handle* h, const std::string& key, float** out, int* r
 }
 
 // ----------------------------------------------------------------------------- scheduler
-// betas = linspace(sqrt(b0), sqrt(b1), T, fp32) ** 2 ; alphas_cumprod = cumprod(1 - betas)
-// (diffusers scaled_linear schedule; fp32 throughout like torch).
+// The scheduler settings the library implements (diffusers DDIMScheduler / DDPMScheduler with epsilon
+// prediction, fixed_small variance, clip_sample_range 1.0).
+static int check_sched_cfg(const mldb_config& c) {
+  if (c.sched_kind != MLDB_SCHED_DDIM && c.sched_kind != MLDB_SCHED_DDPM) FAIL(MLDB_ERR_INVALID, "unknown sched_kind %d", c.sched_kind);
+  if (c.beta_schedule != MLDB_BETA_SCALED_LINEAR && c.beta_schedule != MLDB_BETA_LINEAR &&
+      c.beta_schedule != MLDB_BETA_SQUAREDCOS_CAP_V2)
+    FAIL(MLDB_ERR_INVALID, "unknown beta_schedule %d", c.beta_schedule);
+  if (!(c.eta >= 0.0f && c.eta <= 1.0f)) FAIL(MLDB_ERR_INVALID, "eta must lie in [0, 1], got %g", (double)c.eta);
+  if (c.num_train_timesteps < 2) FAIL(MLDB_ERR_INVALID, "num_train_timesteps must be >= 2");
+  return MLDB_OK;
+}
+
+// alphas_cumprod = cumprod(1 - betas) for the configured beta_schedule (fp32 like torch):
+//   scaled_linear      betas = linspace(sqrt(b0), sqrt(b1), T, fp32) ** 2
+//   linear             betas = linspace(b0, b1, T, fp32)
+//   squaredcos_cap_v2  betas = fp32(min(1 - alpha_bar((i+1)/T) / alpha_bar(i/T), 0.999)) in double,
+//                      alpha_bar(t) = cos((t + 0.008) / 1.008 * pi / 2) ** 2  (diffusers betas_for_alpha_bar)
 static void build_alphas(const mldb_config& c, std::vector<float>* out) {
-  // Bit-exact with torch on CPU (checked in tests/test_scheduler.py): linspace evaluates
-  // start + step*i (first half) / end - step*(T-1-i) (second half) with one rounding (FMA);
-  // cumprod accumulates in double (at::acc_type<float> on CPU) and rounds each output.
+  // Bit-exact with torch on CPU (checked in tests/test_scheduler.py and test_scheduler_stochastic.py):
+  // linspace evaluates start + step*i (first half) / end - step*(T-1-i) (second half) with one rounding
+  // (FMA); cumprod accumulates in double (at::acc_type<float> on CPU) and rounds each output.
   const int T = c.num_train_timesteps;
   out->resize(T);
-  const float s0 = (float)sqrt(c.beta_start), s1 = (float)sqrt(c.beta_end);
+  const bool scaled = c.beta_schedule == MLDB_BETA_SCALED_LINEAR;
+  const float s0 = scaled ? (float)sqrt(c.beta_start) : (float)c.beta_start;
+  const float s1 = scaled ? (float)sqrt(c.beta_end) : (float)c.beta_end;
   const float step = (s1 - s0) / (float)(T - 1);
+  auto alpha_bar = [](double t) { return pow(cos((t + 0.008) / 1.008 * M_PI / 2), 2.0); };
   double prod = 1.0;
   for (int i = 0; i < T; ++i) {
-    const float v = (i < T / 2) ? fmaf(step, (float)i, s0) : fmaf(-step, (float)(T - 1 - i), s1);
-    const float beta = v * v;
+    float beta;
+    if (c.beta_schedule == MLDB_BETA_SQUAREDCOS_CAP_V2) {
+      const double t1 = (double)i / T, t2 = (double)(i + 1) / T;
+      beta = (float)std::min(1.0 - alpha_bar(t2) / alpha_bar(t1), 0.999);
+    } else {
+      const float v = (i < T / 2) ? fmaf(step, (float)i, s0) : fmaf(-step, (float)(T - 1 - i), s1);
+      beta = scaled ? v * v : v;
+    }
     const float alpha = 1.0f - beta;
     prod *= (double)alpha;
     (*out)[i] = (float)prod;
@@ -304,6 +329,7 @@ static void build_alphas(const mldb_config& c, std::vector<float>* out) {
 }
 extern "C" int mldb_scheduler_table(const mldb_config* cfg, float* alphas_cumprod_out) {
   if (!cfg || !alphas_cumprod_out) FAIL(MLDB_ERR_INVALID, "null argument");
+  TRY(check_sched_cfg(*cfg));
   std::vector<float> a;
   build_alphas(*cfg, &a);
   memcpy(alphas_cumprod_out, a.data(), a.size() * sizeof(float));
@@ -325,12 +351,17 @@ static StepCoef make_coef(const mldb_handle* h, int64_t t, int n_inference) {
   const float a_t = ac[t];
   k.c0 = sqrtf(a_t);
   k.c1 = sqrtf(1.0f - a_t);
+  k.clip = c.clip_sample ? 1 : 0;
   if (c.sched_kind == MLDB_SCHED_DDIM) {
     const float a_prev = prev_t >= 0 ? ac[prev_t] : (c.set_alpha_to_one ? 1.0f : ac[0]);
+    // variance = (beta_prod_t_prev / beta_prod_t) * (1 - alpha_prod_t / alpha_prod_t_prev);
+    // std_dev_t = eta * variance ** 0.5 (0 when eta == 0: c3 is then sqrt(1 - a_prev - 0))
+    const float variance = ((1.0f - a_prev) / (1.0f - a_t)) * (1.0f - a_t / a_prev);
+    const float std_dev = c.eta * sqrtf(variance);
     k.kind = 0;
     k.c2 = sqrtf(a_prev);
-    k.c3 = sqrtf(1.0f - a_prev - 0.0f);   // eta == 0 => std_dev_t == 0
-    k.sigma = 0.0f;
+    k.c3 = sqrtf(1.0f - a_prev - std_dev * std_dev);
+    k.sigma = std_dev;
   } else {
     const float a_prev = prev_t >= 0 ? ac[prev_t] : 1.0f;
     const float bpt = 1.0f - a_t, bpp = 1.0f - a_prev;
@@ -625,7 +656,7 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   if (cfg->arch == MLDB_ARCH_TRANS_ENC && cfg->num_layers > 0 && cfg->num_layers % 2 != 1) FAIL(MLDB_ERR_INVALID, "skip encoder needs an odd layer count");
   if (cfg->arch == MLDB_ARCH_TRANS_ENC && cfg->diffusion_only) FAIL(MLDB_ERR_UNSUPPORTED, "diffusion_only requires arch trans_dec");
   if (cfg->vae_kind == MLDB_VAE_MLD && cfg->vae_layers % 2 != 1) FAIL(MLDB_ERR_INVALID, "MldVae needs an odd layer count");
-  if (cfg->sched_kind == MLDB_SCHED_DDIM && cfg->eta != 0.0f) FAIL(MLDB_ERR_UNSUPPORTED, "DDIM eta != 0");
+  TRY(check_sched_cfg(*cfg));
   int ndev = 0;
   CK(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) FAIL(MLDB_ERR_INVALID, "no such CUDA device %d (no CPU fallback exists)", device);
@@ -981,7 +1012,9 @@ extern "C" int mldb_scheduler_step(mldb_handle* h, const float* model_output, in
   if (timestep < 0 || timestep >= h->cfg.num_train_timesteps) FAIL(MLDB_ERR_INVALID, "timestep out of range");
   DeviceGuard guard(h->device);
   StepCoef k = make_coef(h, timestep, (int)h->timesteps.size());
-  if (k.kind == 1 && k.sigma != 0.0f && !noise) FAIL(MLDB_ERR_INVALID, "DDPM step at t > 0 needs the injected noise tensor");
+  if (k.sigma != 0.0f && !noise)
+    FAIL(MLDB_ERR_INVALID, "the step at t = %lld adds noise (%s) and needs the injected N(0,1) noise tensor",
+         (long long)timestep, k.kind == 0 ? "DDIM eta > 0" : "DDPM t > 0");
   k_sched_step<<<(unsigned)((count + 255) / 256), 256, 0, (cudaStream_t)stream>>>(model_output, sample, noise, prev_sample, count, k);
   kcount(h, MLDB_KSTAT_MISC);
   CK(cudaGetLastError());
@@ -1318,6 +1351,13 @@ extern "C" int mldb_denoise(mldb_handle* h, const float* sample, int64_t timeste
   return MLDB_OK;
 }
 
+// Does some step of the current timestep schedule add noise (non-zero std / sigma)?
+static bool steps_add_noise(const mldb_handle* h) {
+  for (const StepCoef& k : h->coefs_host)
+    if (k.sigma != 0.0f) return true;
+  return false;
+}
+
 static int run_reverse(mldb_handle* h, const void* cond, const float* init_noise, const float* step_noise,
                        const int32_t* lengths, int B, int S, int T, float* latents_out, cudaStream_t st,
                        Plan** plan_out) {
@@ -1326,10 +1366,15 @@ static int run_reverse(mldb_handle* h, const void* cond, const float* init_noise
   const bool cfg_on = c.guidance_scale > 1.0f;
   const int Bx = cfg_on ? 2 * B : B;
   if (c.arch == MLDB_ARCH_TRANS_DEC) {
-    // no-VAE model: latents are the motion itself, [B, T, F]; DDPM draws noise every step, which
-    // the caller injects (step_noise [n_steps, B, T, F]).  Eager loop: 1000 big steps, no graph.
+    // no-VAE model: latents are the motion itself, [B, T, F]; DDPM (and DDIM with eta > 0) adds noise at
+    // its steps, which the caller injects (step_noise [n_steps, B, T, F]).  One captured step, replayed.
     if (!c.diffusion_only) FAIL(MLDB_ERR_UNSUPPORTED, "arch trans_dec is built for the no-VAE model (diffusion_only)");
     if (!lengths || T <= 0) FAIL(MLDB_ERR_INVALID, "the no-VAE model needs lengths and T");
+    const int nsteps = (int)h->timesteps.size();
+    const bool needs_noise = steps_add_noise(h);
+    if (needs_noise && !step_noise)
+      FAIL(MLDB_ERR_INVALID, "this scheduler adds noise at its steps (%s): pass step_noise [%d, %d, %d, %d] (N(0,1) per step)",
+           c.sched_kind == MLDB_SCHED_DDIM ? "DDIM eta > 0" : "DDPM", nsteps, B, T, c.nfeats);
     Plan* p = nullptr;
     TRY(decden_plan(h, 5, B, Bx, S, T, &p));
     const int64_t per = (int64_t)T * c.nfeats;
@@ -1337,10 +1382,6 @@ static int run_reverse(mldb_handle* h, const void* cond, const float* init_noise
     k_dup_lengths<<<nblk(Bx), 256, 0, st>>>(lengths, p->lengths, B, Bx);
     kcount(h, MLDB_KSTAT_MISC);
     CK(cudaMemcpyAsync(p->latents, init_noise, (size_t)B * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    const int nsteps = (int)h->timesteps.size();
-    bool needs_noise = false;
-    for (int i = 0; i < nsteps; ++i) needs_noise |= h->coefs_host[i].kind == 1 && h->coefs_host[i].sigma != 0.0f;
-    if (needs_noise && !step_noise) FAIL(MLDB_ERR_INVALID, "DDPM needs step_noise [n_steps, B, T, F]");
     // ONE captured step, replayed n_steps times: the step index lives on the device (k_step_inc), the
     // kernels that depend on it (time token, scheduler coefficients, noise slice) read it through p->d_step.
     // The graph holds the caller's noise pointer: a different buffer re-captures.
@@ -1374,12 +1415,13 @@ static int run_reverse(mldb_handle* h, const void* cond, const float* init_noise
   // latents = init_noise * init_noise_sigma (== 1 for DDIM/DDPM), mld.py:310
   CK(cudaMemcpyAsync(p->latents, init_noise, (size_t)B * per * sizeof(float), cudaMemcpyDeviceToDevice, st));
   const int nsteps = (int)h->timesteps.size();
-  // DDPM draws noise at every step with t > 0 (diffusers DDPMScheduler.step): the caller injects it
+  // DDPM (every step with t > 0) and DDIM with eta > 0 (every step) add std * N(0,1) (diffusers
+  // scheduler.step draws it): the caller injects the draws
   const float* nz_all = nullptr;
-  bool needs_noise = false;
-  for (int i = 0; i < nsteps; ++i) needs_noise |= h->coefs_host[i].kind == 1 && h->coefs_host[i].sigma != 0.0f;
-  if (needs_noise) {
-    if (!step_noise) FAIL(MLDB_ERR_INVALID, "the DDPM scheduler needs step_noise [n_steps, B, n_lat, d] (injected N(0,1) per step)");
+  if (steps_add_noise(h)) {
+    if (!step_noise)
+      FAIL(MLDB_ERR_INVALID, "this scheduler adds noise at its steps (%s): pass step_noise [%d, %d, %d, %d] (N(0,1) per step)",
+           c.sched_kind == MLDB_SCHED_DDIM ? "DDIM eta > 0" : "DDPM", nsteps, B, c.n_lat, d);
     if (p->noise_cap < (size_t)nsteps * B * per) {
       TRY(dev_alloc(h, (void**)&p->step_noise, (size_t)nsteps * B * per * sizeof(float)));
       p->noise_cap = (size_t)nsteps * B * per;
@@ -1570,7 +1612,8 @@ extern "C" int mldb_feats2joints(mldb_handle* h, const float* feats, int32_t B, 
 // ----------------------------------------------------------------------------- full sample
 extern "C" int mldb_sample(mldb_handle* h, const void* cond, const float* init_noise,
                            const int32_t* lengths, int32_t B, int32_t S_ctx, int32_t T,
-                           float* latents_out, float* feats_out, float* joints_out, void* stream) {
+                           float* latents_out, float* feats_out, float* joints_out, void* stream,
+                           const float* step_noise) {
   TRY(check_ready(h, true));
   DeviceGuard guard(h->device);
   if (!cond || !init_noise || !lengths || B <= 0 || T <= 0) FAIL(MLDB_ERR_INVALID, "bad argument");
@@ -1585,7 +1628,7 @@ extern "C" int mldb_sample(mldb_handle* h, const void* cond, const float* init_n
     z = dp->stage_f32;
   }
   if (c.arch != MLDB_ARCH_TRANS_ENC) FAIL(MLDB_ERR_UNSUPPORTED, "mldb_sample is built for the latent (VAE) models");
-  TRY(run_reverse(h, cond, init_noise, nullptr, lengths, B, S_ctx, T, z, st, &rp));
+  TRY(run_reverse(h, cond, init_noise, step_noise, lengths, B, S_ctx, T, z, st, &rp));
   TRY(run_decode(h, z, lengths, B, T, feats_out, st, &dp));
   if (joints_out) TRY(run_f2j(h, feats_out ? feats_out : dp->feats, B, T, joints_out, st));
   return MLDB_OK;
@@ -1598,17 +1641,18 @@ extern "C" int mldb_sample(mldb_handle* h, const void* cond, const float* init_n
 // joints_global on `stream`, and alternate (at least) two joints_global buffers between consecutive calls.
 extern "C" int mldb_sample_gather(mldb_handle* h, const void* cond, const float* init_noise,
                                   const int32_t* lengths, int32_t B, int32_t S_ctx, int32_t T,
-                                  float* joints_global, void* stream) {
+                                  float* joints_global, void* stream, const float* step_noise) {
   TRY(check_ready(h, true));
   DeviceGuard guard(h->device);
   if (!joints_global) FAIL(MLDB_ERR_INVALID, "bad argument");
   const int64_t count = (int64_t)B * T * h->cfg.njoints * 3;
   cudaStream_t st = (cudaStream_t)stream;
   if (!h->nccl_comm) {      // single rank: the gather is the identity
-    return mldb_sample(h, cond, init_noise, lengths, B, S_ctx, T, nullptr, nullptr, joints_global, stream);
+    return mldb_sample(h, cond, init_noise, lengths, B, S_ctx, T, nullptr, nullptr, joints_global, stream, step_noise);
   }
   TRY(mldb_gather_begin(h, st));
-  TRY(mldb_sample(h, cond, init_noise, lengths, B, S_ctx, T, nullptr, nullptr, joints_global + h->comm_rank * count, stream));
+  TRY(mldb_sample(h, cond, init_noise, lengths, B, S_ctx, T, nullptr, nullptr, joints_global + h->comm_rank * count, stream,
+                  step_noise));
   return mldb_gather_async(h, joints_global, count, st);
 }
 
@@ -1616,7 +1660,7 @@ extern "C" int mldb_sample_gather(mldb_handle* h, const void* cond, const float*
 // [nranks * B, T, njoints, 3] (every rank holds all of them after the all-gather), else [B, T, njoints, 3].
 extern "C" int mldb_sample_host(mldb_handle* h, const void* cond_host, const float* init_noise_host,
                                 const int32_t* lengths_host, int32_t B, int32_t S_ctx, int32_t T,
-                                float* joints_host, void* stream) {
+                                float* joints_host, void* stream, const float* step_noise_host) {
   TRY(check_ready(h, true));
   DeviceGuard guard(h->device);
   if (!cond_host || !init_noise_host || !lengths_host || !joints_host || B <= 0 || T <= 0) FAIL(MLDB_ERR_INVALID, "bad argument");
@@ -1643,13 +1687,26 @@ extern "C" int mldb_sample_host(mldb_handle* h, const void* cond_host, const flo
   CK(cudaMemcpyAsync(dp->cond_f, cond_host, cond_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(dp->noise_in, init_noise_host, noise_bytes, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(dp->cond_i, lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  // per-step noise [n_steps, B, n_lat, d]: staged in the decode plan's step_noise buffer (unused by decoding)
+  const float* step_noise = nullptr;
+  if (step_noise_host) {
+    const size_t n = h->timesteps.size() * (size_t)B * c.n_lat * c.latent_dim;
+    if (dp->noise_cap < n) {
+      TRY(dev_alloc(h, (void**)&dp->step_noise, n * sizeof(float)));
+      dp->noise_cap = n;
+    }
+    CK(cudaMemcpyAsync(dp->step_noise, step_noise_host, n * sizeof(float), cudaMemcpyHostToDevice, st));
+    step_noise = dp->step_noise;
+  }
   if (world > 1) {
-    TRY(mldb_sample_gather(h, dp->cond_f, dp->noise_in, (const int32_t*)dp->cond_i, B, S_ctx, T, dp->joints_all, stream));
+    TRY(mldb_sample_gather(h, dp->cond_f, dp->noise_in, (const int32_t*)dp->cond_i, B, S_ctx, T, dp->joints_all, stream,
+                           step_noise));
     TRY(mldb_gather_wait(h, stream));
     CK(cudaMemcpyAsync(joints_host, dp->joints_all, world * joints_elems * sizeof(float), cudaMemcpyDeviceToHost, st));
     return MLDB_OK;
   }
-  TRY(mldb_sample(h, dp->cond_f, dp->noise_in, (const int32_t*)dp->cond_i, B, S_ctx, T, nullptr, nullptr, dp->joints, stream));
+  TRY(mldb_sample(h, dp->cond_f, dp->noise_in, (const int32_t*)dp->cond_i, B, S_ctx, T, nullptr, nullptr, dp->joints, stream,
+                  step_noise));
   CK(cudaMemcpyAsync(joints_host, dp->joints, joints_elems * sizeof(float), cudaMemcpyDeviceToHost, st));
   return MLDB_OK;
 }

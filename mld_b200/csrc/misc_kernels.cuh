@@ -147,28 +147,30 @@ static __global__ void k_permute_01(const float* __restrict__ src, float* __rest
 // Scheduler coefficients for one step, computed on the host in fp32 exactly as diffusers does
 // (0-d fp32 tensor arithmetic; x ** 0.5 == sqrtf).
 struct StepCoef {
-  float c0, c1, c2, c3;  // DDIM: sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev)
+  float c0, c1, c2, c3;  // DDIM: sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-std^2)
                          // DDPM: sqrt(a_t), sqrt(1-a_t), x0 coeff, sample coeff
-  float sigma;           // DDPM: sqrt(clamp(var, 1e-20)) when t > 0 else 0
+  float sigma;           // scale of the injected N(0,1) noise; 0 = the step adds none (and reads none)
+                         // DDIM: std_dev_t = eta * sqrt(variance); DDPM: sqrt(clamp(var, 1e-20)) when t > 0
   int kind;              // 0 DDIM, 1 DDPM
+  int clip;              // clip_sample: x0 clamped to [-1, 1] (clip_sample_range 1.0)
 };
 
 __device__ __forceinline__ float sched_update(const StepCoef& k, float x, float e, float nz) {
   // pred_original_sample = (sample - beta_prod_t ** 0.5 * model_output) / alpha_prod_t ** 0.5
-  const float x0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(k.c1, e)), k.c0);
-  if (k.kind == 0) {
-    // prev = alpha_prod_t_prev ** 0.5 * x0 + (1 - alpha_prod_t_prev) ** 0.5 * model_output
-    return __fadd_rn(__fmul_rn(k.c2, x0), __fmul_rn(k.c3, e));
-  }
-  float p = __fadd_rn(__fmul_rn(k.c2, x0), __fmul_rn(k.c3, x));
+  float x0 = __fdiv_rn(__fsub_rn(x, __fmul_rn(k.c1, e)), k.c0);
+  if (k.clip) x0 = x0 < -1.0f ? -1.0f : (x0 > 1.0f ? 1.0f : x0);   // torch.clamp: a NaN stays NaN
+  // DDIM: prev = alpha_prod_t_prev ** 0.5 * x0 + (1 - alpha_prod_t_prev - std_dev_t ** 2) ** 0.5 * model_output
+  // DDPM: prev = x0 coeff * x0 + sample coeff * sample
+  float p = __fadd_rn(__fmul_rn(k.c2, x0), __fmul_rn(k.c3, k.kind == 0 ? e : x));
+  // + std_dev_t * variance_noise (DDIM, eta > 0) / + variance ** 0.5 * variance_noise (DDPM, t > 0)
   if (k.sigma != 0.0f) p = __fadd_rn(p, __fmul_rn(k.sigma, nz));
   return p;
 }
 
 // Classifier-free guidance (mld.py:339-342) + scheduler.step (mld.py:345), in place on latents.
 //   eps: [Bx, per] with the uncond half first when cfg_on; latents: [B, per];
-//   noise_base: [n_steps, B, per] injected N(0,1) (DDPM) or null; step_ptr != null overrides `step`
-//   (device-side counter of a replayed step graph).
+//   noise_base: [n_steps, B, per] injected N(0,1) or null, read only by steps with a non-zero sigma;
+//   step_ptr != null overrides `step` (device-side counter of a replayed step graph).
 static __global__ void k_cfg_sched(const float* __restrict__ eps, float* __restrict__ latents,
                             const float* __restrict__ noise_base, int64_t n_per_half, int cfg_on,
                             float guidance, const StepCoef* __restrict__ coefs, int step,
@@ -184,7 +186,8 @@ static __global__ void k_cfg_sched(const float* __restrict__ eps, float* __restr
     e = __fadd_rn(e, __fmul_rn(guidance, __fsub_rn(c, e)));
   }
   const StepCoef k = coefs[step];
-  latents[i] = sched_update(k, latents[i], e, noise_base ? noise_base[(int64_t)step * n_per_half + i] : 0.0f);
+  const float nz = noise_base && k.sigma != 0.0f ? noise_base[(int64_t)step * n_per_half + i] : 0.0f;
+  latents[i] = sched_update(k, latents[i], e, nz);
 }
 
 static __global__ void k_sched_step(const float* __restrict__ eps, const float* __restrict__ sample,
@@ -192,7 +195,7 @@ static __global__ void k_sched_step(const float* __restrict__ eps, const float* 
                              StepCoef k) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  out[i] = sched_update(k, sample[i], eps[i], noise ? noise[i] : 0.0f);
+  out[i] = sched_update(k, sample[i], eps[i], noise && k.sigma != 0.0f ? noise[i] : 0.0f);
 }
 
 // feats2joints (mld/data/HumanML3D.py:41-45 -> motion_process.py:415-431, 362-381;

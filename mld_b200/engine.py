@@ -221,6 +221,23 @@ class Engine:
             if host is not None and (int(host.max()) > T or int(host.min()) < 1):
                 raise ValueError(f"lengths must lie in [1, {T}]")
 
+    @property
+    def stochastic(self) -> bool:
+        """True when the scheduler adds noise at its steps (DDPM, or DDIM with eta > 0): the sampling calls
+        then need ``step_noise`` [n_steps, B, ...] of N(0,1) draws."""
+        return self.cfg.sched_kind == _lib.SCHED_DDPM or self.cfg.eta > 0.0
+
+    def _step_noise(self, step_noise: Optional[torch.Tensor], latent_shape, device=None) -> Optional[torch.Tensor]:
+        """``step_noise`` as a contiguous fp32 tensor on ``device`` (default: the engine's), shape-checked
+        against [n_steps, *latent_shape]."""
+        if step_noise is None:
+            return None
+        sn = step_noise.to(device=self.device if device is None else device, dtype=torch.float32).contiguous()
+        n_steps = 0 if self.timesteps is None else len(self.timesteps)
+        if tuple(sn.shape) != (n_steps, *latent_shape):
+            raise ValueError(f"step_noise must be [{n_steps}, {', '.join(map(str, latent_shape))}], got {tuple(sn.shape)}")
+        return sn
+
     # ------------------------------------------------------------------ denoiser
     def _cond(self, cond: torch.Tensor) -> torch.Tensor:
         if self.cfg.cond_kind == _lib.COND_TEXT:
@@ -260,11 +277,7 @@ class Engine:
         S = c.shape[1] if c.dim() == 3 else 1
         T = z0.shape[1] if self.cfg.diffusion_only else 0
         out = torch.empty((z0.shape[1], B, z0.shape[2]), dtype=torch.float32, device=self.device)
-        sn = None if step_noise is None else _f32c(step_noise, self.device)
-        if sn is not None:
-            n_steps = 0 if self.timesteps is None else len(self.timesteps)
-            if tuple(sn.shape) != (n_steps, *z0.shape):
-                raise ValueError(f"step_noise must be [{n_steps}, {', '.join(map(str, z0.shape))}], got {tuple(sn.shape)}")
+        sn = self._step_noise(step_noise, z0.shape)
         check(self.lib.mldb_diffusion_reverse(self._h, _ptr(c), _ptr(z0), _ptr(sn), _ptr(ln), B, S, T,
                                               _ptr(out), self._stream()), "mldb_diffusion_reverse")
         return out
@@ -309,10 +322,14 @@ class Engine:
         return out
 
     # ------------------------------------------------------------------ fused sample
-    def sample(self, cond: torch.Tensor, init_noise: torch.Tensor, lengths, want=("joints",)):
+    def sample(self, cond: torch.Tensor, init_noise: torch.Tensor, lengths, want=("joints",), *,
+               step_noise: Optional[torch.Tensor] = None):
         """reverse diffusion -> decode -> feats2joints on device tensors.  Returns a dict with the
-        requested subset of {"latents" [n_lat,B,d], "feats" [B,T,F], "joints" [B,T,J,3]}."""
+        requested subset of {"latents" [n_lat,B,d], "feats" [B,T,F], "joints" [B,T,J,3]}.
+        ``step_noise`` [n_steps, B, n_lat, d]: the N(0,1) draws of the scheduler steps, required when
+        :attr:`stochastic` (as for :meth:`diffusion_reverse`)."""
         c, z0 = self._cond(cond), _f32c(init_noise, self.device)
+        sn = self._step_noise(step_noise, z0.shape)
         ln = self._lengths(lengths)
         B = z0.shape[0]
         self._check_latent(z0, B, "init_noise")
@@ -332,7 +349,7 @@ class Engine:
         if "joints" in want:
             jo = out["joints"] = torch.empty((B, T, cfg.njoints, 3), dtype=torch.float32, device=self.device)
         check(self.lib.mldb_sample(self._h, _ptr(c), _ptr(z0), _ptr(ln), B, S, T, _ptr(lat), _ptr(fe),
-                                   _ptr(jo), self._stream()), "mldb_sample")
+                                   _ptr(jo), self._stream(), _ptr(sn)), "mldb_sample")
         return out
 
     # ------------------------------------------------------------------ multi-GPU (one process per GPU)
@@ -365,12 +382,14 @@ class Engine:
         return out
 
     def sample_gather(self, cond: torch.Tensor, init_noise: torch.Tensor, lengths, T: Optional[int] = None,
-                      out: Optional[torch.Tensor] = None, wait: bool = True) -> torch.Tensor:
+                      out: Optional[torch.Tensor] = None, wait: bool = True, *,
+                      step_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         """This rank's shard through ``mldb_sample_gather``: joints of ALL ranks ``[world * B, T, J, 3]``.
         ``T`` must be the same on every rank (pad to the global max length).  ``wait=False`` leaves the gather
         running on the side stream (call :meth:`gather_wait` before reading ``out``; alternate two ``out``
-        buffers between consecutive calls)."""
+        buffers between consecutive calls).  ``step_noise`` is this rank's shard [n_steps, B, n_lat, d]."""
         c, z0 = self._cond(cond), _f32c(init_noise, self.device)
+        sn = self._step_noise(step_noise, z0.shape)
         ln = self._lengths(lengths)
         B = z0.shape[0]
         self._check_latent(z0, B, "init_noise")
@@ -385,8 +404,8 @@ class Engine:
             out = torch.empty(shape, dtype=torch.float32, device=self.device)
         elif tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous():
             raise ValueError(f"out must be a contiguous float32 {list(shape)} tensor")
-        check(self.lib.mldb_sample_gather(self._h, _ptr(c), _ptr(z0), _ptr(ln), B, S, T, _ptr(out), self._stream()),
-              "mldb_sample_gather")
+        check(self.lib.mldb_sample_gather(self._h, _ptr(c), _ptr(z0), _ptr(ln), B, S, T, _ptr(out), self._stream(),
+                                          _ptr(sn)), "mldb_sample_gather")
         if wait:
             self.gather_wait()
         return out
@@ -395,10 +414,15 @@ class Engine:
         check(self.lib.mldb_gather_wait(self._h, self._stream()), "mldb_gather_wait")
 
     def sample_host(self, cond_cpu: torch.Tensor, noise_cpu: torch.Tensor, lengths_cpu: torch.Tensor,
-                    joints_cpu: torch.Tensor, T: int):
+                    joints_cpu: torch.Tensor, T: int, *, step_noise: Optional[torch.Tensor] = None):
         """End-to-end through HOST buffers (pinned recommended); asynchronous on the current
-        stream - synchronise before reading ``joints_cpu``."""
+        stream - synchronise before reading ``joints_cpu``.  ``step_noise``: contiguous f32 HOST tensor
+        [n_steps, B, n_lat, d], as for :meth:`sample`."""
         B = noise_cpu.shape[0]
+        if step_noise is not None and (step_noise.device.type != "cpu" or step_noise.dtype != torch.float32
+                                       or not step_noise.is_contiguous()):
+            raise ValueError("sample_host takes step_noise as a contiguous f32 HOST tensor")
+        sn = self._step_noise(step_noise, noise_cpu.shape, device="cpu")
         S = cond_cpu.shape[1] if cond_cpu.dim() == 3 else 1
         for t, dt in ((cond_cpu, torch.float32 if self.cfg.cond_kind == _lib.COND_TEXT else torch.int64),
                       (noise_cpu, torch.float32), (lengths_cpu, torch.int32), (joints_cpu, torch.float32)):
@@ -411,7 +435,7 @@ class Engine:
         if joints_cpu.numel() != world * B * T * self.cfg.njoints * 3:
             raise ValueError(f"joints buffer must hold [{world * B}, {T}, {self.cfg.njoints}, 3] floats")
         check(self.lib.mldb_sample_host(self._h, _ptr(cond_cpu), _ptr(noise_cpu), _ptr(lengths_cpu), B, S, T,
-                                        _ptr(joints_cpu), self._stream()), "mldb_sample_host")
+                                        _ptr(joints_cpu), self._stream(), _ptr(sn)), "mldb_sample_host")
         return joints_cpu
 
 
@@ -422,9 +446,15 @@ def make_config(*, condition: str = "text", arch: str = "trans_enc", latent_dim:
                 vae: str = "mld", vae_layers: Optional[int] = None, vae_heads: int = 4, vae_ff: int = 1024,
                 vae_nfeats: Optional[int] = None, scheduler: str = "ddim", num_train_timesteps: int = 1000,
                 beta_start: float = 0.00085, beta_end: float = 0.012, steps_offset: int = 1,
-                set_alpha_to_one: bool = False, eta: float = 0.0, njoints: int = 22) -> MldbConfig:
+                set_alpha_to_one: bool = False, eta: float = 0.0, njoints: int = 22,
+                beta_schedule: str = "scaled_linear", clip_sample: bool = False) -> MldbConfig:
     """Build an ``mldb_config`` from the reference's ctor kwargs / yaml params
-    (configs/modules/{denoiser,motion_vae,scheduler}.yaml)."""
+    (configs/modules/{denoiser,motion_vae,scheduler}.yaml).  ``eta`` (the yaml's scheduler.eta, in [0, 1]),
+    ``beta_schedule`` (scaled_linear | linear | squaredcos_cap_v2) and ``clip_sample`` are diffusers'."""
+    if beta_schedule not in _lib.BETA_SCHEDULES:
+        raise ValueError(f"beta_schedule must be one of {sorted(_lib.BETA_SCHEDULES)}, got {beta_schedule!r}")
+    if not 0.0 <= eta <= 1.0:
+        raise ValueError(f"eta must lie in [0, 1], got {eta}")
     c = _lib.default_config()
     c.cond_kind = {"text": _lib.COND_TEXT, "action": _lib.COND_ACTION}[condition]
     c.arch = {"trans_enc": _lib.ARCH_TRANS_ENC, "trans_dec": _lib.ARCH_TRANS_DEC}[arch]
@@ -440,4 +470,5 @@ def make_config(*, condition: str = "text", arch: str = "trans_enc", latent_dim:
     c.sched_kind = {"ddim": _lib.SCHED_DDIM, "ddpm": _lib.SCHED_DDPM}[scheduler]
     c.num_train_timesteps, c.beta_start, c.beta_end = num_train_timesteps, beta_start, beta_end
     c.steps_offset, c.set_alpha_to_one, c.eta, c.njoints = steps_offset, int(set_alpha_to_one), eta, njoints
+    c.beta_schedule, c.clip_sample = _lib.BETA_SCHEDULES[beta_schedule], int(clip_sample)
     return c

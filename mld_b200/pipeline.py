@@ -14,11 +14,13 @@ The text encoder is a separate callable ``text_encoder(List[str]) -> Tensor[2B, 
 """
 from __future__ import annotations
 
+import ctypes as C
 from types import SimpleNamespace
 from typing import Callable, Dict, List, Optional, Sequence
 
 import torch
 
+from . import _lib
 from .engine import Engine, make_config
 
 
@@ -43,15 +45,38 @@ class B200Scheduler:
     def scale_model_input(self, sample, timestep=None):
         return sample
 
-    def step(self, model_output, timestep, sample, eta: float = 0.0, noise=None, **kw):
-        if eta != 0.0:
-            raise NotImplementedError("only eta == 0 (the shipped config) is built")
+    def step(self, model_output, timestep, sample, eta: float = 0.0, noise=None, generator=None,
+             variance_noise=None, **kw):
+        """``DDIMScheduler.step`` / ``DDPMScheduler.step``.  The step adds noise when the scheduler is DDIM with
+        ``eta > 0`` or DDPM at ``t > 0``.  That N(0,1) tensor is ``variance_noise`` (``noise`` is the same
+        argument under its earlier name); when it is not given it is drawn here as current diffusers' ``randn_tensor``
+        does: ``torch.randn(model_output.shape, generator=generator, device=model_output.device,
+        dtype=model_output.dtype)``.  Older diffusers releases drew it on the CPU and moved it to the device, so
+        their seeded runs give other numbers.  The DDIM coefficients are built in the library from the
+        configured ``eta`` (``make_config(eta=...)``); ``eta`` here must equal it."""
+        cfg = self._e.cfg
+        ddim = cfg.sched_kind == _lib.SCHED_DDIM
+        if ddim and C.c_float(eta).value != cfg.eta:
+            raise ValueError(f"eta={eta} differs from the configured eta={cfg.eta}; build the model with that eta")
+        if variance_noise is not None:
+            noise = variance_noise
+        if generator is not None and noise is not None:
+            raise ValueError("pass either generator or variance_noise, not both")
         t = int(timestep.reshape(-1)[0]) if torch.is_tensor(timestep) else int(timestep)
+        if noise is None and (eta > 0 if ddim else t > 0):
+            noise = torch.randn(model_output.shape, generator=generator, device=model_output.device,
+                                dtype=model_output.dtype)
         return SimpleNamespace(prev_sample=self._e.scheduler_step(model_output, t, sample, noise))
 
 
 class B200MLD:
-    """Text/action-to-motion sampler with the reference ``MLD`` call surface."""
+    """Text/action-to-motion sampler with the reference ``MLD`` call surface.
+
+    ``cfg_kwargs`` are :func:`make_config`'s, the scheduler's among them: ``scheduler``, ``eta``,
+    ``beta_schedule``, ``clip_sample``, ...  When the scheduler adds noise at its steps (DDIM with ``eta > 0``,
+    DDPM), :meth:`forward` draws with torch's default generator in the reference's order: the initial latents,
+    then one ``[B, n_lat, d]`` draw per step (DDPM: none for the last step, ``t == 0``, whose slice stays zero).
+    ``batch["init_noise"]`` and ``batch["step_noise"]`` ([n_steps, B, n_lat, d]) replace those draws."""
 
     def __init__(self, denoiser_sd: Dict[str, torch.Tensor], vae_sd: Dict[str, torch.Tensor], *,
                  mean: torch.Tensor, std: torch.Tensor, text_encoder: Optional[Callable] = None,
@@ -83,7 +108,10 @@ class B200MLD:
                 B = len(lengths)
                 noise = torch.randn((B, self.latent_dim[0], self.latent_dim[-1]), device=self.device,
                                     dtype=torch.float)
-            out = self.engine.sample(text_emb, noise, lengths, want=("joints",))
+            step_noise = batch.get("step_noise")
+            if step_noise is None:
+                step_noise = self._draw_step_noise(noise.shape[0])
+            out = self.engine.sample(text_emb, noise, lengths, want=("joints",), step_noise=step_noise)
             joints = out["joints"]
         elif self.stage == "vae":
             z, _ = self._encode_motion(batch["motion"], lengths)
@@ -112,15 +140,33 @@ class B200MLD:
 
     # -- mld.py:290-360 ------------------------------------------------------------------
     def _diffusion_reverse(self, encoder_hidden_states: torch.Tensor, lengths=None,
-                           init_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+                           init_noise: Optional[torch.Tensor] = None,
+                           step_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         bsz = encoder_hidden_states.shape[0]
         if self.do_classifier_free_guidance:
             bsz = bsz // 2
         if init_noise is None:
             init_noise = torch.randn((bsz, self.latent_dim[0], self.latent_dim[-1]), device=self.device,
                                      dtype=torch.float)
+        if step_noise is None:
+            step_noise = self._draw_step_noise(bsz)
         return self.engine.diffusion_reverse(encoder_hidden_states, init_noise * self.scheduler.init_noise_sigma,
-                                             lengths)
+                                             lengths, step_noise=step_noise)
+
+    def _draw_step_noise(self, B: int) -> Optional[torch.Tensor]:
+        """The N(0,1) draws of the reference loop's ``scheduler.step`` calls (mld.py:345), in its order, as
+        ``[n_steps, B, n_lat, d]``: DDIM with eta > 0 draws at every step, DDPM at every step with t > 0
+        (the slice of a step that draws nothing is zero).  None when no step draws (DDIM, eta == 0)."""
+        if not self.engine.stochastic:
+            return None
+        shape = (B, self.latent_dim[0], self.latent_dim[-1])
+        ddpm = self.cfg.sched_kind == _lib.SCHED_DDPM
+        ts = self.scheduler.timesteps.tolist()
+        out = torch.zeros((len(ts), *shape), device=self.device, dtype=torch.float)
+        for i, t in enumerate(ts):
+            if not (ddpm and t == 0):
+                out[i] = torch.randn(shape, device=self.device, dtype=torch.float)
+        return out
 
     def _encode_motion(self, motion: torch.Tensor, lengths: Sequence[int]):
         mu, logvar = self.engine.vae_encode(motion, lengths)
