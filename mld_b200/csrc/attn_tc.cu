@@ -9,7 +9,7 @@
 // persistent) runs TWO independent pipelines, each a consumer warpgroup with its own Q buffer and
 // K / V ring and its own TMA warp in the producer warpgroup; while one warpgroup is in its softmax the
 // other one's MMAs keep the tensor cores busy.  Keys are processed in blocks of 64 (the last block
-// padded to a multiple of 16):
+// padded to a multiple of 16 with zero rows, never with the next sequence's keys):
 //   S[:, kb]  = Q K_kb^T            M = 64, N = 64, K = head_dim            (A, B K-major in shared memory)
 //   P         = exp2(scale*(S - max))  two exact passes over the WHOLE score row, which lives in
 //                                   registers (<= 256 columns) - no online rescaling
@@ -161,11 +161,17 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
             const uint32_t full = smem_u32(&r_full[sl_i]);
             mbar_expect_tx(full, (uint32_t)(2 * NS * rows * 128));
             const uint32_t base = smem_u32(sR + sl_i * SLOT_BYTES);
-            const int r0 = it.s * p.Lk + kb * KBLK;
+            // the last block's rows past Lk would be the next sequence's first keys: its [seq, key, col] map
+            // zero-fills them, since P = 0 times a non-finite V is NaN
 #pragma unroll
             for (int sl = 0; sl < NS; ++sl) {
-              tma_load_2d(base + sl * TILE, last ? &tmRh : &tmKh, full, col0 + sl * 64, r0);
-              tma_load_2d(base + SL_PLANE + sl * TILE, last ? &tmRl : &tmKl, full, col0 + sl * 64, r0);
+              if (last) {
+                tma_load_3d(base + sl * TILE, &tmRh, full, col0 + sl * 64, kb * KBLK, it.s);
+                tma_load_3d(base + SL_PLANE + sl * TILE, &tmRl, full, col0 + sl * 64, kb * KBLK, it.s);
+              } else {
+                tma_load_2d(base + sl * TILE, &tmKh, full, col0 + sl * 64, it.s * p.Lk + kb * KBLK);
+                tma_load_2d(base + SL_PLANE + sl * TILE, &tmKl, full, col0 + sl * 64, it.s * p.Lk + kb * KBLK);
+              }
             }
           }
           __syncwarp();
@@ -349,6 +355,16 @@ bool make_map(CUtensorMap* m, const __half* base, int rows, int cols, int box_ro
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
+// the same plane seen as [nseq, L, cols]: a box never reaches past its own sequence, rows >= L are zero-filled
+bool make_seq_map(CUtensorMap* m, const __half* base, int nseq, int L, int cols, int box_rows) {
+  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)L, (cuuint64_t)nseq};
+  cuuint64_t strides[2] = {(cuuint64_t)cols * sizeof(__half), (cuuint64_t)L * cols * sizeof(__half)};
+  cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
+  cuuint32_t estr[3] = {1, 1, 1};
+  return g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)base, dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
 
 // launch geometry for a shape; false when it does not fit
 bool plan_shape(const AttnArgs& a, AtcParams* p) {
@@ -399,7 +415,8 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   CUtensorMap mQh, mQl, mKh, mKl, mRh, mRl;
   const bool ok = make_map(&mQh, a.q.hi, a.q.rows, a.q.cols, QROWS) && make_map(&mQl, a.q.lo(), a.q.rows, a.q.cols, QROWS) &&
                   make_map(&mKh, a.kv.hi, a.kv.rows, a.kv.cols, KBLK) && make_map(&mKl, a.kv.lo(), a.kv.rows, a.kv.cols, KBLK) &&
-                  make_map(&mRh, a.kv.hi, a.kv.rows, a.kv.cols, p.rem) && make_map(&mRl, a.kv.lo(), a.kv.rows, a.kv.cols, p.rem);
+                  make_seq_map(&mRh, a.kv.hi, a.nseq, a.Lk, a.kv.cols, p.rem) &&
+                  make_seq_map(&mRl, a.kv.lo(), a.nseq, a.Lk, a.kv.cols, p.rem);
   if (!ok) return false;
   p.nseq = a.nseq; p.heads = a.heads; p.Lq = a.Lq; p.Lk = a.Lk;
   p.q_col0 = a.q_col0; p.k_col0 = a.k_col0; p.v_col0 = a.v_col0;
