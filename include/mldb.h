@@ -250,7 +250,7 @@ int mldb_debug_timeline(int32_t enable, int64_t* out, int32_t cap, int32_t* coun
  * split16 planes (the production path; N % 8 == 0) which are then widened to fp32.  Synchronous.
  * R given without gamma selects the residual-add epilogue out = A W^T + b + R (fp32 output, act must be 0 on
  * the wgmma path; R == out runs it in place, as the text tower does).  act: 0 none, 1 GELU, 2 ReLU, 3 SiLU,
- * 4 quick-GELU x * sigmoid(1.702 x) (CLIP).  N up to 4096 runs on the wgmma kernel here. */
+ * 4 quick-GELU x * sigmoid(1.702 x) (CLIP), 5 LeakyReLU(0.2) (T2M evaluator).  N up to 4096 runs on the wgmma kernel here. */
 int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float* bias, const float* gamma,
                     const float* beta, const float* R, int32_t M, int32_t N, int32_t K, int32_t K1,
                     int32_t act, int32_t use_tc, int32_t split_out, float* out, void* stream);
@@ -313,6 +313,50 @@ int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg);
  * indices with gemm=simt / attn=simt), the row LayerNorms under MLDB_KSTAT_TEXT_LN. */
 int mldb_text_encode(mldb_handle* h, const int64_t* ids, int32_t n, int32_t L, int32_t mode, float* out, void* stream);
 
+/* ---- T2M evaluator (MLD.t2m_eval, mld/models/modeltype/mld.py:618-708): the movement, motion and text encoders of
+ * Guo et al.'s text-motion matching model (mld/models/architectures/t2m_motionenc.py, t2m_textenc.py) whose embeddings
+ * feed R-precision, matching score, FID, diversity and MultiModality.  Weights come from finest.tar (keys text_encoder,
+ * movement_encoder, motion_encoder), in eval mode (dropout is the identity). */
+#define MLDB_T2M_ABI_VERSION 1
+#define MLDB_T2M_TEXT 1       /* parts: TextEncoderBiGRUCo      keys "t2m_textencoder."   + its state_dict keys */
+#define MLDB_T2M_MOVEMENT 2   /* parts: MovementConvEncoder     keys "t2m_moveencoder."   */
+#define MLDB_T2M_MOTION 4     /* parts: MotionEncoderBiGRUCo    keys "t2m_motionencoder." */
+typedef struct mldb_t2m_config {
+  int32_t abi_version;        /* must be MLDB_T2M_ABI_VERSION */
+  int32_t parts;              /* MLDB_T2M_* mask: only these modules' keys are expected (strict) */
+  int32_t dim_word;           /* model.t2m_textencoder.dim_word 300 */
+  int32_t dim_pos_ohot;       /* dim_pos_ohot 15 */
+  int32_t dim_text_hidden;    /* dim_text_hidden 512 (GRU hidden: a multiple of 64, <= 1024) */
+  int32_t dim_coemb_hidden;   /* dim_coemb_hidden 512 (text embedding) */
+  int32_t dim_pose;           /* movement input_size = DATASET.NFEATS - 4 = 259 */
+  int32_t dim_move_hidden;    /* model.t2m_motionencoder.dim_move_hidden 512 (a multiple of 64) */
+  int32_t dim_move_latent;    /* dim_move_latent 512 (a multiple of 64) */
+  int32_t dim_motion_hidden;  /* dim_motion_hidden 1024 (GRU hidden: a multiple of 64, <= 1024) */
+  int32_t dim_motion_latent;  /* dim_motion_latent 512 (motion embedding) */
+} mldb_t2m_config;
+void mldb_default_t2m_config(mldb_t2m_config* cfg);
+/* Add the configured parts' keys to the strict key spec; after mldb_create, before mldb_finalize_weights. */
+int mldb_t2m_configure(mldb_handle* h, const mldb_t2m_config* cfg);
+/* Replaces: MovementConvEncoder.forward(x) (t2m_motionenc.py:21-25), no length mask (as the reference: every one of
+ * the T frames is read, padding frames included).
+ *   x    [B, T, dim_pose] with a row stride of ld >= dim_pose floats (ld = 263 passes feats[..., :-4] uncopied), T >= 4
+ *   out  [B, (T / 2) / 2, dim_move_latent] */
+int mldb_t2m_movement(mldb_handle* h, const float* x, int32_t ld, int32_t B, int32_t T, float* out, void* stream);
+/* Replaces: MotionEncoderBiGRUCo.forward(x, m_lens) (t2m_motionenc.py:51-64).
+ *   x        [B, L, dim_move_latent];  lengths  device int32 [B], any order, each in [1, L] (values outside are
+ *            clamped; the torch module rejects them, as pack_padded_sequence does)
+ *   out      [B, dim_motion_latent] */
+int mldb_t2m_motion(mldb_handle* h, const float* x, const int32_t* lengths, int32_t B, int32_t L, float* out,
+                    void* stream);
+/* Replaces: TextEncoderBiGRUCo.forward(word_embs, pos_ohot, cap_lens) (t2m_textenc.py:33-48).
+ *   word_embs [B, L, dim_word]; pos_ohot [B, L, dim_pos_ohot]; lengths as above; out [B, dim_coemb_hidden] */
+int mldb_t2m_text(mldb_handle* h, const float* word_embs, const float* pos_ohot, const int32_t* lengths, int32_t B,
+                  int32_t L, float* out, void* stream);
+/* All three run eagerly on `stream` in batch chunks that bound the workspace (which grows on demand, outside any
+ * capture, and synchronises the device when it does).  Every sequence is computed independently of the others and
+ * of the chunking.  The GEMMs count under MLDB_KSTAT_GEMM_TC (GEMM_SIMT with gemm=simt), the recurrent steps under
+ * MLDB_KSTAT_GRU_TC (with gemm=simt: two GEMM_SIMT and one MISC gate kernel per step). */
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);
@@ -332,7 +376,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
 #define MLDB_KSTAT_LN_UNFUSED 8   /* k_ln behind a GEMM whose LayerNorm could NOT be fused (a fallback) */
 #define MLDB_KSTAT_MISC 9         /* token assembly, scheduler step, feats2joints, ... */
 #define MLDB_KSTAT_TEXT_LN 10     /* k_text_ln: the text tower's row LayerNorm (+ embedding / eos gather) */
-#define MLDB_KSTAT_COUNT 11
+#define MLDB_KSTAT_GRU_TC 11      /* k_gru_step_tc: one recurrent step of the T2M evaluator's bidirectional GRU */
+#define MLDB_KSTAT_COUNT 12
 int mldb_kernel_stats(const mldb_handle* h, int64_t* out, int32_t n);
 int mldb_reset_kernel_stats(mldb_handle* h);
 
@@ -347,6 +392,7 @@ int mldb_reset_kernel_stats(mldb_handle* h);
  *                                        summed in a different order, so they depend on the batch size in the last bits
  *   "branches"   1..4                   concurrent sub-batch branches inside a denoiser step (2)      MLDB_BRANCHES
  *   "graph"      0 | 1                  CUDA-graph replay of the step loop (1)                        MLDB_GRAPH
+ *   "t2m_chunk"  0 | n                  T2M evaluator: sequences per batch chunk (0: sized from the workspace budget)
  * Environment only: MLDB_PDL (programmatic dependent launch, 1); MLDB_SNAKE (1: attention and the fused FFN walk
  * the token tiles downwards, the GEMMs upwards, so every kernel starts on the rows its producer wrote last). */
 int mldb_set_option(mldb_handle* h, const char* name, const char* value);

@@ -22,10 +22,13 @@ BETA_SCHEDULES = {"scaled_linear": 0, "linear": 1, "squaredcos_cap_v2": 2}
 DTYPE_F32 = 0
 # mldb_kernel_stats indices (MLDB_KSTAT_* in include/mldb.h)
 KSTAT_NAMES = ("gemm_tc", "gemm_ln_tc", "ffn_tc", "attn_tc", "attn_mma", "attn_simt", "gemm_simt", "ln_simt",
-               "ln_unfused", "misc", "text_ln")
+               "ln_unfused", "misc", "text_ln", "gru_tc")
 # CLIP text tower (mldb_text_config, mldb_text_encode)
 MLDB_TEXT_ABI_VERSION = 1
 TEXT_HIDDEN, TEXT_POOLED = 0, 1
+# T2M evaluator (mldb_t2m_config, mldb_t2m_*)
+MLDB_T2M_ABI_VERSION = 1
+T2M_TEXT, T2M_MOVEMENT, T2M_MOTION = 1, 2, 4
 
 
 class MldbConfig(C.Structure):
@@ -52,6 +55,16 @@ class MldbTextConfig(C.Structure):
         ("abi_version", C.c_int32), ("vocab_size", C.c_int32), ("max_positions", C.c_int32),
         ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32), ("ff", C.c_int32),
         ("projection_dim", C.c_int32), ("eos_token_id", C.c_int32), ("ln_eps", C.c_float),
+    ]
+
+
+class MldbT2mConfig(C.Structure):
+    """``mldb_t2m_config`` (include/mldb.h)."""
+    _fields_ = [
+        ("abi_version", C.c_int32), ("parts", C.c_int32), ("dim_word", C.c_int32), ("dim_pos_ohot", C.c_int32),
+        ("dim_text_hidden", C.c_int32), ("dim_coemb_hidden", C.c_int32), ("dim_pose", C.c_int32),
+        ("dim_move_hidden", C.c_int32), ("dim_move_latent", C.c_int32), ("dim_motion_hidden", C.c_int32),
+        ("dim_motion_latent", C.c_int32),
     ]
 
 
@@ -88,6 +101,11 @@ _SIGNATURES = {
     "mldb_default_text_config": (None, [C.POINTER(MldbTextConfig)]),
     "mldb_text_configure": (C.c_int, [_P, C.POINTER(MldbTextConfig)]),
     "mldb_text_encode": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_default_t2m_config": (None, [C.POINTER(MldbT2mConfig)]),
+    "mldb_t2m_configure": (C.c_int, [_P, C.POINTER(MldbT2mConfig)]),
+    "mldb_t2m_movement": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_t2m_motion": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_t2m_text": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
@@ -140,4 +158,10 @@ def default_config() -> MldbConfig:
 def default_text_config() -> MldbTextConfig:
     cfg = MldbTextConfig()
     lib().mldb_default_text_config(C.byref(cfg))
+    return cfg
+
+
+def default_t2m_config() -> MldbT2mConfig:
+    cfg = MldbT2mConfig()
+    lib().mldb_default_t2m_config(C.byref(cfg))
     return cfg

@@ -86,7 +86,7 @@ static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 #endif
 
-enum ActKind { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3, ACT_QUICKGELU = 4 };
+enum ActKind { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2, ACT_SILU = 3, ACT_QUICKGELU = 4, ACT_LEAKY = 5 };
 
 __device__ __forceinline__ float apply_act(float v, int act) {
   switch (act) {
@@ -94,6 +94,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     case ACT_RELU: return fmaxf(v, 0.0f);
     case ACT_SILU: return silu_f(v);
     case ACT_QUICKGELU: return quick_gelu_f(v);
+    case ACT_LEAKY: return v > 0.0f ? v : v * 0.2f;   // nn.LeakyReLU(0.2) (the T2M evaluator)
     default: return v;
   }
 }

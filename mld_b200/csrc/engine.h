@@ -53,6 +53,29 @@ struct TextW {
   std::vector<void*> ws_allocs;
 };
 
+// T2M evaluator (mldb_t2m_configure): bidirectional GRU + BiGRUCo head, the movement convolutions
+struct GruW {
+  int H = 0;
+  LinW w_ih[2];                   // per direction [3H, in], gates r | z | n, bias b_ih
+  LinW w_hh;                      // both directions [2 * 3H, H], rows in gru_packed_col order, no bias
+  float* b_hh = nullptr;          // [2][3H] fp32
+  float* h0 = nullptr;            // the learned `hidden` [2][H]
+  LinW head1, head2;              // output_net.0 (2H -> H), output_net.3 (H -> out)
+  LnW ln;                         // output_net.1
+};
+struct T2mW {
+  bool on = false;
+  mldb_t2m_config cfg{};
+  LinW pos_emb, text_in;          // text: pos_emb (K padded to 64), input_emb (K padded to 64)
+  LinW conv1, conv2, move_out;    // movement: main.0 / main.3 as [out, 4 * Cp] operands, out_net
+  LinW motion_in;                 // motion: input_emb
+  GruW text_gru, motion_gru;
+  int chunk = 0;                  // option t2m_chunk (0: from the workspace budget)
+  static constexpr int NBUF = 10;
+  void* buf[NBUF] = {};           // workspace slots, grown on demand
+  size_t cap[NBUF] = {};
+};
+
 struct RawTensor {
   std::vector<float> host;
   std::vector<int64_t> shape;
@@ -123,6 +146,7 @@ struct mldb_handle {
   float* global_token = nullptr;     // [2*n_lat, d]
   float* mean = nullptr; float* stdv = nullptr; int nstat = 0;
   TextW text;          // CLIP text tower (mldb_text_configure)
+  T2mW t2m;            // T2M evaluator (mldb_t2m_configure)
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;

@@ -18,6 +18,7 @@
 //   LayerNorm: BN == N == 256, so a quad owns COMPLETE rows: bias + residual, exact two-pass
 //              statistics over the registers with quad shuffles, normalise -> split16.
 //   residual:  bias + fp32 residual R -> fp32 (may run in place, out == R: the text tower's residual stream).
+//   fp32:      bias + activation -> fp32 with float2 stores, identity row mapping (GemmArgs::vec_f32: the T2M evaluator).
 #include "gemm_tc.h"
 
 #include <stdio.h>
@@ -59,7 +60,7 @@ struct TcParams {
   long long* tl; // debug timeline (nullptr normally)
 };
 
-enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2, EPI_RES = 3 };     // epilogue variants of k_gemm_tc (see the kernel)
+enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2, EPI_RES = 3, EPI_F32 = 4 };     // epilogue variants of k_gemm_tc (see the kernel)
 
 template <int BN>
 struct TileCfg {
@@ -161,8 +162,9 @@ __device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const flo
 // EPI selects the epilogue: EPI_FAST = plain, split16 output, identity row mapping, N a whole number of tiles
 // (the per-layer GEMMs); EPI_LN = residual + LayerNorm; EPI_GENERIC = plain with everything else (positional
 // table, row remapping, zeroed padding rows, fp32 output, ragged N: the per-batch embedding / final-layer
-// GEMMs) kept out of the hot kernels' instruction stream; EPI_RES = bias + fp32 residual -> fp32, N even.
-template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast epilogue's activation (NONE | GELU | QUICKGELU)
+// GEMMs) kept out of the hot kernels' instruction stream; EPI_RES = bias + fp32 residual -> fp32, N even;
+// EPI_F32 = bias + activation -> fp32, identity row mapping, N even.
+template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast / fp32 epilogue's activation (NONE | GELU | QUICKGELU | LEAKY)
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
           const __grid_constant__ CUtensorMap tmA2h, const __grid_constant__ CUtensorMap tmA2l,
@@ -290,6 +292,9 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
         if (ACT == ACT_QUICKGELU) {
           x0 = quick_gelu_f(x0); x1 = quick_gelu_f(x1); x2 = quick_gelu_f(x2); x3 = quick_gelu_f(x3);
         }
+        if (ACT == ACT_LEAKY) {
+          x0 = apply_act(x0, ACT_LEAKY); x1 = apply_act(x1, ACT_LEAKY); x2 = apply_act(x2, ACT_LEAKY); x3 = apply_act(x3, ACT_LEAKY);
+        }
         if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x0, x1);
         if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x2, x3);
       }
@@ -308,6 +313,20 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
           const float2 r = *reinterpret_cast<const float2*>(p.res_f32 + o);
           *reinterpret_cast<float2*>(p.out_f32 + o) =
               make_float2(fmaf(d[4 * j + 2 * h], sc, b.x) + r.x, fmaf(d[4 * j + 2 * h + 1], sc, b.y) + r.y);
+        }
+      }
+    } else if constexpr (EPI == EPI_F32) {
+      const float sc = p.inv_scale;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + cp;
+        if (n >= p.N) continue;                        // N even: a column pair is in or out together
+        const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (r_lo + 8 * h >= p.M) continue;
+          const float x0 = apply_act(fmaf(d[4 * j + 2 * h], sc, b.x), ACT), x1 = apply_act(fmaf(d[4 * j + 2 * h + 1], sc, b.y), ACT);
+          *reinterpret_cast<float2*>(p.out_f32 + (int64_t)(r_lo + 8 * h) * p.ldc + n) = make_float2(x0, x1);
         }
       }
     } else {
@@ -644,6 +663,9 @@ TcCtx* tc_create(int device) {
   opt_in(k_gemm_tc<128, EPI_FAST, ACT_QUICKGELU>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_RES>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_RES>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_LN>, TileCfg<256>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_FAST, ACT_LEAKY>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST, ACT_LEAKY>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_F32>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_F32>, TileCfg<128>::SMEM_BYTES);
+  opt_in(k_gemm_tc<256, EPI_F32, ACT_LEAKY>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_F32, ACT_LEAKY>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_ffn_tc, FfnCfg::SMEM_BYTES);
   if (e != cudaSuccess) {
     mldb_set_err(std::string("cudaFuncSetAttribute(k_gemm_tc): ") + cudaGetErrorString(e));
@@ -733,7 +755,11 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   // the fast plain epilogue: split16 output, identity row mapping, N a whole number of tiles
   const bool fast = !ln && g.out.hi && !g.out_f32 && !g.addtab && !g.zero_lengths && g.in_group >= g.M &&
                     g.out_group == 0 && g.out_off == 0 && g.w.N % bn == 0 && g.w.bias != nullptr &&
-                    (g.act == ACT_NONE || g.act == ACT_GELU || g.act == ACT_QUICKGELU);
+                    (g.act == ACT_NONE || g.act == ACT_GELU || g.act == ACT_QUICKGELU || g.act == ACT_LEAKY);
+  // the vectorised fp32 epilogue, for callers that ask for it (vec_f32)
+  const bool f32 = !ln && g.vec_f32 && !g.out.hi && g.out_f32 && !g.res_f32 && !g.addtab && !g.zero_lengths &&
+                   g.in_group >= g.M && g.out_group == 0 && g.out_off == 0 && g.w.N % 2 == 0 && g.ldc % 2 == 0 &&
+                   ((uintptr_t)g.out_f32 & 7) == 0 && (g.act == ACT_NONE || g.act == ACT_LEAKY);
   const int ntiles = p.m_tiles * p.n_tiles;
   dim3 grid(ntiles < c->sm_count ? ntiles : c->sm_count);
 #define MLDB_LAUNCH(BN_, ...)                                                                                      \
@@ -747,6 +773,9 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   else if (g.res_f32)                 MLDB_LAUNCH_SHAPE(EPI_RES);
   else if (fast && g.act == ACT_GELU) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_GELU);
   else if (fast && g.act == ACT_QUICKGELU) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_QUICKGELU);
+  else if (fast && g.act == ACT_LEAKY) MLDB_LAUNCH_SHAPE(EPI_FAST, ACT_LEAKY);
+  else if (f32 && g.act == ACT_LEAKY) MLDB_LAUNCH_SHAPE(EPI_F32, ACT_LEAKY);
+  else if (f32)                       MLDB_LAUNCH_SHAPE(EPI_F32);
   else if (fast)                      MLDB_LAUNCH_SHAPE(EPI_FAST);
   else                                MLDB_LAUNCH_SHAPE(EPI_GENERIC);
 #undef MLDB_LAUNCH_SHAPE

@@ -39,6 +39,9 @@ struct GemmArgs {
   const float* res_f32 = nullptr;
   int wide_n = 0;                       // 1: the wgmma kernel may take N up to 4096 (the text tower's 2304 / 3072);
                                         // the sampling path keeps its N <= 1024 kernel selection
+  int vec_f32 = 0;                      // 1: fp32 output (no residual, identity rows, N even) through the wgmma kernel's
+                                        // vectorised epilogue fmaf(acc, scale, bias) (the T2M evaluator); the
+                                        // sampling path keeps the generic epilogue it was validated with
 };
 
 // y = LayerNorm(c + res + rowvec[r / rv_group]) * gamma + beta, eps 1e-5; optional second LN
@@ -53,6 +56,7 @@ struct LnArgs {
   // input row selection: in_row = (r / sel_group) * in_group + r % sel_group (identity default)
   int sel_group = 1 << 30, in_group = 0;
   ActBuf out{}; float* out_f32 = nullptr; int ld_out = 0;
+  int act = ACT_NONE;                        // activation on the normalised output (CUDA-core kernels only)
 };
 
 // Multi-head attention over per-sequence token groups.  Row of (seq s, token t) = s*L + t.
@@ -104,5 +108,33 @@ struct TextLnArgs {
 };
 bool text_ln_supported(int d);
 void text_ln(const TextLnArgs& a, cudaStream_t st);
+// --- bidirectional GRU of the T2M evaluator (gru_tc.cu) ---
+// State buffers are [2 * rows_pad, H]: direction d's row m at d * rows_pad + m (rows_pad a multiple of 128).
+struct GruStepArgs {
+  ActBuf h_in{}, h_out{};              // split16 state h_{s-1} (the MMA operand) / h_s
+  const float* hf_in = nullptr;        // fp32 state h_{s-1} (the z * h term and the copy-through)
+  float* hf_out = nullptr;
+  const float* gi = nullptr;           // [rows * L, 6H]: x_t W_ih^T + b_ih, forward then backward, gates r | z | n
+  const float* gh = nullptr;           // CUDA-core path: [2 * rows_pad, 3H] h W_hh^T in the packed column order
+  const float* b_hh = nullptr;         // [2][3H] fp32, gates r | z | n
+  const int32_t* lengths = nullptr;    // [rows] valid steps per sequence (clamped to [0, L])
+  const __half* w_hh = nullptr;        // packed W_hh planes [2][2 * 3H][H] (gru_packed_col order)
+  int64_t w_plane_stride = 0;
+  float w_inv_scale = 1.0f;
+  int rows = 0, rows_pad = 0, L = 0, H = 0, step = 0;
+};
+// column of gate g (0 r, 1 z, 2 n) of hidden unit u inside one direction's 3H packed rows: 32-unit tiles of 96 rows,
+// 8-row group 3 * jj + g holds units 8 * jj .. 8 * jj + 7 of the tile
+__host__ __device__ __forceinline__ int gru_packed_col(int g, int u) {
+  const int t = u >> 5, uu = u & 31;
+  return t * 96 + (3 * (uu >> 3) + g) * 8 + (uu & 7);
+}
+bool gru_tc_init(int device);                                    // once per process, outside stream capture
+bool gru_shape_supported(int H);                                 // 64 <= H <= 1024, H % 64 == 0
+bool gru_step_tc(const GruStepArgs& a, cudaStream_t st);         // false: tensor-map encoding failed, nothing launched
+void gru_gate_simt(const GruStepArgs& a, cudaStream_t st);       // the gate update from a.gh (CUDA cores)
+void gru_init_state(const GruStepArgs& a, const float* h0, cudaStream_t st);   // h_out / hf_out = h0 [2][H] per row
+// Conv1d(k = 4, stride 2, padding 1) im2col: src [rows / T_out sequences][T_in][ld] fp32 -> X [rows, 4 * Cp] split16
+void im2col_k4s2(ActBuf X, const float* src, int64_t ld, int T_in, int C, int Cp, int T_out, int rows, cudaStream_t st);
 // --- wgmma implementations (gemm_tc.cu) ---
 struct TcCtx;

@@ -163,6 +163,7 @@ __global__ void __launch_bounds__(256) k_ln(const LnArgs a) {
   for (int i = 0; i < VPL; ++i) {
     const int n = i * 32 + lane;
     if (n >= a.d) continue;
+    v[i] = apply_act(v[i], a.act);
     if (a.out.hi) {
       __half h, l;
       split_f32(v[i], h, l);
@@ -368,6 +369,11 @@ __global__ void __launch_bounds__(256) k_ln_vec(const LnArgs a) {
   (void)s;
   normalise(a.gamma, a.beta);
   if (a.gamma2) normalise(a.gamma2, a.beta2);   // stack-final LayerNorm on top (cross_attention.py:62-63)
+  if (a.act != ACT_NONE)
+#pragma unroll
+    for (int i = 0; i < NIT; ++i)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) v[i][k] = apply_act(v[i][k], a.act);
 #pragma unroll
   for (int i = 0; i < NIT; ++i) {
     const int n = i * 256 + lane * 8;

@@ -160,6 +160,73 @@ class Engine:
               "mldb_text_encode")
         return out
 
+    # ------------------------------------------------------------------ T2M evaluator
+    def t2m_configure(self, tcfg):
+        """Add the evaluator parts' keys (``t2m_textencoder.`` / ``t2m_moveencoder.`` / ``t2m_motionencoder.``) to the
+        strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_t2m_configure(self._h, C.byref(tcfg)), "mldb_t2m_configure")
+        self.t2m_cfg = tcfg
+
+    def _t2m(self, part: int, name: str):
+        tc = getattr(self, "t2m_cfg", None)
+        if tc is None or not tc.parts & part:
+            raise RuntimeError(f"the T2M {name} encoder was not configured (t2m_configure) before finalize()")
+        return tc
+
+    def _t2m_lengths(self, lengths, B: int, L: int) -> torch.Tensor:
+        ln = torch.as_tensor(lengths).reshape(-1)
+        if ln.numel() != B:
+            raise ValueError(f"lengths must hold {B} values, got {ln.numel()}")
+        if ln.dtype.is_floating_point or ln.dtype == torch.bool:
+            raise ValueError("lengths must be integers")
+        if B and (int(ln.min()) < 1 or int(ln.max()) > L):
+            raise ValueError(f"lengths must lie in [1, {L}]")
+        return ln.to(device=self.device, dtype=torch.int32).contiguous()
+
+    def t2m_movement(self, x: torch.Tensor) -> torch.Tensor:
+        """MovementConvEncoder: [B, T, dim_pose] (T >= 4; the last dimension may be a strided slice such as
+        ``feats[..., :-4]``) -> [B, T // 2 // 2, dim_move_latent]."""
+        tc = self._t2m(_lib.T2M_MOVEMENT, "movement")
+        if x.dim() != 3 or x.shape[2] != tc.dim_pose or x.shape[0] < 1 or x.shape[1] < 4:
+            raise ValueError(f"x must be [B >= 1, T >= 4, {tc.dim_pose}], got {tuple(x.shape)}")
+        x = x.to(device=self.device, dtype=torch.float32)
+        if x.stride(2) != 1 or x.stride(0) != x.shape[1] * x.stride(1):
+            x = x.contiguous()
+        B, T = x.shape[:2]
+        out = torch.empty((B, T // 2 // 2, tc.dim_move_latent), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_t2m_movement(self._h, _ptr(x), x.stride(1), B, T, _ptr(out), self._stream()),
+              "mldb_t2m_movement")
+        return out
+
+    def t2m_motion(self, x: torch.Tensor, lengths) -> torch.Tensor:
+        """MotionEncoderBiGRUCo: [B, L, dim_move_latent] + lengths (any order, each in [1, L]) -> [B, dim_motion_latent]."""
+        tc = self._t2m(_lib.T2M_MOTION, "motion")
+        if x.dim() != 3 or x.shape[2] != tc.dim_move_latent or x.shape[0] < 1 or x.shape[1] < 1:
+            raise ValueError(f"x must be [B >= 1, L >= 1, {tc.dim_move_latent}], got {tuple(x.shape)}")
+        xd = _f32c(x, self.device)
+        B, L = xd.shape[:2]
+        ln = self._t2m_lengths(lengths, B, L)
+        out = torch.empty((B, tc.dim_motion_latent), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_t2m_motion(self._h, _ptr(xd), _ptr(ln), B, L, _ptr(out), self._stream()), "mldb_t2m_motion")
+        return out
+
+    def t2m_text(self, word_embs: torch.Tensor, pos_ohot: torch.Tensor, lengths) -> torch.Tensor:
+        """TextEncoderBiGRUCo: word_embs [B, L, dim_word], pos_ohot [B, L, dim_pos_ohot] + lengths (any order, each
+        in [1, L]) -> [B, dim_coemb_hidden]."""
+        tc = self._t2m(_lib.T2M_TEXT, "text")
+        if word_embs.dim() != 3 or word_embs.shape[2] != tc.dim_word or word_embs.shape[0] < 1 or word_embs.shape[1] < 1:
+            raise ValueError(f"word_embs must be [B >= 1, L >= 1, {tc.dim_word}], got {tuple(word_embs.shape)}")
+        if tuple(pos_ohot.shape) != (*word_embs.shape[:2], tc.dim_pos_ohot):
+            raise ValueError(f"pos_ohot must be [{word_embs.shape[0]}, {word_embs.shape[1]}, {tc.dim_pos_ohot}], "
+                             f"got {tuple(pos_ohot.shape)}")
+        w, p = _f32c(word_embs, self.device), _f32c(pos_ohot, self.device)
+        B, L = w.shape[:2]
+        ln = self._t2m_lengths(lengths, B, L)
+        out = torch.empty((B, tc.dim_coemb_hidden), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_t2m_text(self._h, _ptr(w), _ptr(p), _ptr(ln), B, L, _ptr(out), self._stream()),
+              "mldb_t2m_text")
+        return out
+
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:
         """Which kernel each operator was enqueued on since the last reset (mldb_kernel_stats)."""
         arr = (C.c_int64 * len(_lib.KSTAT_NAMES))()

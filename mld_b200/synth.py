@@ -236,3 +236,89 @@ def clip_text_ids(n: int, L: int = 77, seed: int = 7, eos_lo: int = 8, eos_hi: i
     ids[:, 0] = bos
     ids[torch.arange(L).expand(n, L) >= pos[:, None]] = eos
     return ids
+
+
+# ---------------------------------------------------------------------------- T2M evaluator (finest.tar layout)
+T2M_DIMS = dict(dim_word=300, dim_pos_ohot=15, dim_text_hidden=512, dim_coemb_hidden=512, dim_pose=259,
+                dim_move_hidden=512, dim_move_latent=512, dim_motion_hidden=1024, dim_motion_latent=512)
+
+
+def _t2m_uniform(g: _Gen, bound: float, *shape) -> Tensor:
+    return (g.uniform(*shape) * 2 - 1) * bound
+
+
+def _t2m_linear(sd, g: _Gen, p: str, out_f: int, in_f: int, k: int = 1):
+    """torch's default Linear / Conv1d init: weight and bias U(-1/sqrt(fan_in), 1/sqrt(fan_in))."""
+    b = 1.0 / math.sqrt(in_f * k)
+    sd[p + "weight"] = _t2m_uniform(g, b, out_f, in_f, k) if k > 1 else _t2m_uniform(g, b, out_f, in_f)
+    sd[p + "bias"] = _t2m_uniform(g, b, out_f)
+
+
+def _t2m_bigru(sd, g: _Gen, in_f: int, H: int, out: int):
+    """nn.GRU(in_f, H, bidirectional) (default init U(-1/sqrt(H), 1/sqrt(H))), the learned initial state
+    ``hidden`` (torch.randn, as the reference) and the BiGRUCo output_net."""
+    b = 1.0 / math.sqrt(H)
+    for sfx in ("", "_reverse"):
+        sd["gru.weight_ih_l0" + sfx] = _t2m_uniform(g, b, 3 * H, in_f)
+        sd["gru.weight_hh_l0" + sfx] = _t2m_uniform(g, b, 3 * H, H)
+        sd["gru.bias_ih_l0" + sfx] = _t2m_uniform(g, b, 3 * H)
+        sd["gru.bias_hh_l0" + sfx] = _t2m_uniform(g, b, 3 * H)
+    _t2m_linear(sd, g, "output_net.0.", H, 2 * H)
+    _ln(sd, g, "output_net.1.", H)
+    _t2m_linear(sd, g, "output_net.3.", out, H)
+    sd["hidden"] = g.normal(2, 1, H)
+
+
+def t2m_state_dicts(seed: int = 2468, **dims) -> Dict[str, Dict[str, Tensor]]:
+    """The three evaluator state dicts under finest.tar's keys ``text_encoder``, ``movement_encoder`` and
+    ``motion_encoder`` (mld.py:176-181), shaped by ``T2M_DIMS`` (configs/base.yaml model.t2m_*; dim_pose is
+    NFEATS - 4).  Linear, Conv1d and GRU weights follow torch's default init; the LayerNorm affine is randomised as
+    elsewhere in this module so that parity tests exercise every term."""
+    d = {**T2M_DIMS, **dims}
+    g = _Gen(seed)
+    text: Dict[str, Tensor] = {}
+    _t2m_linear(text, g, "pos_emb.", d["dim_word"], d["dim_pos_ohot"])
+    _t2m_linear(text, g, "input_emb.", d["dim_text_hidden"], d["dim_word"])
+    _t2m_bigru(text, g, d["dim_text_hidden"], d["dim_text_hidden"], d["dim_coemb_hidden"])
+    move: Dict[str, Tensor] = {}
+    _t2m_linear(move, g, "main.0.", d["dim_move_hidden"], d["dim_pose"], 4)
+    _t2m_linear(move, g, "main.3.", d["dim_move_latent"], d["dim_move_hidden"], 4)
+    _t2m_linear(move, g, "out_net.", d["dim_move_latent"], d["dim_move_latent"])
+    motion: Dict[str, Tensor] = {}
+    _t2m_linear(motion, g, "input_emb.", d["dim_motion_hidden"], d["dim_move_latent"])
+    _t2m_bigru(motion, g, d["dim_motion_hidden"], d["dim_motion_hidden"], d["dim_motion_latent"])
+    return {"text_encoder": text, "movement_encoder": move, "motion_encoder": motion}
+
+
+def t2m_text_inputs(B: int, L: int = 22, seed: int = 11, dim_word: int = 300, dim_pos_ohot: int = 15):
+    """GloVe-shaped word vectors ``[B, L, 300]`` (element std ~0.4, as GloVe 300d) and one-hot POS rows
+    ``[B, L, 15]`` (one random category per token, padding tokens included, as the dataset pads with a word)."""
+    g = torch.Generator().manual_seed(seed)
+    word = torch.randn(B, L, dim_word, generator=g) * 0.4
+    cat = torch.randint(0, dim_pos_ohot, (B, L), generator=g)
+    pos = torch.nn.functional.one_hot(cat, dim_pos_ohot).float()
+    return word, pos
+
+
+def t2m_mean_std(nfeats: int = 263, seed: int = 6):
+    """Synthetic evaluator statistics (``mean_eval`` / ``std_eval``, the t2m model's Mean.npy / Std.npy): the
+    dataset statistics of :func:`mean_std` perturbed, so that ``renorm4t2m`` maps zero padding rows to non-zero."""
+    mean, std = mean_std(nfeats)
+    g = torch.Generator().manual_seed(seed)
+    return mean + 0.1 * std * torch.randn(nfeats, generator=g), std * (0.8 + 0.4 * torch.rand(nfeats, generator=g))
+
+
+def t2m_feats(B: int, T: int, lengths: List[int], seed: int = 12, nfeats: int = 263) -> Tensor:
+    """Dataset-normalised motion features ``[B, T, nfeats]``: N(0, 1) rows up to each length, zero padding after
+    (the HumanML3D loader pads normalised motions with zeros)."""
+    g = torch.Generator().manual_seed(seed)
+    x = torch.randn(B, T, nfeats, generator=g)
+    for b, n in enumerate(lengths):
+        x[b, n:] = 0.0
+    return x
+
+
+def renorm4t2m(feats: Tensor, mean: Tensor, std: Tensor, mean_eval: Tensor, std_eval: Tensor) -> Tensor:
+    """HumanML3DDataModule.renorm4t2m (mld/data/HumanML3D.py:54-62)."""
+    feats = feats * std.to(feats) + mean.to(feats)
+    return (feats - mean_eval.to(feats)) / std_eval.to(feats)
