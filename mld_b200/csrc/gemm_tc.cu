@@ -7,11 +7,13 @@
 // [N, K] (PyTorch's [out, in] layout is already the K-major B operand), also split into hi/lo
 // planes.  Three f16 MMAs per K-step reproduce the reference's fp32 GEMM to ~1e-6.
 //
-// CTA = three warpgroups, one CTA per SM, persistent over tiles: warpgroup 0 gives its registers
-// away (setmaxnreg) and its first warp is the TMA producer; warpgroups 1 and 2 each own 64 rows of
-// the tile, issue wgmma.mma_async on operands that stream through a ring of 128B-swizzled
+// k_gemm_tc: CTA = three warpgroups, one CTA per SM, persistent over tiles: warpgroup 0 gives its
+// registers away (setmaxnreg) and its first warp is the TMA producer; warpgroups 1 and 2 each own 64
+// rows of the tile, issue wgmma.mma_async on operands that stream through a ring of 128B-swizzled
 // shared-memory tiles (BK = 64 halves = one swizzle row) and run the epilogue on their accumulator
-// registers while the producer already fills the ring for the next tile.
+// registers while the producer already fills the ring for the next tile.  k_ffn_tc keeps the two
+// consumer warpgroups and drops the producer one (see there): its body needs more than the 168
+// registers per thread a 384-thread CTA allows.
 // Epilogues (a thread holds column pairs of two rows, a row is spread over the 4 lanes of a quad):
 //   fast:      bias + activation -> split16, identity row mapping (the per-layer GEMMs)
 //   generic:   + positional table, row remapping, zeroed padding rows, fp32 output, ragged N
@@ -36,7 +38,8 @@ namespace {
 using namespace tc;
 
 constexpr int BM = 128, BK = 64;
-constexpr int NUM_THREADS = 384;                     // producer warpgroup + two consumer warpgroups
+constexpr int NUM_THREADS = 384;                     // k_gemm_tc: producer warpgroup + two consumer warpgroups
+constexpr int FFN_THREADS = 256;                     // k_ffn_tc: the two consumer warpgroups only
 constexpr int CONSUMER_WARPS = 8;
 constexpr int MAX_N = 1024;
 constexpr int MAX_N_WIDE = 4096;                     // GemmArgs::wide_n
@@ -374,9 +377,13 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
 //   E1(c): acc1 -> *s1 + b1 -> GELU -> split16 A fragments (the accumulator layout of 16 columns IS the
 //          register-operand layout of a 16-deep k-step, so the hidden chunk never touches shared memory)
 //   F2(c): acc2[64 x 256] += H[64 x 64] . W2[:, c*64..]^T                  (A from registers)
-// and finishes with the residual + LayerNorm epilogue on acc2.  The TMA warp streams W1 / W2 through a ring of
-// three 32 KB slots, four per chunk: W1 k-blocks 0-1, W1 k-blocks 2-3, W2 hi plane, W2 lo plane.  F2(c)'s last
-// group stays in flight under F1(c + 1); the other warpgroup's MMAs cover this one's GELU.
+// and finishes with the residual + LayerNorm epilogue on acc2.  W1 / W2 stream through a ring of three 32 KB
+// slots, four per chunk: W1 k-blocks 0-1, W1 k-blocks 2-3, W2 hi plane, W2 lo plane.  F2(c)'s last group stays in
+// flight under F1(c + 1); the other warpgroup's MMAs cover this one's GELU.
+// CTA = the two MMA warpgroups only, 256 threads, one CTA per SM.  ptxas compiles a kernel under 65536 / (threads
+// rounded up to whole warpgroups) registers per thread whatever setmaxnreg does at run time: 168 with a third
+// (producer) warpgroup, which this body (~208) does not fit - it spilled and had its wgmma serialised - and 255
+// without one.  The TMA loads are a handful of instructions, so warp 0 issues them between its own MMAs.
 struct FfnParams {
   int M, m_tiles, n_chunks;
   // Work decomposition (see k_ffn_tc): every CTA runs `full` whole m-tiles; the `left` tiles that do
@@ -399,7 +406,7 @@ struct FfnCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(FFN_THREADS, 1)
 k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
          const __grid_constant__ CUtensorMap tmW1h, const __grid_constant__ CUtensorMap tmW1l,
          const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l, const FfnParams p) {
@@ -409,7 +416,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* ring = smem + Cfg::X_BYTES;
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
-  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per consumer warp)
+  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
   uint64_t* bar_xfull = bar_empty + STAGES;   // x tile landed
   uint64_t* bar_xempty = bar_xfull + 1;       // ... and read by the tile's last F1
 
@@ -434,6 +441,13 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
     return Item{rev(p.full * ncta + t), c0, c1, p.parts == 1 ? 0 : (part == p.parts - 1 ? 2 : 1),
                 p.parts == 1 ? 0 : slot0 + (part == p.parts - 1 ? 0 : part)};
   };
+  // ring positions of this CTA: four per chunk of every item, in item order
+  const int per_tile = 4 * NC;
+  int total = p.full * per_tile;
+  if (nlocal > p.full) {
+    const Item it = item(p.full);
+    total += 4 * (it.c1 - it.c0);
+  }
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
@@ -451,59 +465,69 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   pdl_wait();
   tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
 
-  if (warp < 4) {
-    reg_dec<40>();
-    if (warp != 0) return;
-    // ---------------------------------------------------------------- TMA producer
-    int rc = 0;                                    // ring position
-    auto slot_wait = [&]() { mbar_wait(smem_u32(&bar_empty[rc % STAGES]), (((uint32_t)(rc / STAGES)) & 1u) ^ 1u); };
-    for (int j = 0; j < nlocal; ++j) {
-      const Item it = item(j);
-      const int m0 = it.mt * BM;
-      mbar_wait(smem_u32(bar_xempty), ((uint32_t)j & 1u) ^ 1u);
-      if (elect_one()) {
-        const uint32_t full = smem_u32(bar_xfull);
-        mbar_expect_tx(full, Cfg::X_BYTES);
-        for (int kb = 0; kb < 4; ++kb) {
-          tma_load_2d(smem_u32(smem + kb * 16384), &tmXh, full, kb * BK, m0);
-          tma_load_2d(smem_u32(smem + 65536 + kb * 16384), &tmXl, full, kb * BK, m0);
+  // ---------------------------------------------------------------- TMA issue (warp 0, one elected lane)
+  // Ring position q holds, for chunk c of its item: q % 4 = 0 / 1: W1 rows [c*64, +64), k-blocks 0-1 / 2-3, hi
+  // then lo; 2 / 3: the hi / lo plane of W2[:, c*64 .. +64).  It is loaded once position q - 3 (same slot) has
+  // been freed by all eight warps.
+  int q_next = 0, x_next = 0;                      // next ring position / next item whose x tile is to be loaded
+  auto load_slot = [&](int q) {
+    const int j = min(q / per_tile, p.full);
+    const Item it = item(j);
+    const int r = q - j * per_tile, c = it.c0 + (r >> 2), k = r & 3;
+    if (elect_one()) {
+      const uint32_t full = smem_u32(&bar_full[q % STAGES]);
+      const uint32_t dst = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES);
+      mbar_expect_tx(full, Cfg::STAGE_BYTES);
+      if (k < 2) {
+        for (int kk = 0; kk < 2; ++kk) {
+          tma_load_2d(dst + kk * 8192, &tmW1h, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
+          tma_load_2d(dst + 16384 + kk * 8192, &tmW1l, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
         }
-        if (j + 1 < nlocal) {                      // next tile's x rows -> L2, a whole tile ahead
-          const int m1 = item(j + 1).mt * BM;
-          for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1); }
-        }
-      }
-      __syncwarp();
-      for (int c = it.c0; c < it.c1; ++c) {
-        for (int half = 0; half < 2; ++half, ++rc) {           // W1 rows [c*64, +64): k-blocks 2*half, 2*half + 1, hi then lo
-          slot_wait();
-          if (elect_one()) {
-            const uint32_t full = smem_u32(&bar_full[rc % STAGES]);
-            const uint32_t dst = smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES);
-            mbar_expect_tx(full, Cfg::STAGE_BYTES);
-            for (int k = 0; k < 2; ++k) {
-              tma_load_2d(dst + k * 8192, &tmW1h, full, (2 * half + k) * BK, c * Cfg::CHUNK);
-              tma_load_2d(dst + 16384 + k * 8192, &tmW1l, full, (2 * half + k) * BK, c * Cfg::CHUNK);
-            }
-          }
-          __syncwarp();
-        }
-        for (int pl = 0; pl < 2; ++pl, ++rc) {                 // W2[:, c*64 .. +64): hi plane, then lo plane
-          slot_wait();
-          if (elect_one()) {
-            const uint32_t full = smem_u32(&bar_full[rc % STAGES]);
-            mbar_expect_tx(full, Cfg::STAGE_BYTES);
-            tma_load_2d(smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES), pl ? &tmW2l : &tmW2h, full, c * Cfg::CHUNK, 0);
-          }
-          __syncwarp();
-        }
+      } else {
+        tma_load_2d(dst, k == 3 ? &tmW2l : &tmW2h, full, c * Cfg::CHUNK, 0);
       }
     }
-    return;
-  }
-  // ------------------------------------------------------------------ consumer warpgroups
-  reg_inc<232>();
-  const int cw = (warp >> 2) - 1;
+    __syncwarp();
+  };
+  auto load_x = [&](int j) {
+    if (elect_one()) {
+      const int m0 = item(j).mt * BM;
+      const uint32_t full = smem_u32(bar_xfull);
+      mbar_expect_tx(full, Cfg::X_BYTES);
+      for (int kb = 0; kb < 4; ++kb) {
+        tma_load_2d(smem_u32(smem + kb * 16384), &tmXh, full, kb * BK, m0);
+        tma_load_2d(smem_u32(smem + 65536 + kb * 16384), &tmXl, full, kb * BK, m0);
+      }
+      if (j + 1 < nlocal) {                        // next tile's x rows -> L2, a whole tile ahead
+        const int m1 = item(j + 1).mt * BM;
+        for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1); }
+      }
+    }
+    __syncwarp();
+  };
+  // Load every ring position up to `need` (waiting for its slot: warp 0 reads that position next), then those
+  // whose slot is already free, and the next x tile once the current one has been read.  Freeing position q
+  // never needs a load past q + 2, and the x tile of item j is loaded before any position of item j is waited
+  // for, so the other warpgroup can always free what warp 0 waits on.  Called by warp 0 only, warp-uniformly.
+  auto produce = [&](int need) {
+    while (q_next < total) {
+      const uint32_t bar = smem_u32(&bar_empty[q_next % STAGES]), par = (((uint32_t)(q_next / STAGES)) & 1u) ^ 1u;
+      if (q_next <= need) mbar_wait(bar, par);
+      else if (!__shfl_sync(0xffffffffu, (int)mbar_test(bar, par), 0)) break;
+      load_slot(q_next++);
+    }
+    if (x_next < nlocal && __shfl_sync(0xffffffffu, (int)mbar_test(smem_u32(bar_xempty), ((uint32_t)x_next & 1u) ^ 1u), 0))
+      load_x(x_next++);
+  };
+  auto produce_x = [&](int j) {                    // the x tile of item j, waiting for the previous one to be read
+    while (x_next <= j) {
+      mbar_wait(smem_u32(bar_xempty), ((uint32_t)x_next & 1u) ^ 1u);
+      load_x(x_next++);
+    }
+  };
+
+  // ------------------------------------------------------------------ both warpgroups: MMA + epilogue
+  const int cw = warp >> 2;                        // which 64 rows of the tile
   const int cp = 2 * (lane & 3);
   const uint32_t sX = smem_u32(smem) + cw * (64 * 128);
   float acc2[128];
@@ -515,6 +539,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   for (int j = 0; j < nlocal; ++j) {
     const Item it = item(j);
     const int m0 = it.mt * BM;
+    if (warp == 0) produce_x(j);
     mbar_wait(smem_u32(bar_xfull), (uint32_t)j & 1u);
     tl_event(p.tl, tl_n, 2, j);                                      // x tile landed
     int pend = -1;                                   // ring position of the F2 group still in flight
@@ -522,7 +547,9 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       // ---- F1(c)
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
+        if (warp == 0) produce(rc + half);
         slot_full(rc + half);
+        tl_event(p.tl, tl_n, 10 + half, c);                          // W1 k-blocks 2 * half, +1 landed
         const uint32_t w = smem_u32(ring + ((rc + half) % STAGES) * Cfg::STAGE_BYTES);
         wg_fence();
 #pragma unroll
@@ -534,10 +561,12 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       }
       wg_wait<0>();
       acc_fence(acc1);
+      tl_event(p.tl, tl_n, 13, c);                                   // F1(c) retired
       if (pend >= 0) slot_free(pend);
       slot_free(rc); slot_free(rc + 1);
       rc += 2;
       if (c == it.c1 - 1 && lane == 0) mbar_arrive(smem_u32(bar_xempty));     // the x tile may be overwritten
+      if (warp == 0) produce(-1);
       // ---- E1(c): bias + GELU -> split16 A fragments
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
@@ -551,8 +580,11 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
                  hh[ks][2 * g + 1], hl[ks][2 * g + 1]);
         }
       }
+      tl_event(p.tl, tl_n, 14, c);                                   // GELU done
       // ---- F2(c): H_lo.W2_hi + H_hi.W2_hi on the hi slot, H_hi.W2_lo on the lo slot
+      if (warp == 0) produce(rc);
       slot_full(rc);
+      tl_event(p.tl, tl_n, 12, c);                                   // W2 hi plane landed
       wg_fence();
       {
         const uint64_t wd = make_desc(smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES));
@@ -563,6 +595,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
         }
       }
       wg_commit();
+      if (warp == 0) produce(rc + 1);
       slot_full(rc + 1);
       {
         const uint64_t wd = make_desc(smem_u32(ring + ((rc + 1) % STAGES) * Cfg::STAGE_BYTES));
@@ -574,10 +607,12 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       slot_free(rc);
       pend = rc + 1;
       rc += 2;
+      if (warp == 0) produce(-1);
     }
     wg_wait<0>();
     acc_fence(acc2);
     if (pend >= 0) slot_free(pend);
+    if (warp == 0) produce(-1);
     tl_event(p.tl, tl_n, 4, j);                                      // acc2 complete
     const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first row inside the tile
     if (it.mode == 1) {
@@ -589,8 +624,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
         *reinterpret_cast<float2*>(dst + (rl + 8) * 256 + 8 * jj + cp) = make_float2(acc2[4 * jj + 2], acc2[4 * jj + 3]);
       }
       __threadfence();
-      named_bar_sync(1, CONSUMER_WARPS * 32);
-      if (threadIdx.x == 128) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.flags + it.piece0), "r"(1) : "memory");
+      named_bar_sync(1, FFN_THREADS);
+      if (threadIdx.x == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.flags + it.piece0), "r"(1) : "memory");
       continue;
     }
     const int nparts = it.mode == 2 ? p.parts - 1 : 0;
@@ -617,8 +652,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
           acc2[4 * jj] += a.x; acc2[4 * jj + 1] += a.y; acc2[4 * jj + 2] += b.x; acc2[4 * jj + 3] += b.y;
         }
       }
-      named_bar_sync(1, CONSUMER_WARPS * 32);                // everyone is past its partial loads: re-arm the flags
-      if (threadIdx.x == 128)
+      named_bar_sync(1, FFN_THREADS);                        // everyone is past its partial loads: re-arm the flags
+      if (threadIdx.x == 0)
         for (int pp = 0; pp < nparts; ++pp) p.flags[it.piece0 + pp] = 0;
     }
     ln_epilogue(acc2, p.inv_s2, p.b2, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
@@ -834,6 +869,6 @@ bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, 
   const int ncta = p.full > 0 ? ncta_max : p.left * p.parts;
   static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
   p.reverse = snake;
-  launch_pdl(k_ffn_tc, dim3(ncta), dim3(NUM_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
+  launch_pdl(k_ffn_tc, dim3(ncta), dim3(FFN_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
   return true;
 }
