@@ -365,7 +365,7 @@ int64_t mldb_launch_count(const mldb_handle* h);
 /* Which kernel every operator of the path was ENQUEUED on since the last reset (recorded launches: a CUDA
  * graph counts once, at capture).  out: HOST int64[MLDB_KSTAT_COUNT], index = MLDB_KSTAT_*.  Lets a caller
  * (and the tests) assert that nothing fell back from the wgmma kernels to the CUDA-core kernels. */
-#define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue */
+#define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue; k_proj_tc (its K = 256 split16 projections) */
 #define MLDB_KSTAT_GEMM_LN_TC 1   /* k_gemm_tc, fused residual + LayerNorm epilogue */
 #define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block) */
 #define MLDB_KSTAT_ATTN_TC 3      /* k_attn_tc (wgmma attention) */

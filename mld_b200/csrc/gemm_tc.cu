@@ -1,5 +1,5 @@
 // Warpgroup-MMA (wgmma) split-fp16 kernels for sm_90a: the persistent GEMM with fused epilogues
-// (k_gemm_tc) and the fused FFN block (k_ffn_tc).
+// (k_gemm_tc), the fused FFN block (k_ffn_tc) and the K = 256 projection (k_proj_tc).
 //
 //   D[128 x BN] (fp32, registers) = A_hi W_hi^T + A_lo W_hi^T + A_hi W_lo^T        per 128-row tile
 //
@@ -39,7 +39,7 @@ using namespace tc;
 
 constexpr int BM = 128, BK = 64;
 constexpr int NUM_THREADS = 384;                     // k_gemm_tc: producer warpgroup + two consumer warpgroups
-constexpr int FFN_THREADS = 256;                     // k_ffn_tc: the two consumer warpgroups only
+constexpr int MMA_THREADS = 256;                     // k_ffn_tc, k_proj_tc: the two MMA warpgroups only
 constexpr int CONSUMER_WARPS = 8;
 constexpr int MAX_N = 1024;
 constexpr int MAX_N_WIDE = 4096;                     // GemmArgs::wide_n
@@ -103,6 +103,45 @@ __device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, 
   split2(x0, x1, h, l);
   *reinterpret_cast<uint32_t*>(hi + o) = h;
   *reinterpret_cast<uint32_t*>(lo + o) = l;
+}
+
+// The fast epilogue's math on 8-column group j of an accumulator fragment: x[0..1] = act(d * sc + b) of this
+// thread's first row, x[2..3] of its second.  b: the bias of the thread's column pair in group j.
+template <int ACT, int N>
+__device__ __forceinline__ void fast_group(const float (&d)[N], int j, float sc, float2 b, float (&x)[4]) {
+  x[0] = fmaf(d[4 * j], sc, b.x); x[1] = fmaf(d[4 * j + 1], sc, b.y);
+  x[2] = fmaf(d[4 * j + 2], sc, b.x); x[3] = fmaf(d[4 * j + 3], sc, b.y);
+#pragma unroll
+  for (int e = 0; e < 4; ++e) {
+    if (ACT == ACT_GELU) x[e] = gelu_fast(x[e]);
+    if (ACT == ACT_QUICKGELU) x[e] = quick_gelu_f(x[e]);
+    if (ACT == ACT_LEAKY) x[e] = apply_act(x[e], ACT_LEAKY);
+  }
+}
+
+// 4 x 4 transpose across the lanes of a quad: lane l holds v[g] = word l of group g and gets word g of group l.
+// Two shuffle rounds of two words each.
+__device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int l) {
+  const bool b2 = l & 2, b1 = l & 1;
+  uint32_t r0 = __shfl_xor_sync(0xffffffffu, b2 ? v[0] : v[2], 2), r1 = __shfl_xor_sync(0xffffffffu, b2 ? v[1] : v[3], 2);
+  if (b2) { v[0] = r0; v[1] = r1; } else { v[2] = r0; v[3] = r1; }
+  r0 = __shfl_xor_sync(0xffffffffu, b1 ? v[0] : v[1], 1); r1 = __shfl_xor_sync(0xffffffffu, b1 ? v[2] : v[3], 1);
+  if (b1) { v[0] = r0; v[2] = r1; } else { v[1] = r0; v[3] = r1; }
+}
+
+// Ring producer of the two-warpgroup kernels (k_ffn_tc, k_proj_tc), run by warp 0 between its own MMAs: load every
+// position up to `need` (blocking on its slot: warp 0 reads that position next), then those whose slot is already
+// free.  Position q goes to slot q % stages once position q - stages has been freed (bar_empty, one arrival per
+// warp).  Warp-uniform.
+template <class Load>
+__device__ __forceinline__ void ring_produce(int& q_next, int total, int need, const uint64_t* bar_empty, int stages,
+                                             Load&& load) {
+  while (q_next < total) {
+    const uint32_t bar = smem_u32(&bar_empty[q_next % stages]), par = (((uint32_t)(q_next / stages)) & 1u) ^ 1u;
+    if (q_next <= need) mbar_wait(bar, par);
+    else if (!__shfl_sync(0xffffffffu, (int)mbar_test(bar, par), 0)) break;
+    load(q_next++);
+  }
 }
 
 // y = LayerNorm(acc * sc + bias + residual) * gamma + beta over the 256-wide rows of a [64 x 256] accumulator
@@ -283,23 +322,14 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
       ln_epilogue(d, p.inv_scale, p.bias, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
                   r_lo, p.M, cp);
     } else if constexpr (EPI == EPI_FAST) {
-      const float sc = p.inv_scale;
       const bool ok0 = r_lo < p.M, ok1 = r_lo + 8 < p.M;
       const int64_t o0 = (int64_t)r_lo * p.ld_out + p.out_col0 + n0 + cp, o1 = o0 + (int64_t)8 * p.ld_out;
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp));
-        float x0 = fmaf(d[4 * j], sc, b.x), x1 = fmaf(d[4 * j + 1], sc, b.y);
-        float x2 = fmaf(d[4 * j + 2], sc, b.x), x3 = fmaf(d[4 * j + 3], sc, b.y);
-        if (ACT == ACT_GELU) { x0 = gelu_fast(x0); x1 = gelu_fast(x1); x2 = gelu_fast(x2); x3 = gelu_fast(x3); }
-        if (ACT == ACT_QUICKGELU) {
-          x0 = quick_gelu_f(x0); x1 = quick_gelu_f(x1); x2 = quick_gelu_f(x2); x3 = quick_gelu_f(x3);
-        }
-        if (ACT == ACT_LEAKY) {
-          x0 = apply_act(x0, ACT_LEAKY); x1 = apply_act(x1, ACT_LEAKY); x2 = apply_act(x2, ACT_LEAKY); x3 = apply_act(x3, ACT_LEAKY);
-        }
-        if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x0, x1);
-        if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x2, x3);
+        float x[4];
+        fast_group<ACT>(d, j, p.inv_scale, __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp)), x);
+        if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x[0], x[1]);
+        if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x[2], x[3]);
       }
     } else if constexpr (EPI == EPI_RES) {
       // each element of R is read and then overwritten by the same thread: in place is safe (plain loads, no __ldg)
@@ -406,7 +436,7 @@ struct FfnCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-__global__ void __launch_bounds__(FFN_THREADS, 1)
+__global__ void __launch_bounds__(MMA_THREADS, 1)
 k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
          const __grid_constant__ CUtensorMap tmW1h, const __grid_constant__ CUtensorMap tmW1l,
          const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l, const FfnParams p) {
@@ -510,12 +540,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   // never needs a load past q + 2, and the x tile of item j is loaded before any position of item j is waited
   // for, so the other warpgroup can always free what warp 0 waits on.  Called by warp 0 only, warp-uniformly.
   auto produce = [&](int need) {
-    while (q_next < total) {
-      const uint32_t bar = smem_u32(&bar_empty[q_next % STAGES]), par = (((uint32_t)(q_next / STAGES)) & 1u) ^ 1u;
-      if (q_next <= need) mbar_wait(bar, par);
-      else if (!__shfl_sync(0xffffffffu, (int)mbar_test(bar, par), 0)) break;
-      load_slot(q_next++);
-    }
+    ring_produce(q_next, total, need, bar_empty, STAGES, load_slot);
     if (x_next < nlocal && __shfl_sync(0xffffffffu, (int)mbar_test(smem_u32(bar_xempty), ((uint32_t)x_next & 1u) ^ 1u), 0))
       load_x(x_next++);
   };
@@ -624,7 +649,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
         *reinterpret_cast<float2*>(dst + (rl + 8) * 256 + 8 * jj + cp) = make_float2(acc2[4 * jj + 2], acc2[4 * jj + 3]);
       }
       __threadfence();
-      named_bar_sync(1, FFN_THREADS);
+      named_bar_sync(1, MMA_THREADS);
       if (threadIdx.x == 0) asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p.flags + it.piece0), "r"(1) : "memory");
       continue;
     }
@@ -652,13 +677,207 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
           acc2[4 * jj] += a.x; acc2[4 * jj + 1] += a.y; acc2[4 * jj + 2] += b.x; acc2[4 * jj + 3] += b.y;
         }
       }
-      named_bar_sync(1, FFN_THREADS);                        // everyone is past its partial loads: re-arm the flags
+      named_bar_sync(1, MMA_THREADS);                        // everyone is past its partial loads: re-arm the flags
       if (threadIdx.x == 0)
         for (int pp = 0; pp < nparts; ++pp) p.flags[it.piece0 + pp] = 0;
     }
     ln_epilogue(acc2, p.inv_s2, p.b2, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
                 m0 + rl, p.M, cp);
     tl_event(p.tl, tl_n, 5, j);                                      // LN tail done
+  }
+  tl_event(p.tl, tl_n, 42);                       // kernel exit
+}
+
+// ------------------------------------------------------------------------------ K = 256 projection
+// out = act(A W^T * s + b) -> split16 for K = 256 with one A source and N a multiple of 128 (the fast epilogue's
+// shapes): the QKV / kv / q projections of the encoder layers and the VAE's d = 256 projections.  With only four
+// k-blocks, k_gemm_tc spends about as long in its epilogue as in its MMAs, and both warpgroups reach the epilogue
+// together, so nothing overlaps it.  Here the CTA is k_ffn_tc's F1 with a store epilogue:
+//   - the two MMA warpgroups only (256 threads, 255 registers), warp 0 issues the TMA loads between its MMAs;
+//   - the 128 x 256 A tile (both planes, 128 KB, one barrier pair per k-block) stays in shared memory while W
+//     streams through three 32 KB ring slots, one k-block of a 128-column chunk per slot;
+//   - each warpgroup keeps two 64 x 128 accumulators: the epilogue of chunk i - 1 runs while chunk i's k-blocks 1
+//     and 2 are on the tensor cores.
+// Work items are (m-tile, chunk) pairs in m-major order; each CTA takes one contiguous range of near-equal
+// length and walks it upwards (the GEMMs' direction in the snake order), loading each A tile it touches once.
+// The per-element accumulation order is kblock_ss's over k-blocks 0..3, as in k_gemm_tc, so the outputs are
+// identical to k_gemm_tc's.
+struct ProjParams {
+  int M, n_chunks, items;                        // items = m-tiles x n_chunks
+  float inv_scale;
+  const float* bias;
+  __half* out_hi; __half* out_lo; int ld_out, out_col0;
+  long long* tl;
+};
+struct ProjCfg {
+  static constexpr int CHUNK = 128;                      // output columns per chunk
+  static constexpr int A_BYTES = 2 * 4 * BM * 128;       // [plane][k-block][128 rows x 128 B], as k_ffn_tc's x tile
+  static constexpr int STAGE_BYTES = 2 * CHUNK * 128, STAGES = 3;   // one k-block of a chunk, both planes
+  static constexpr int SMEM_BYTES = A_BYTES + STAGES * STAGE_BYTES + 256 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+};
+
+template <int ACT>                                     // the fast epilogue's activation (NONE | GELU | QUICKGELU | LEAKY)
+__global__ void __launch_bounds__(MMA_THREADS, 1)
+k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+          const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const ProjParams p) {
+  using Cfg = ProjCfg;
+  constexpr int STAGES = Cfg::STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* ring = smem + Cfg::A_BYTES;
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
+  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
+  uint64_t* bar_afull = bar_empty + STAGES;   // [4] k-block k of the A tile landed
+  uint64_t* bar_aempty = bar_afull + 4;       // [4] ... and read by the last chunk of its tile (one arrival per warp)
+
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
+  int tl_n = 0;
+  tl_event(p.tl, tl_n, 40);                       // kernel entry
+  const int NC = p.n_chunks;
+  // this CTA's items [t0, t0 + n), n >= 1 (the grid is at most the item count); local item i, local A tile j
+  const int t0 = (int)((long long)blockIdx.x * p.items / gridDim.x);
+  const int n = (int)((long long)(blockIdx.x + 1) * p.items / gridDim.x) - t0;
+  const int mt0 = t0 / NC, ntiles = (t0 + n - 1) / NC - mt0 + 1;
+  auto tile_of = [&](int i) { return (t0 + i) / NC - mt0; };
+  auto first_of_tile = [&](int i) { return i == 0 || (t0 + i) % NC == 0; };
+  auto last_of_tile = [&](int i) { return i == n - 1 || (t0 + i + 1) % NC == 0; };
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(smem_u32(&bar_full[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
+    }
+    for (int k = 0; k < 4; ++k) {
+      mbar_init(smem_u32(&bar_afull[k]), 1);
+      mbar_init(smem_u32(&bar_aempty[k]), CONSUMER_WARPS);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
+  }
+  pdl_trigger();
+  __syncthreads();
+  pdl_wait();
+  tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
+
+  // ---------------------------------------------------------------- TMA issue (warp 0, one elected lane)
+  // Two rings, both filled by ring_produce: W position q = 4 i + k (k-block k of item i's chunk) in slot q % 3, and
+  // A position a = 4 j + k (k-block k of local tile j) in k-block slot k.  Freeing W position q never needs a load
+  // past q + 2, and A k-block k of tile j is freed by MMAs that only need W positions and A tiles up to tile j, so
+  // the other warpgroup can always free what warp 0 waits on.
+  int q_next = 0, a_next = 0;
+  auto load_w = [&](int q) {
+    if (elect_one()) {
+      const int c = (t0 + (q >> 2)) % NC, k = q & 3;
+      const uint32_t full = smem_u32(&bar_full[q % STAGES]);
+      const uint32_t dst = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES);
+      mbar_expect_tx(full, Cfg::STAGE_BYTES);
+      tma_load_2d(dst, &tmWh, full, k * BK, c * Cfg::CHUNK);         // rows >= N are zero-filled (and counted)
+      tma_load_2d(dst + Cfg::STAGE_BYTES / 2, &tmWl, full, k * BK, c * Cfg::CHUNK);
+    }
+    __syncwarp();
+  };
+  auto load_a = [&](int a) {
+    if (elect_one()) {
+      const int j = a >> 2, k = a & 3, m0 = (mt0 + j) * BM;
+      const uint32_t full = smem_u32(&bar_afull[k]);
+      mbar_expect_tx(full, 2 * BM * 128);
+      tma_load_2d(smem_u32(smem + k * 16384), &tmAh, full, k * BK, m0);
+      tma_load_2d(smem_u32(smem + 65536 + k * 16384), &tmAl, full, k * BK, m0);
+      if (k == 0 && j + 1 < ntiles)                // the next tile's rows -> L2, a whole tile ahead
+        for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmAh, k2 * BK, m0 + BM); tma_prefetch_2d(&tmAl, k2 * BK, m0 + BM); }
+    }
+    __syncwarp();
+  };
+  auto produce = [&](int need_w, int need_a) {     // warp 0 only, warp-uniformly
+    ring_produce(a_next, 4 * ntiles, need_a, bar_aempty, 4, load_a);
+    ring_produce(q_next, 4 * n, need_w, bar_empty, STAGES, load_w);
+  };
+
+  // ------------------------------------------------------------------ both warpgroups: MMA + epilogue
+  const int cw = warp >> 2;                        // which 64 rows of the tile
+  const int cp = 2 * (lane & 3);
+  const uint32_t sA = smem_u32(smem) + cw * (64 * 128);
+  float acc0[64], acc1[64];
+  auto retire = [&](int q) {                       // this warp's MMAs of W position q have retired
+    if (lane == 0) {
+      mbar_arrive(smem_u32(&bar_empty[q % STAGES]));
+      if (last_of_tile(q >> 2)) mbar_arrive(smem_u32(&bar_aempty[q & 3]));
+    }
+  };
+  // The fast epilogue's math, then a quad transpose per four 8-column groups, so that each lane stores one group
+  // of a row as 16 B per plane: a warp store writes 64 B row pieces instead of k_gemm_tc's 16 B ones.
+  auto epilogue = [&](const float (&d)[64], int i) {
+    const int t = t0 + i, r_lo = (t / NC) * BM + cw * 64 + (warp & 3) * 16 + (lane >> 2), n0 = (t % NC) * Cfg::CHUNK;
+    const int l = lane & 3;
+    const bool ok0 = r_lo < p.M, ok1 = r_lo + 8 < p.M;
+    const int64_t o0 = (int64_t)r_lo * p.ld_out + p.out_col0 + n0 + 8 * l, o1 = o0 + (int64_t)8 * p.ld_out;
+    tl_event(p.tl, tl_n, 52, i);                                     // epilogue of item i begins
+#pragma unroll
+    for (int jb = 0; jb < Cfg::CHUNK / 32; ++jb) {
+      uint32_t h0[4], l0[4], h1[4], l1[4];        // [group jb * 4 + g]: hi / lo words of the first / second row
+#pragma unroll
+      for (int g = 0; g < 4; ++g) {
+        const int j = 4 * jb + g;
+        float x[4];
+        fast_group<ACT>(d, j, p.inv_scale, __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp)), x);
+        split2(x[0], x[1], h0[g], l0[g]);
+        split2(x[2], x[3], h1[g], l1[g]);
+      }
+      quad_transpose(h0, l); quad_transpose(l0, l); quad_transpose(h1, l); quad_transpose(l1, l);
+      if (ok0) {
+        *reinterpret_cast<uint4*>(p.out_hi + o0 + 32 * jb) = make_uint4(h0[0], h0[1], h0[2], h0[3]);
+        *reinterpret_cast<uint4*>(p.out_lo + o0 + 32 * jb) = make_uint4(l0[0], l0[1], l0[2], l0[3]);
+      }
+      if (ok1) {
+        *reinterpret_cast<uint4*>(p.out_hi + o1 + 32 * jb) = make_uint4(h1[0], h1[1], h1[2], h1[3]);
+        *reinterpret_cast<uint4*>(p.out_lo + o1 + 32 * jb) = make_uint4(l1[0], l1[1], l1[2], l1[3]);
+      }
+    }
+    tl_event(p.tl, tl_n, 53, i);                                     // ... stores issued
+  };
+  // Item i into `cur`.  After issuing each k-block, wait for the one before it and free its W slot (and A k-block);
+  // item i - 1 is complete once k-block 0 has been issued, and its epilogue runs behind k-blocks 1 and 2.
+  auto step = [&](int i, float (&cur)[64], float (&prev)[64]) {
+    const bool fresh = first_of_tile(i);
+    const int j = tile_of(i);
+    tl_event(p.tl, tl_n, 50, i);                                     // item i begins
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int q = 4 * i + k;
+      if (warp == 0) produce(q, fresh ? 4 * j + k : -1);
+      if (fresh) {
+        mbar_wait(smem_u32(&bar_afull[k]), (uint32_t)j & 1u);
+        if (k == 0) tl_event(p.tl, tl_n, 51, j);                    // A k-block 0 of tile j landed
+      }
+      mbar_wait(smem_u32(&bar_full[q % STAGES]), ((uint32_t)(q / STAGES)) & 1u);
+      const uint32_t w = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES), a = sA + k * 16384;
+      wg_fence();
+      kblock_ss<128>(cur, a, a + 65536, w, w + Cfg::STAGE_BYTES / 2, k == 0);
+      wg_commit();
+      if (k == 2) {
+        if (warp == 0) produce(q + 1, -1);         // k-block 3's load must not wait behind the epilogue
+        if (i > 0) epilogue(prev, i - 1);
+      }
+      if (q > 0) {
+        wg_wait<1>();
+        retire(q - 1);
+      }
+      if (k == 0 && i > 0) acc_fence(prev);
+    }
+  };
+  for (int i = 0; i < n; i += 2) {
+    step(i, acc0, acc1);
+    if (i + 1 < n) step(i + 1, acc1, acc0);
+  }
+  wg_wait<0>();
+  retire(4 * n - 1);
+  if ((n - 1) & 1) {
+    acc_fence(acc1);
+    epilogue(acc1, n - 1);
+  } else {
+    acc_fence(acc0);
+    epilogue(acc0, n - 1);
   }
   tl_event(p.tl, tl_n, 42);                       // kernel exit
 }
@@ -702,6 +921,8 @@ TcCtx* tc_create(int device) {
   opt_in(k_gemm_tc<256, EPI_F32>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_F32>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_F32, ACT_LEAKY>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_F32, ACT_LEAKY>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_ffn_tc, FfnCfg::SMEM_BYTES);
+  opt_in(k_proj_tc<ACT_NONE>, ProjCfg::SMEM_BYTES); opt_in(k_proj_tc<ACT_GELU>, ProjCfg::SMEM_BYTES);
+  opt_in(k_proj_tc<ACT_QUICKGELU>, ProjCfg::SMEM_BYTES); opt_in(k_proj_tc<ACT_LEAKY>, ProjCfg::SMEM_BYTES);
   if (e != cudaSuccess) {
     mldb_set_err(std::string("cudaFuncSetAttribute(k_gemm_tc): ") + cudaGetErrorString(e));
     delete c;
@@ -777,9 +998,39 @@ static bool map_fail(const char* what, int M, int N, int K) {
   return false;
 }
 
+// k_proj_tc: the fast epilogue with K = 256 from one A source (every N here is a multiple of 128)
+static bool tc_proj(TcCtx* c, const GemmArgs& g, cudaStream_t st) {
+  CUtensorMap mAh, mAl, mWh, mWl;
+  const bool ok = make_map(c, &mAh, g.a1.hi, g.M, g.K1, BM) && make_map(c, &mAl, g.a1.lo(), g.M, g.K1, BM) &&
+                  make_map(c, &mWh, g.w.w, g.w.N, g.w.K, ProjCfg::CHUNK) &&
+                  make_map(c, &mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, ProjCfg::CHUNK);
+  if (!ok) return map_fail("proj", g.M, g.w.N, g.w.K);
+  ProjParams p{};
+  p.M = g.M; p.n_chunks = g.w.N / ProjCfg::CHUNK; p.items = (g.M + BM - 1) / BM * p.n_chunks;
+  p.inv_scale = g.w.inv_scale; p.bias = g.w.bias;
+  p.out_hi = g.out.hi; p.out_lo = g.out.lo(); p.ld_out = g.out.cols; p.out_col0 = g.out_col0;
+  p.tl = tc::mldb_timeline_buffer();
+  const dim3 grid(p.items < c->sm_count ? p.items : c->sm_count);
+  switch (g.act) {
+    case ACT_GELU: launch_pdl(k_proj_tc<ACT_GELU>, grid, dim3(MMA_THREADS), ProjCfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, p); break;
+    case ACT_QUICKGELU: launch_pdl(k_proj_tc<ACT_QUICKGELU>, grid, dim3(MMA_THREADS), ProjCfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, p); break;
+    case ACT_LEAKY: launch_pdl(k_proj_tc<ACT_LEAKY>, grid, dim3(MMA_THREADS), ProjCfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, p); break;
+    default: launch_pdl(k_proj_tc<ACT_NONE>, grid, dim3(MMA_THREADS), ProjCfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, p); break;
+  }
+  return true;
+}
+
 bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
-  CUtensorMap mA1h, mA1l, mA2h, mA2l, mWh, mWl;
   const int bn = ln ? 256 : pick_bn(g);
+  // the fast plain epilogue: split16 output, identity row mapping, N a whole number of tiles
+  const bool fast = !ln && g.out.hi && !g.out_f32 && !g.addtab && !g.zero_lengths && g.in_group >= g.M &&
+                    g.out_group == 0 && g.out_off == 0 && g.w.N % bn == 0 && g.w.bias != nullptr &&
+                    (g.act == ACT_NONE || g.act == ACT_GELU || g.act == ACT_QUICKGELU || g.act == ACT_LEAKY);
+  // K = 256 from one source: keep the A tile on the SM and overlap each chunk's epilogue with the next chunk's MMAs
+  // (16-byte stores: both output planes 16-byte aligned)
+  if (fast && g.K1 == 256 && g.K2 == 0 && ((uintptr_t)g.out.hi & 15) == 0 && ((uintptr_t)g.out.lo() & 15) == 0)
+    return tc_proj(c, g, st);
+  CUtensorMap mA1h, mA1l, mA2h, mA2l, mWh, mWl;
   bool ok = make_map(c, &mA1h, g.a1.hi, g.M, g.K1, BM) && make_map(c, &mA1l, g.a1.lo(), g.M, g.K1, BM);
   if (g.K2 > 0) ok = ok && make_map(c, &mA2h, g.a2.hi, g.M, g.K2, BM) && make_map(c, &mA2l, g.a2.lo(), g.M, g.K2, BM);
   else { mA2h = mA1h; mA2l = mA1l; }
@@ -787,10 +1038,6 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   if (!ok) return map_fail("gemm", g.M, g.w.N, g.w.K);
   TcParams p;
   fill_params(g, ln, bn, &p);
-  // the fast plain epilogue: split16 output, identity row mapping, N a whole number of tiles
-  const bool fast = !ln && g.out.hi && !g.out_f32 && !g.addtab && !g.zero_lengths && g.in_group >= g.M &&
-                    g.out_group == 0 && g.out_off == 0 && g.w.N % bn == 0 && g.w.bias != nullptr &&
-                    (g.act == ACT_NONE || g.act == ACT_GELU || g.act == ACT_QUICKGELU || g.act == ACT_LEAKY);
   // the vectorised fp32 epilogue, for callers that ask for it (vec_f32)
   const bool f32 = !ln && g.vec_f32 && !g.out.hi && g.out_f32 && !g.res_f32 && !g.addtab && !g.zero_lengths &&
                    g.in_group >= g.M && g.out_group == 0 && g.out_off == 0 && g.w.N % 2 == 0 && g.ldc % 2 == 0 &&
@@ -869,6 +1116,6 @@ bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, 
   const int ncta = p.full > 0 ? ncta_max : p.left * p.parts;
   static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
   p.reverse = snake;
-  launch_pdl(k_ffn_tc, dim3(ncta), dim3(FFN_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
+  launch_pdl(k_ffn_tc, dim3(ncta), dim3(MMA_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
   return true;
 }

@@ -10,6 +10,7 @@ TAGS = {1: "prod:tile", 2: "mma:tile_begin", 3: "mma:tile_issued", 4: "epi:acc_r
         10: "mma:F1_start", 11: "mma:F1_issued", 12: "mma:F2_start", 13: "e1:acc1_ready", 14: "e1:hs_written", 15: "ln:acc2_ready", 16: "ln:done",
         20: "prod:Q", 21: "prod:Vslot", 22: "mma:S_go", 23: "mma:K_landed", 24: "mma:S_issued", 25: "mma:P_written", 26: "mma:V_landed",
         40: "entry", 41: "pdl_waited", 42: "exit",
+        50: "proj:item", 51: "proj:A_landed", 52: "proj:epi_begin", 53: "proj:epi_stored",
         30: "sm:wait_S", 31: "sm:S_ready", 32: "sm:pass1", 33: "sm:pass2", 34: "sm:O_ready", 35: "sm:epi_done"}
 op = sys.argv[1] if len(sys.argv) > 1 else "attn"
 maxe = int(sys.argv[2]) if len(sys.argv) > 2 else 400
