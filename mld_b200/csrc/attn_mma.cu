@@ -250,9 +250,8 @@ bool mma_attention_supported(const AttnArgs& a) {
   return smem <= 227 * 1024;
 }
 
-void mma_attention_init() {
-  cudaFuncSetAttribute(k_attn_mma<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-  cudaFuncSetAttribute(k_attn_mma<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+bool mma_attention_init() {
+  return smem_opt_in(k_attn_mma<64>, 227 * 1024, "k_attn_mma") && smem_opt_in(k_attn_mma<128>, 227 * 1024, "k_attn_mma");
 }
 
 void mma_attention(const AttnArgs& a, cudaStream_t st) {

@@ -18,10 +18,6 @@
 //                                   the register-operand layout of a 16-deep k-step; B = V_kb exactly as
 //                                   TMA delivers the [keys x d] box: an MN-major operand, no transpose)
 // every product in the 3-term split-fp16 form (hi.hi + lo.hi + hi.lo, fp32 accumulation).
-#include <stdio.h>
-#include <stdlib.h>
-#include <string.h>
-
 #include "ops.cuh"
 #include "tc_common.cuh"
 
@@ -71,10 +67,6 @@ __device__ __forceinline__ float quad_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
   return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
 
 // CAUSAL is a template parameter so that the non-causal instantiations (the sampling path) carry no mask state.
 // KB (2 or 4) sizes the score row held in registers: S[KB][32] is 32 * KB registers per thread, and the consumer
@@ -94,7 +86,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   static_assert(KB >= 1 && KB <= MAX_KB, "score row");
   static_assert(RS >= 2 && RS <= MAX_RS, "ring depth");
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * PIPE_BYTES);
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -208,17 +200,9 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
         const uint32_t kbase = smem_u32(sR + sl_i * SLOT_BYTES);
         wg_fence();
 #pragma unroll
-        for (int sl = 0; sl < NS; ++sl) {
-          uint64_t qh = make_desc(qbase + sl * TILE), ql = make_desc(qbase + SL_PLANE + sl * TILE);
-          uint64_t kh = make_desc(kbase + sl * TILE), kl = make_desc(kbase + SL_PLANE + sl * TILE);
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {
-            wgmma_ss_n64(S[kb], ql, kh, (sl | kk) != 0 ? 1u : 0u);
-            wgmma_ss_n64(S[kb], qh, kl, 1u);
-            wgmma_ss_n64(S[kb], qh, kh, 1u);
-            qh += 2; ql += 2; kh += 2; kl += 2;       // next 16 elements of the head dimension: +32 B
-          }
-        }
+        for (int sl = 0; sl < NS; ++sl)               // one k-block per 64-wide slice of the head dimension
+          kblock_ss<64>(S[kb], qbase + sl * TILE, qbase + SL_PLANE + sl * TILE, kbase + sl * TILE,
+                        kbase + SL_PLANE + sl * TILE, sl == 0);
         wg_commit();
         if (kb > 0) {
           wg_wait<1>();
@@ -341,30 +325,8 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   tl_event(p.tl, tl_n, 42);                       // kernel exit
 }
 
-PFN_tmapEncodeTiled g_encode = nullptr;
 int g_sm_count = 132;
 bool g_ready = false;
-
-// fp16 plane [rows, cols]; box = 64 columns x box_rows rows, SWIZZLE_128B, out-of-bounds rows zero-filled
-bool make_map(CUtensorMap* m, const __half* base, int rows, int cols, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(__half)};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-// the same plane seen as [nseq, L, cols]: a box never reaches past its own sequence, rows >= L are zero-filled
-bool make_seq_map(CUtensorMap* m, const __half* base, int nseq, int L, int cols, int box_rows) {
-  cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)L, (cuuint64_t)nseq};
-  cuuint64_t strides[2] = {(cuuint64_t)cols * sizeof(__half), (cuuint64_t)L * cols * sizeof(__half)};
-  cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
-  cuuint32_t estr[3] = {1, 1, 1};
-  return g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, (void*)base, dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
 
 // launch geometry for a shape; false when it does not fit
 bool plan_shape(const AttnArgs& a, AtcParams* p) {
@@ -383,18 +345,12 @@ auto pick_kernel(int nkb) { return nkb <= 2 ? k_attn_tc<HD, CAUSAL, 2> : k_attn_
 
 bool tc_attention_init(int device) {
   if (g_ready) return true;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || !fn)
-    return false;
-  g_encode = (PFN_tmapEncodeTiled)fn;
   cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, device);
   using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, AtcParams);
   const Kernel kernels[] = {k_attn_tc<64, false, 2>, k_attn_tc<64, false, 4>, k_attn_tc<64, true, 2>, k_attn_tc<64, true, 4>,
                             k_attn_tc<128, false, 2>, k_attn_tc<128, false, 4>, k_attn_tc<128, true, 2>, k_attn_tc<128, true, 4>};
   for (Kernel k : kernels)
-    if (cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess) return false;
+    if (!smem_opt_in(k, SMEM_BYTES, "k_attn_tc")) return false;
   g_ready = true;
   return true;
 }
@@ -424,11 +380,7 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   p.out_hi = a.out.hi; p.out_lo = a.out.lo(); p.ld_out = a.out.cols;
   p.scale_log2e = 1.4426950408889634f / sqrtf((float)a.hd);
   p.tl = tc::mldb_timeline_buffer();
-  // Snake order across the per-layer kernels: the GEMMs walk the token tiles upwards, attention and the fused FFN
-  // downwards, so every kernel starts on the rows its producer wrote LAST - those are the ones most likely to be
-  // still in L2.  MLDB_SNAKE=0 turns it off (A/B).
-  static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
-  p.reverse = snake;
+  p.reverse = tc::snake_order();
   p.items = p.nseq * p.heads * p.n_qt;
   p.heads_log2 = -1;
   for (int k = 0; k < 8; ++k) if ((1 << k) == p.heads) p.heads_log2 = k;

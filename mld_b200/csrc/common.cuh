@@ -4,6 +4,10 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <string>
+
+void mldb_set_err(const std::string& s);   // engine.cu: the message mldb_last_error() returns
+
 // ---------------------------------------------------------------------------------------
 // "split16" activation format.  Every activation tensor that feeds a GEMM is stored as two
 // fp16 planes hi = fp16(x), lo = fp16(x - hi); hi + lo carries ~22 significant bits.  The
@@ -83,6 +87,14 @@ template <typename... KArgs, typename... Args>
 static inline void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                               Args&&... args) {
   launch_pdl_cluster(kernel, grid, block, smem, st, 1, static_cast<Args&&>(args)...);
+}
+// Opt `kernel` in to `bytes` of dynamic shared memory (outside stream capture).  false: the attribute was refused
+// and mldb_last_error() says so.
+template <typename... KArgs>
+static inline bool smem_opt_in(void (*kernel)(KArgs...), int bytes, const char* name) {
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) mldb_set_err(std::string("cudaFuncSetAttribute(") + name + "): " + cudaGetErrorString(e));
+  return e == cudaSuccess;
 }
 #endif
 

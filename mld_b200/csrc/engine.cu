@@ -670,12 +670,11 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   build_alphas(h->cfg, &h->alphas_cumprod);
   cudaError_t e = cudaStreamCreateWithFlags(&h->cap_stream, cudaStreamNonBlocking);
   if (e != cudaSuccess) { delete h; FAIL(MLDB_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
-  simt_init();
-  mma_attention_init();
+  // kernel setup: each step records its own message in mldb_last_error() when it fails
+  if (!simt_init() || !mma_attention_init()) { delete h; return MLDB_ERR_CUDA; }
   h->tc = tc_create(device);
   if (!h->tc) { delete h; return MLDB_ERR_CUDA; }
-  if (!tc_attention_init(device)) { tc_destroy(h->tc); delete h; FAIL(MLDB_ERR_CUDA, "wgmma attention kernel: setup failed"); }
-  if (!gru_tc_init(device)) { tc_destroy(h->tc); delete h; FAIL(MLDB_ERR_CUDA, "wgmma GRU step kernel: setup failed"); }
+  if (!tc_attention_init(device) || !gru_tc_init()) { tc_destroy(h->tc); delete h; return MLDB_ERR_CUDA; }
   const char* env = getenv("MLDB_GEMM");
   if (env && !strcmp(env, "simt")) h->use_tc = false;
   env = getenv("MLDB_GRAPH");

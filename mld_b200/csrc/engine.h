@@ -192,8 +192,6 @@ struct mldb_handle {
   int64_t gather_count = 0;
 };
 
-// helpers implemented in engine.cu
-void mldb_set_err(const std::string& s);
 // comm.cu
 void mldb_comm_release(mldb_handle* h);
 int mldb_gather_begin(mldb_handle* h, cudaStream_t stream);

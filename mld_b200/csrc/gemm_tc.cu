@@ -23,16 +23,9 @@
 //   fp32:      bias + activation -> fp32 with float2 stores, identity row mapping (GemmArgs::vec_f32: the T2M evaluator).
 #include "gemm_tc.h"
 
-#include <stdio.h>
-#include <stdlib.h>
-
 #include <algorithm>
-#include <string>
-#include <string.h>
 
 #include "tc_common.cuh"
-
-void mldb_set_err(const std::string& s);
 
 namespace {
 using namespace tc;
@@ -75,29 +68,6 @@ struct TileCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-template <int BN>
-__device__ __forceinline__ void wgmma_ss(float (&d)[BN / 2], uint64_t a, uint64_t b, uint32_t acc) {
-  if constexpr (BN == 256) wgmma_ss_n256(d, a, b, acc);
-  else if constexpr (BN == 128) wgmma_ss_n128(d, a, b, acc);
-  else wgmma_ss_n64(d, a, b, acc);
-}
-// one k-block (64 deep) of this warpgroup's [64 x BN] tile: 4 x (A_lo.W_hi + A_hi.W_lo + A_hi.W_hi)
-template <int BN>
-__device__ __forceinline__ void kblock_ss(float (&d)[BN / 2], uint32_t sAh, uint32_t sAl, uint32_t sWh, uint32_t sWl, bool first) {
-  uint64_t ah = make_desc(sAh), al = make_desc(sAl), wh = make_desc(sWh), wl = make_desc(sWl);
-#pragma unroll
-  for (int kk = 0; kk < BK / 16; ++kk) {
-    wgmma_ss<BN>(d, al, wh, (first && kk == 0) ? 0u : 1u);
-    wgmma_ss<BN>(d, ah, wl, 1u);
-    wgmma_ss<BN>(d, ah, wh, 1u);
-    ah += 2; al += 2; wh += 2; wl += 2;                // next 16-wide slice: +32 B (>> 4)
-  }
-}
-
-__device__ __forceinline__ float quad_sum(float v) {
-  v += __shfl_xor_sync(0xffffffffu, v, 1);
-  return v + __shfl_xor_sync(0xffffffffu, v, 2);
-}
 __device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, float x0, float x1) {
   uint32_t h, l;
   split2(x0, x1, h, l);
@@ -215,8 +185,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
   using Cfg = TileCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-B alignment by pointer arithmetic (an integer round trip would lose the shared address space)
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);   // [STAGES] TMA tx
   uint64_t* bar_empty = bar_full + STAGES;                                              // [STAGES] one arrival per consumer warp
 
@@ -443,7 +412,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   using Cfg = FfnCfg;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint8_t* ring = smem + Cfg::X_BYTES;
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
   uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
@@ -724,7 +693,7 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   using Cfg = ProjCfg;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint8_t* ring = smem + Cfg::A_BYTES;
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
   uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
@@ -890,26 +859,15 @@ struct TcCtx {
   int sm_count = 132;
   int ffn_fused = 1;          // FFN1 + GELU + FFN2 + residual + LayerNorm as one launch (option ffn_fused)
   int ffn_split = 1;          // cut the leftover tiles of the fused FFN along the hidden dimension (option ffn_split)
-  tc::PFN_tmapEncodeTiled encode = nullptr;
 };
 
 TcCtx* tc_create(int device) {
+  if (!tc::tmap_encoder()) return nullptr;
   TcCtx* c = new TcCtx();
   c->device = device;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres);
-  if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) {
-    mldb_set_err("cuTensorMapEncodeTiled is not available from the driver");
-    delete c;
-    return nullptr;
-  }
-  c->encode = (tc::PFN_tmapEncodeTiled)fn;
   cudaDeviceGetAttribute(&c->sm_count, cudaDevAttrMultiProcessorCount, device);
-  e = cudaSuccess;
-  auto opt_in = [&](auto kernel, int bytes) {
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  };
+  bool ok = true;
+  auto opt_in = [&](auto kernel, int bytes) { ok = ok && smem_opt_in(kernel, bytes, "k_gemm_tc"); };
   opt_in(k_gemm_tc<256, EPI_FAST>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_FAST, ACT_GELU>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_FAST, ACT_GELU>, TileCfg<128>::SMEM_BYTES);
   opt_in(k_gemm_tc<256, EPI_GENERIC>, TileCfg<256>::SMEM_BYTES); opt_in(k_gemm_tc<128, EPI_GENERIC>, TileCfg<128>::SMEM_BYTES);
@@ -923,27 +881,13 @@ TcCtx* tc_create(int device) {
   opt_in(k_ffn_tc, FfnCfg::SMEM_BYTES);
   opt_in(k_proj_tc<ACT_NONE>, ProjCfg::SMEM_BYTES); opt_in(k_proj_tc<ACT_GELU>, ProjCfg::SMEM_BYTES);
   opt_in(k_proj_tc<ACT_QUICKGELU>, ProjCfg::SMEM_BYTES); opt_in(k_proj_tc<ACT_LEAKY>, ProjCfg::SMEM_BYTES);
-  if (e != cudaSuccess) {
-    mldb_set_err(std::string("cudaFuncSetAttribute(k_gemm_tc): ") + cudaGetErrorString(e));
+  if (!ok) {
     delete c;
     return nullptr;
   }
   return c;
 }
 void tc_destroy(TcCtx* c) { delete c; }
-
-// 2-D map over one fp16 plane [rows, cols] (cols contiguous), box = 64 cols x box_rows, 128B swizzle.
-// Out-of-bounds rows/cols are zero-filled, so M and N need not be tile multiples.
-static bool make_map(const TcCtx* c, CUtensorMap* m, const __half* base, int rows, int cols, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(__half)};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = c->encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
 
 static int pick_bn(const GemmArgs& g) { return (g.w.N % 256 == 0) ? 256 : 128; }
 
@@ -991,20 +935,13 @@ static void fill_params(const GemmArgs& g, const LnArgs* ln, int bn, TcParams* o
   *out = p;
 }
 
-static bool map_fail(const char* what, int M, int N, int K) {
-  char buf[160];
-  snprintf(buf, sizeof buf, "cuTensorMapEncodeTiled failed (%s M=%d N=%d K=%d)", what, M, N, K);
-  mldb_set_err(buf);
-  return false;
-}
-
 // k_proj_tc: the fast epilogue with K = 256 from one A source (every N here is a multiple of 128)
 static bool tc_proj(TcCtx* c, const GemmArgs& g, cudaStream_t st) {
   CUtensorMap mAh, mAl, mWh, mWl;
-  const bool ok = make_map(c, &mAh, g.a1.hi, g.M, g.K1, BM) && make_map(c, &mAl, g.a1.lo(), g.M, g.K1, BM) &&
-                  make_map(c, &mWh, g.w.w, g.w.N, g.w.K, ProjCfg::CHUNK) &&
-                  make_map(c, &mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, ProjCfg::CHUNK);
-  if (!ok) return map_fail("proj", g.M, g.w.N, g.w.K);
+  const bool ok = make_map(&mAh, g.a1.hi, g.M, g.K1, BM) && make_map(&mAl, g.a1.lo(), g.M, g.K1, BM) &&
+                  make_map(&mWh, g.w.w, g.w.N, g.w.K, ProjCfg::CHUNK) &&
+                  make_map(&mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, ProjCfg::CHUNK);
+  if (!ok) return false;
   ProjParams p{};
   p.M = g.M; p.n_chunks = g.w.N / ProjCfg::CHUNK; p.items = (g.M + BM - 1) / BM * p.n_chunks;
   p.inv_scale = g.w.inv_scale; p.bias = g.w.bias;
@@ -1031,11 +968,11 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   if (fast && g.K1 == 256 && g.K2 == 0 && ((uintptr_t)g.out.hi & 15) == 0 && ((uintptr_t)g.out.lo() & 15) == 0)
     return tc_proj(c, g, st);
   CUtensorMap mA1h, mA1l, mA2h, mA2l, mWh, mWl;
-  bool ok = make_map(c, &mA1h, g.a1.hi, g.M, g.K1, BM) && make_map(c, &mA1l, g.a1.lo(), g.M, g.K1, BM);
-  if (g.K2 > 0) ok = ok && make_map(c, &mA2h, g.a2.hi, g.M, g.K2, BM) && make_map(c, &mA2l, g.a2.lo(), g.M, g.K2, BM);
+  bool ok = make_map(&mA1h, g.a1.hi, g.M, g.K1, BM) && make_map(&mA1l, g.a1.lo(), g.M, g.K1, BM);
+  if (g.K2 > 0) ok = ok && make_map(&mA2h, g.a2.hi, g.M, g.K2, BM) && make_map(&mA2l, g.a2.lo(), g.M, g.K2, BM);
   else { mA2h = mA1h; mA2l = mA1l; }
-  ok = ok && make_map(c, &mWh, g.w.w, g.w.N, g.w.K, bn) && make_map(c, &mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, bn);
-  if (!ok) return map_fail("gemm", g.M, g.w.N, g.w.K);
+  ok = ok && make_map(&mWh, g.w.w, g.w.N, g.w.K, bn) && make_map(&mWl, g.w.w + g.w.plane_stride, g.w.N, g.w.K, bn);
+  if (!ok) return false;
   TcParams p;
   fill_params(g, ln, bn, &p);
   // the vectorised fp32 epilogue, for callers that ask for it (vec_f32)
@@ -1090,12 +1027,12 @@ bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, co
 bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* scratch, int* flags, cudaStream_t st) {
   CUtensorMap mXh, mXl, mW1h, mW1l, mW2h, mW2l;
   const int m_tiles = (g1.M + BM - 1) / BM;
-  const bool ok = make_map(c, &mXh, g1.a1.hi, g1.M, g1.K1, BM) && make_map(c, &mXl, g1.a1.lo(), g1.M, g1.K1, BM) &&
-                  make_map(c, &mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
-                  make_map(c, &mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
-                  make_map(c, &mW2h, g2.w.w, g2.w.N, g2.w.K, 256) &&
-                  make_map(c, &mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256);
-  if (!ok) return map_fail("ffn", g1.M, g1.w.N, g1.w.K);
+  const bool ok = make_map(&mXh, g1.a1.hi, g1.M, g1.K1, BM) && make_map(&mXl, g1.a1.lo(), g1.M, g1.K1, BM) &&
+                  make_map(&mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+                  make_map(&mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+                  make_map(&mW2h, g2.w.w, g2.w.N, g2.w.K, 256) &&
+                  make_map(&mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256);
+  if (!ok) return false;
   FfnParams p{};
   p.M = g1.M; p.m_tiles = m_tiles; p.n_chunks = g1.w.N / FfnCfg::CHUNK;
   p.tl = tc::mldb_timeline_buffer();
@@ -1114,8 +1051,7 @@ bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, 
     if (parts >= 2 && (size_t)p.left * (parts - 1) * (BM * 256 * 4) <= TC_FFN_SCRATCH_BYTES) p.parts = parts;
   }
   const int ncta = p.full > 0 ? ncta_max : p.left * p.parts;
-  static const int snake = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
-  p.reverse = snake;
+  p.reverse = tc::snake_order();
   launch_pdl(k_ffn_tc, dim3(ncta), dim3(MMA_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
   return true;
 }

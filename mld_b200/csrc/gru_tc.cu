@@ -19,12 +19,8 @@
 // CTA = three warpgroups as in k_gemm_tc (gemm_tc.cu): warp 0 streams the A (state) and W_hh k-blocks through a
 // ring of 128B-swizzled stages with TMA, warpgroups 1 and 2 each own 64 rows of the 128-row tile.  Grid =
 // (H / 32 unit tiles, row tiles, 2 directions); no CTA waits on another, steps are ordered by the stream.
-#include <string>
-
 #include "ops.cuh"
 #include "tc_common.cuh"
-
-void mldb_set_err(const std::string& s);
 
 namespace {
 using namespace tc;
@@ -36,28 +32,6 @@ constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;       // 56 KB
 constexpr int STAGES = 4;
 constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
 static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-
-tc::PFN_tmapEncodeTiled g_encode = nullptr;
-
-// D[64 x 96] (+)= A[64 x 16] . B[16 x 96], both K-major in shared memory
-__device__ __forceinline__ void wgmma_ss_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %50, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
-      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
-      "%48, %49, p, 1, 1, 0, 0;\n\t}"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
-        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
-        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
-      : "l"(adesc), "l"(bdesc), "r"(acc)
-      : "memory");
-}
 
 // accurate expf / tanhf (not the fast intrinsics): the recurrence compounds their error over up to 49 steps
 __device__ __forceinline__ float gru_cell(float gr, float gz, float gn, float hr, float hz, float hn, float h) {
@@ -92,7 +66,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1)
 k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
               const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const GruStepArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* bar_empty = bar_full + STAGES;
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
@@ -140,16 +114,9 @@ k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ 
     const int s = kb % STAGES;
     mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kb / STAGES)) & 1u);
     const uint32_t base = smem_u32(smem + s * STAGE_BYTES);
-    uint64_t ah = make_desc(base + cw * (64 * 128)), al = make_desc(base + A_BYTES + cw * (64 * 128));
-    uint64_t wh = make_desc(base + 2 * A_BYTES), wl = make_desc(base + 2 * A_BYTES + W_BYTES);
     wg_fence();
-#pragma unroll
-    for (int kk = 0; kk < BK / 16; ++kk) {
-      wgmma_ss_n96(d, al, wh, (kb == 0 && kk == 0) ? 0u : 1u);
-      wgmma_ss_n96(d, ah, wl, 1u);
-      wgmma_ss_n96(d, ah, wh, 1u);
-      ah += 2; al += 2; wh += 2; wl += 2;
-    }
+    kblock_ss<BN>(d, base + cw * (64 * 128), base + A_BYTES + cw * (64 * 128), base + 2 * A_BYTES,
+                  base + 2 * A_BYTES + W_BYTES, kb == 0);
     wg_commit();
     if (kb > 0) {
       wg_wait<1>();
@@ -253,30 +220,10 @@ __global__ void k_im2col_k4s2(ActBuf X, const float* __restrict__ src, int64_t l
   X.lo()[idx] = lo;
 }
 
-bool make_map(CUtensorMap* m, const __half* base, int rows, int cols, int box_rows) {
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(__half)};
-  cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return g_encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, (void*)base, dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 }  // namespace
 
-bool gru_tc_init(int device) {
-  (void)device;
-  if (g_encode) return true;
-  void* fn = nullptr;
-  cudaDriverEntryPointQueryResult q;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
-      q != cudaDriverEntryPointSuccess || !fn)
-    return false;
-  if (cudaFuncSetAttribute(k_gru_step_tc, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES) != cudaSuccess)
-    return false;
-  g_encode = (tc::PFN_tmapEncodeTiled)fn;
-  return true;
+bool gru_tc_init() {
+  return smem_opt_in(k_gru_step_tc, SMEM_BYTES, "k_gru_step_tc");
 }
 
 bool gru_shape_supported(int H) { return H >= 64 && H <= 1024 && H % 64 == 0; }
@@ -285,10 +232,7 @@ bool gru_step_tc(const GruStepArgs& a, cudaStream_t st) {
   CUtensorMap mAh, mAl, mWh, mWl;
   const bool ok = make_map(&mAh, a.h_in.hi, 2 * a.rows_pad, a.H, BM) && make_map(&mAl, a.h_in.lo(), 2 * a.rows_pad, a.H, BM) &&
                   make_map(&mWh, a.w_hh, 6 * a.H, a.H, BN) && make_map(&mWl, a.w_hh + a.w_plane_stride, 6 * a.H, a.H, BN);
-  if (!ok) {
-    mldb_set_err("cuTensorMapEncodeTiled failed (gru step, H=" + std::to_string(a.H) + ")");
-    return false;
-  }
+  if (!ok) return false;
   const dim3 grid((unsigned)(a.H / UNITS), (unsigned)((a.rows + BM - 1) / BM), 2);
   launch_pdl(k_gru_step_tc, grid, dim3(NUM_THREADS), SMEM_BYTES, st, mAh, mAl, mWh, mWl, a);
   return true;

@@ -82,13 +82,13 @@ bool simt_attention(const AttnArgs& a, cudaStream_t st);
 bool simt_attention_supported(int hd);
 // --- mma.sync tensor-core attention (attn_mma.cu) ---
 bool mma_attention_supported(const AttnArgs& a);
-void mma_attention_init();
+bool mma_attention_init();                                // outside stream capture
 void mma_attention(const AttnArgs& a, cudaStream_t st);
 // attn_tc.cu: wgmma attention core (Lk <= 256, head_dim 64 / 128)
 bool tc_attention_init(int device);                       // once per process, outside stream capture
 bool tc_attention_supported(const AttnArgs& a);
 bool tc_attention(const AttnArgs& a, cudaStream_t st);    // false: tensor-map encoding failed, nothing launched
-void simt_init();
+bool simt_init();                                         // reads MLDB_PDL; outside stream capture
 // --- CLIP text tower row kernels (text_ln.cu) ---
 // One warp per row, d a multiple of 128 up to 1024, exact two-pass statistics, no shared memory.
 //   TEXT_LN_ROWS:  out = LN(x[r])                                   (pre-norm LN1 / LN2, final LN of every row)
@@ -129,7 +129,7 @@ __host__ __device__ __forceinline__ int gru_packed_col(int g, int u) {
   const int t = u >> 5, uu = u & 31;
   return t * 96 + (3 * (uu >> 3) + g) * 8 + (uu & 7);
 }
-bool gru_tc_init(int device);                                    // once per process, outside stream capture
+bool gru_tc_init();                                              // once per process, outside stream capture
 bool gru_shape_supported(int H);                                 // 64 <= H <= 1024, H % 64 == 0
 bool gru_step_tc(const GruStepArgs& a, cudaStream_t st);         // false: tensor-map encoding failed, nothing launched
 void gru_gate_simt(const GruStepArgs& a, cudaStream_t st);       // the gate update from a.gh (CUDA cores)

@@ -445,10 +445,9 @@ bool simt_attention_supported(int hd) { return hd >= 1 && attn_chunk(hd, 1 << 30
 
 int g_mldb_pdl = 1;
 
-void simt_init() {
+bool simt_init() {
   if (const char* e = getenv("MLDB_PDL")) g_mldb_pdl = atoi(e) != 0;
-  // opt in to the full 227 KB once (not during stream capture)
-  cudaFuncSetAttribute(k_attn_simt, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ATT_SMEM_MAX);
+  return smem_opt_in(k_attn_simt, (int)ATT_SMEM_MAX, "k_attn_simt");
 }
 
 bool simt_attention(const AttnArgs& a, cudaStream_t st) {

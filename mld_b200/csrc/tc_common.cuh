@@ -1,13 +1,25 @@
-// PTX wrappers shared by the warpgroup-MMA kernels (gemm_tc.cu, attn_tc.cu): mbarriers, TMA (bulk tensor
-// copies), wgmma.mma_async and its shared-memory matrix descriptors.  sm_90a only.
+// PTX wrappers shared by the warpgroup-MMA kernels (gemm_tc.cu, attn_tc.cu, gru_tc.cu): mbarriers, TMA (bulk
+// tensor copies), wgmma.mma_async and its shared-memory matrix descriptors, the split16 k-block; on the host, the
+// tensor maps of split16 planes.  sm_90a only.
 #pragma once
 #include <cuda.h>
+#include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
+
+#include <string>
 
 #include "common.cuh"
 
 namespace tc {
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+// Bytes from the dynamic shared-memory window `raw` up to the next 1024-B boundary: a 128B-swizzled tile (TMA box
+// and wgmma descriptor, make_desc) must start on one, so every kernel reserves 1024 B of slack and takes its tiles
+// from raw + smem_pad1024(raw) (pointer arithmetic: an integer round trip would lose the shared address space).
+// An offset rather than the aligned pointer: nvcc folds a returned pointer into k_ffn_tc's and k_proj_tc's ring
+// addresses differently.
+__device__ __forceinline__ uint32_t smem_pad1024(const void* raw) { return (1024u - (smem_u32(raw) & 1023u)) & 1023u; }
 
 // ---------------------------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -174,6 +186,25 @@ __device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t adesc, ui
       : "l"(adesc), "l"(bdesc), "r"(acc)
       : "memory");
 }
+// D[64 x 96] (+)= A[64 x 16] . B[16 x 96], both K-major in shared memory
+__device__ __forceinline__ void wgmma_ss_n96(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "%48, %49, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+      : "l"(adesc), "l"(bdesc), "r"(acc)
+      : "memory");
+}
 // D[64 x 64] (+)= A[64 x 16] . B[16 x 64], both K-major in shared memory
 __device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t acc) {
   asm volatile(
@@ -241,6 +272,36 @@ __device__ __forceinline__ void wgmma_rs_n64_tb(float (&d)[32], const uint32_t (
       : "memory");
 }
 
+template <int N>
+__device__ __forceinline__ void wgmma_ss(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+  static_assert(N == 256 || N == 128 || N == 96 || N == 64, "wgmma_ss width");
+  if constexpr (N == 256) wgmma_ss_n256(d, a, b, acc);
+  else if constexpr (N == 128) wgmma_ss_n128(d, a, b, acc);
+  else if constexpr (N == 96) wgmma_ss_n96(d, a, b, acc);
+  else wgmma_ss_n64(d, a, b, acc);
+}
+// The split16 product of one k-block into a warpgroup's [64 x N] tile: four 16-deep steps of
+// A_lo.W_hi + A_hi.W_lo + A_hi.W_hi, in that order, both operands K-major and 64 deep (one 128B swizzle row).
+// `first` makes the first MMA overwrite the accumulator.  Every shared-memory-operand kernel goes through here:
+// this order fixes the bits of its results.
+template <int N>
+__device__ __forceinline__ void kblock_ss(float (&d)[N / 2], uint32_t sAh, uint32_t sAl, uint32_t sWh, uint32_t sWl, bool first) {
+  uint64_t ah = make_desc(sAh), al = make_desc(sAl), wh = make_desc(sWh), wl = make_desc(sWl);
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    wgmma_ss<N>(d, al, wh, (first && kk == 0) ? 0u : 1u);
+    wgmma_ss<N>(d, ah, wl, 1u);
+    wgmma_ss<N>(d, ah, wh, 1u);
+    ah += 2; al += 2; wh += 2; wl += 2;                // next 16-wide slice: +32 B (>> 4)
+  }
+}
+
+// sum over the 4 lanes of a quad (the lanes that hold one accumulator row)
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
 // fp32 pair -> packed fp16 hi pair and lo pair (x = hi + lo to ~22 bits)
 __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_t& lo) {
   const __half2 h2 = __floats2half2_rn(x0, x1);
@@ -264,9 +325,68 @@ __device__ __forceinline__ void tl_event(long long* tl, int& n, int tag, int aux
 }
 long long* mldb_timeline_buffer();   // engine.cu: the device buffer while a timeline is being recorded, else nullptr
 
+// ---------------------------------------------------------------------------------- host: tensor maps
 typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                         CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
                                         CUtensorMapFloatOOBfill);
+
+// The driver's cuTensorMapEncodeTiled, looked up once per process.  nullptr (and mldb_last_error() set) when the
+// driver does not provide it.
+inline PFN_tmapEncodeTiled tmap_encoder() {
+  static const PFN_tmapEncodeTiled fn = [] {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    const cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q);
+    return e == cudaSuccess && q == cudaDriverEntryPointSuccess ? (PFN_tmapEncodeTiled)p : nullptr;
+  }();
+  if (!fn) mldb_set_err("cuTensorMapEncodeTiled is not available from the driver");
+  return fn;
+}
+
+// A tensor map of one split16 plane (fp16, columns contiguous): boxes of 64 columns (one 128B swizzle row) x
+// box[1] rows, SWIZZLE_128B, L2 256B promotion, and elements outside the plane zero-filled - so M and N need not
+// be tile multiples, and a box never brings in rows of another sequence (DESIGN §2).  dims / strides / box are
+// innermost first.  false: encoding failed and mldb_last_error() names the plane.
+inline bool encode_plane_map(CUtensorMap* m, const __half* base, int rank, const cuuint64_t* dims,
+                             const cuuint64_t* strides, const cuuint32_t* box) {
+  const PFN_tmapEncodeTiled encode = tmap_encoder();
+  if (!encode) return false;
+  const cuuint32_t estr[3] = {1, 1, 1};
+  const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, (void*)base, dims, strides, box,
+                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    std::string shape;
+    for (int i = rank - 1; i >= 0; --i) shape += std::to_string(dims[i]) + (i ? " x " : "");
+    char buf[96];
+    snprintf(buf, sizeof buf, "(CUresult %d): fp16 plane at %p", (int)r, (const void*)base);
+    mldb_set_err("cuTensorMapEncodeTiled failed " + std::string(buf) + ", [" + shape + "], box " +
+                 std::to_string(box[1]) + " rows");
+  }
+  return r == CUDA_SUCCESS;
+}
+// a [rows, cols] plane
+inline bool make_map(CUtensorMap* m, const __half* base, int rows, int cols, int box_rows) {
+  const cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  const cuuint64_t strides[1] = {(cuuint64_t)cols * sizeof(__half)};
+  const cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  return encode_plane_map(m, base, 2, dims, strides, box);
+}
+// the same plane seen as [nseq, L, cols]: a box never reaches past its own sequence, rows >= L are zero-filled
+inline bool make_seq_map(CUtensorMap* m, const __half* base, int nseq, int L, int cols, int box_rows) {
+  const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)L, (cuuint64_t)nseq};
+  const cuuint64_t strides[2] = {(cuuint64_t)cols * sizeof(__half), (cuuint64_t)L * cols * sizeof(__half)};
+  const cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
+  return encode_plane_map(m, base, 3, dims, strides, box);
+}
+
+// Snake order across the per-layer kernels: the GEMMs walk the token tiles upwards, attention and the fused FFN
+// downwards, so every kernel starts on the rows its producer wrote LAST - those are the ones most likely to be
+// still in L2.  MLDB_SNAKE=0 turns it off (A/B); read once per process.
+inline int snake_order() {
+  static const int on = [] { const char* e = getenv("MLDB_SNAKE"); return (e && !strcmp(e, "0")) ? 0 : 1; }();
+  return on;
+}
 
 }  // namespace tc

@@ -47,6 +47,25 @@ def test_no_cpu_fallback(built_lib):
         Engine(cfg, 0)
 
 
+@pytest.mark.parametrize("field, value, code, cause", [
+    ("abi_version", -1, 1, b"abi_version"),
+    ("latent_dim", 250, 1, b"latent_dim must be a multiple"),
+    ("latent_dim", 2048, 4, b"latent_dim > 1024"),
+])
+def test_create_failure_records_its_own_message(built_lib, field, value, code, cause):
+    """A refused mldb_create names its own cause: the message of an earlier failure is never left behind."""
+    stale = _lib.default_config()
+    stale.eta = 1.25
+    assert built_lib.mldb_create(C.byref(stale), 0, C.byref(C.c_void_p())) == 1
+    assert b"eta" in built_lib.mldb_last_error()
+    cfg = _lib.default_config()
+    setattr(cfg, field, value)
+    h = C.c_void_p()
+    assert built_lib.mldb_create(C.byref(cfg), 0, C.byref(h)) == code and h.value is None
+    msg = built_lib.mldb_last_error()
+    assert cause in msg and b"eta" not in msg, msg
+
+
 def test_modules_keep_reference_state_dict_keys():
     """The drop-in modules expose exactly the reference's state-dict keys and shapes."""
     from types import SimpleNamespace
