@@ -176,7 +176,12 @@ int mldb_vae_decode(mldb_handle* h, const float* z, const int32_t* lengths, int3
                     int32_t T, float* feats_out, void* stream);
 
 /* Replaces: vae.encode(features, lengths) up to the distribution parameters
- * (mld_vae.py:124-178): mu, logvar [n_lat, B, d]; the rsample() at :181-183 stays in torch. */
+ * (mld_vae.py:124-178): mu, logvar [n_lat, B, d]; the rsample() at :181-183 stays in torch.
+ * ActorVae (actor_vae.py:62-75,120-170): mu, logvar [1, B, d] (n_lat != 1 is MLDB_ERR_UNSUPPORTED); T + 2 may
+ * reach the 5000 rows of its sine PE table.  Its "vae.encoder.*" keys are all or none: a decoder-only state dict
+ * finalizes and decodes, and this call then returns MLDB_ERR_STATE; a partial set fails mldb_finalize_weights,
+ * which names the first missing key.
+ * feats [B, T, nfeats] fp32 device; lengths device int32[B], each in [1, T]; frames past a length must be finite. */
 int mldb_vae_encode(mldb_handle* h, const float* feats, const int32_t* lengths, int32_t B,
                     int32_t T, float* mu, float* logvar, void* stream);
 

@@ -160,6 +160,14 @@ static int build_spec(mldb_handle* h) {
     spec_add(h, V + "final_layer.weight", {c.vae_nfeats, d});
     spec_add(h, V + "final_layer.bias", {c.vae_nfeats});
   } else if (c.vae_kind == MLDB_VAE_ACTOR) {
+    // the encoder half (actor_vae.py:86-118) is all or none: see mldb_finalize_weights
+    spec_add(h, V + "encoder.mu_token", {d});
+    spec_add(h, V + "encoder.logvar_token", {d});
+    spec_add(h, V + "encoder.skel_embedding.weight", {d, c.vae_nfeats});
+    spec_add(h, V + "encoder.skel_embedding.bias", {d});
+    spec_add(h, V + "encoder.sequence_pos_encoding.pe", {5000, 1, d});
+    for (int i = 0; i < c.vae_layers; ++i)
+      spec_layer(h, V + "encoder.seqTransEncoder.layers." + std::to_string(i) + ".", d, c.vae_ff, false);
     spec_add(h, V + "decoder.sequence_pos_encoding.pe", {5000, 1, d});
     for (int i = 0; i < c.vae_layers; ++i)
       spec_layer(h, V + "decoder.seqTransDecoder.layers." + std::to_string(i) + ".", d, c.vae_ff, true);
@@ -250,6 +258,12 @@ static int pack_dec_layer(mldb_handle* h, const std::string& p, int d, DecW* w) 
   TRY(pack_ln(h, p + "norm3.", d, &w->n3));
   return MLDB_OK;
 }
+// the q rows and the k | v rows of an encoder layer's in_proj as separate operands (enc_layer_selected)
+static int pack_trimmed_qkv(mldb_handle* h, const std::string& p, int d, EncW* w) {
+  TRY(pack_named(h, p + "self_attn.in_proj_weight", p + "self_attn.in_proj_bias", &w->q_only, 0, d));
+  TRY(pack_named(h, p + "self_attn.in_proj_weight", p + "self_attn.in_proj_bias", &w->kv_only, d, 2 * d));
+  return MLDB_OK;
+}
 static int pack_skip_stack(mldb_handle* h, const std::string& p, int d, int ff, int heads, int layers,
                            bool dec, StackW* s) {
   s->kind = dec ? STACK_SKIP_DEC : STACK_SKIP_ENC;
@@ -263,12 +277,8 @@ static int pack_skip_stack(mldb_handle* h, const std::string& p, int d, int ff, 
     if (dec) { s->dec.emplace_back(); TRY(pack_dec_layer(h, n, d, &s->dec.back())); }
     else     { s->enc.emplace_back(); TRY(pack_enc_layer(h, n, d, &s->enc.back())); }
   }
-  if (!dec) {   // the last block only has to produce the first few tokens of every sequence
-    const std::string& n = names.back();
-    EncW& w = s->enc.back();
-    TRY(pack_named(h, n + "self_attn.in_proj_weight", n + "self_attn.in_proj_bias", &w.q_only, 0, d));
-    TRY(pack_named(h, n + "self_attn.in_proj_weight", n + "self_attn.in_proj_bias", &w.kv_only, d, 2 * d));
-  }
+  if (!dec) TRY(pack_trimmed_qkv(h, names.back(), d, &s->enc.back()));   // the last block only has to produce
+                                                                             // the first few tokens of every sequence
   for (int i = 0; i < nb; ++i) {
     s->skip.emplace_back();
     const std::string lp = p + "linear_blocks." + std::to_string(i) + ".";
@@ -281,6 +291,27 @@ static int upload_pe(mldb_handle* h, const std::string& key, float** out, int* r
   const RawTensor& t = rt(h, key);
   if (rows) *rows = (int)t.shape[0];
   return upload_f32(h, t.host.data(), t.host.size(), out);
+}
+// ActorAgnosticEncoder (actor_vae.py:86-118): a plain encoder stack, [mu_token; logvar_token] as a 2-row token
+// table, the skel embedding with K zero-padded for the tensor cores, and the encoder's own sine PE table
+static int pack_actor_encoder(mldb_handle* h) {
+  const mldb_config& c = h->cfg;
+  const int d = c.latent_dim;
+  const std::string E = "vae.encoder.";
+  StackW* s = &h->venc;
+  s->kind = STACK_PLAIN_ENC; s->d = d; s->ff = c.vae_ff; s->heads = c.vae_heads; s->layers = c.vae_layers;
+  for (int i = 0; i < c.vae_layers; ++i) {
+    const std::string n = E + "seqTransEncoder.layers." + std::to_string(i) + ".";
+    s->enc.emplace_back();
+    TRY(pack_enc_layer(h, n, d, &s->enc.back()));
+    if (i == c.vae_layers - 1) TRY(pack_trimmed_qkv(h, n, d, &s->enc.back()));
+  }
+  std::vector<float> tok(rt(h, E + "mu_token").host);
+  const std::vector<float>& lv = rt(h, E + "logvar_token").host;
+  tok.insert(tok.end(), lv.begin(), lv.end());
+  TRY(upload_f32(h, tok.data(), tok.size(), &h->global_token));
+  TRY(pack_named(h, E + "skel_embedding.weight", E + "skel_embedding.bias", &h->skel_emb, 0, -1, true));
+  return upload_pe(h, E + "sequence_pos_encoding.pe", &h->vae_enc_pe, &h->vae_enc_pe_rows);
 }
 
 // ----------------------------------------------------------------------------- scheduler
@@ -453,21 +484,22 @@ static int alloc_stack_ws(mldb_handle* h, const StackW& sw, int nseq, int L, int
   TRY(alloc_act(h, M, d, &ws->att));
   TRY(alloc_act(h, M, 3 * d, &ws->qkv));
   TRY(alloc_act(h, M, sw.ff, &ws->h));
-  if (sw.kind != STACK_SKIP_ENC) {
+  const bool enc = sw.kind == STACK_SKIP_ENC || sw.kind == STACK_PLAIN_ENC;
+  if (!enc) {
     TRY(alloc_act(h, M, d, &ws->x2));
     TRY(alloc_act(h, M, d, &ws->qc));
     TRY(alloc_act(h, nseq * Lmem, 2 * d, &ws->kvm));
     TRY(alloc_act(h, nseq, d, &ws->vrow));
     TRY(dev_alloc(h, (void**)&ws->cvec, (size_t)nseq * d * sizeof(float)));
   }
-  if (sw.kind != STACK_PLAIN_DEC) {
+  if (sw.kind == STACK_SKIP_ENC || sw.kind == STACK_SKIP_DEC) {
     TRY(alloc_act(h, M, d, &ws->cat));
     const int nb = (sw.layers - 1) / 2;
     ws->ys.resize(nb);
     for (int i = 0; i < nb; ++i) TRY(alloc_act(h, M, d, &ws->ys[i]));
   }
   TRY(dev_alloc(h, (void**)&ws->cf32, (size_t)M * d * sizeof(float)));
-  if (sw.kind == STACK_SKIP_ENC && n_sel > 0) {
+  if (enc && n_sel > 0) {
     ws->n_sel = n_sel;
     const int R = nseq * n_sel;
     TRY(alloc_act(h, R, d, &ws->sx));
@@ -610,11 +642,21 @@ static ActBuf enc_layer_selected(mldb_handle* h, const StackW& sw, const EncW& w
   return ws.sout;
 }
 
-// SkipTransformerEncoder/Decoder.forward (cross_attention.py:41-64, 89-125) and the plain
-// decoder stacks (cross_attention.py:204-233; torch nn.TransformerDecoder for ActorVae).
-// Returns the buffer holding the last layer's output (before the stack's final norm).
+// SkipTransformerEncoder/Decoder.forward (cross_attention.py:41-64, 89-125), the plain
+// decoder stacks (cross_attention.py:204-233; torch nn.TransformerDecoder for ActorVae) and
+// ActorVae's torch nn.TransformerEncoder (actor_vae.py:114-118, no final norm).
+// Returns the buffer holding the last layer's output (before the stack's final norm); the compact
+// [nseq * n_sel] rows when the last layer runs trimmed.
 static ActBuf run_stack(mldb_handle* h, const StackW& sw, ActBuf x0, ActBuf mem, StackWs& ws,
                         const SeqInfo& si, cudaStream_t st) {
+  if (sw.kind == STACK_PLAIN_ENC) {   // only the distribution tokens leave the stack (actor_vae.py:169)
+    ActBuf x = x0;
+    for (int i = 0; i + 1 < sw.layers; ++i) {
+      enc_layer(h, sw, sw.enc[i], x, ws.cur[i & 1], ws, si, st);
+      x = ws.cur[i & 1];
+    }
+    return enc_layer_selected(h, sw, sw.enc.back(), x, ws, si, st);
+  }
   if (sw.kind == STACK_PLAIN_DEC) {
     ActBuf x = x0;
     for (int i = 0; i < sw.layers; ++i) {
@@ -766,11 +808,7 @@ extern "C" int mldb_load_tensor(mldb_handle* h, const char* key, const void* dat
   if (dtype != MLDB_DTYPE_F32) FAIL(MLDB_ERR_UNSUPPORTED, "only fp32 tensors are accepted");
   if (h->finalized) FAIL(MLDB_ERR_STATE, "weights already finalized");
   auto it = h->raw.find(key);
-  if (it == h->raw.end()) {
-    // ActorVae's encoder half is not on the sampling path: accept and ignore
-    if (h->cfg.vae_kind == MLDB_VAE_ACTOR && !strncmp(key, "vae.encoder.", 12)) return MLDB_OK;
-    FAIL(MLDB_ERR_INVALID, "unexpected state-dict key '%s'", key);
-  }
+  if (it == h->raw.end()) FAIL(MLDB_ERR_INVALID, "unexpected state-dict key '%s'", key);
   RawTensor& t = it->second;
   if ((int)t.shape.size() != ndim) FAIL(MLDB_ERR_INVALID, "key '%s': rank %d, expected %d", key, ndim, (int)t.shape.size());
   size_t n = 1;
@@ -999,10 +1037,18 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
   (void)stream;
   if (!h) FAIL(MLDB_ERR_INVALID, "null handle");
   if (h->finalized) FAIL(MLDB_ERR_STATE, "already finalized");
-  for (auto& kv : h->raw)
-    if (!kv.second.loaded) FAIL(MLDB_ERR_STATE, "missing state-dict key '%s' (strict load)", kv.first.c_str());
-  DeviceGuard guard(h->device);
   const mldb_config& c = h->cfg;
+  // ActorVae's encoder keys are all or none: a decoder-only state dict samples and decodes (mldb_vae_encode then
+  // refuses), a partial encoder is an incomplete load
+  const std::string AE = "vae.encoder.";
+  auto is_actor_enc = [&](const std::string& k) { return c.vae_kind == MLDB_VAE_ACTOR && !k.compare(0, AE.size(), AE); };
+  bool actor_enc = false;
+  for (auto& kv : h->raw)
+    if (is_actor_enc(kv.first) && kv.second.loaded) actor_enc = true;
+  for (auto& kv : h->raw)
+    if (!kv.second.loaded && (actor_enc || !is_actor_enc(kv.first)))
+      FAIL(MLDB_ERR_STATE, "missing state-dict key '%s' (strict load)", kv.first.c_str());
+  DeviceGuard guard(h->device);
   const int d = c.latent_dim;
   const std::string D = "denoiser.", V = "vae.";
   if (c.num_layers > 0) {
@@ -1035,7 +1081,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
     TRY(pack_skip_stack(h, V + "encoder.", d, c.vae_ff, c.vae_heads, c.vae_layers, false, &h->venc));
     TRY(pack_skip_stack(h, V + "decoder.", d, c.vae_ff, c.vae_heads, c.vae_layers, true, &h->vdec));
     TRY(upload_pe(h, V + "query_pos_decoder.pe", &h->vae_dec_pe, &h->vae_dec_pe_rows));
-    TRY(upload_pe(h, V + "query_pos_encoder.pe", &h->vae_enc_pe));
+    TRY(upload_pe(h, V + "query_pos_encoder.pe", &h->vae_enc_pe, &h->vae_enc_pe_rows));
     TRY(upload_f32(h, rt(h, V + "global_motion_token").host.data(), (size_t)2 * c.n_lat * d, &h->global_token));
     TRY(pack_named(h, V + "skel_embedding.weight", V + "skel_embedding.bias", &h->skel_emb, 0, -1, true));
     TRY(pack_named(h, V + "final_layer.weight", V + "final_layer.bias", &h->final_layer));
@@ -1048,6 +1094,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
     }
     TRY(upload_pe(h, V + "decoder.sequence_pos_encoding.pe", &h->vae_dec_pe, &h->vae_dec_pe_rows));
     TRY(pack_named(h, V + "decoder.final_layer.weight", V + "decoder.final_layer.bias", &h->final_layer));
+    if (actor_enc) TRY(pack_actor_encoder(h));
   }
   if (h->text.on) TRY(pack_text(h));
   if (h->t2m.on) TRY(pack_t2m(h));
@@ -1666,6 +1713,11 @@ extern "C" int mldb_vae_decode(mldb_handle* h, const float* z, const int32_t* le
 }
 
 // ----------------------------------------------------------------------------- VAE encode
+// the first n elements of a split16 buffer whose rows are contiguous (cols == leading dimension), widened to fp32
+__global__ void k_split_to_f32(ActBuf X, float* __restrict__ out, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = join_f32(X.hi[i], X.lo()[i]);
+}
 __global__ void k_rows_out_permuted(const float* __restrict__ src, float* __restrict__ mu, float* __restrict__ logvar,
                                     int B, int n_lat, int d) {
   // src rows (b, j) j < 2*n_lat -> mu[j, b, :] (j < n_lat) / logvar[j - n_lat, b, :]
@@ -1684,14 +1736,20 @@ extern "C" int mldb_vae_encode(mldb_handle* h, const float* feats, const int32_t
   DeviceGuard guard(h->device);
   if (!feats || !lengths || !mu || !logvar || B <= 0 || T <= 0) FAIL(MLDB_ERR_INVALID, "bad argument");
   const mldb_config& c = h->cfg;
-  if (c.vae_kind != MLDB_VAE_MLD) FAIL(MLDB_ERR_UNSUPPORTED, "encode is built for MldVae only");
+  const bool actor = c.vae_kind == MLDB_VAE_ACTOR;
+  if (c.vae_kind != MLDB_VAE_MLD && !actor) FAIL(MLDB_ERR_UNSUPPORTED, "encode needs a VAE (MldVae or ActorVae)");
+  if (actor && h->venc.enc.empty())
+    FAIL(MLDB_ERR_STATE, "the ActorVae encoder was not loaded: the state dict held no 'vae.encoder.*' keys");
+  if (actor && c.n_lat != 1) FAIL(MLDB_ERR_UNSUPPORTED, "the ActorVae encoder yields one latent token, not n_lat = %d", c.n_lat);
   cudaStream_t st = (cudaStream_t)stream;
   const int d = c.latent_dim, G = 2 * c.n_lat, L = G + T;
-  if (L > 500) FAIL(MLDB_ERR_INVALID, "sequence too long for the learned PE table");
+  if (L > h->vae_enc_pe_rows)
+    FAIL(MLDB_ERR_INVALID, "T + %d = %d tokens exceed the encoder's positional table (%d rows)", G, L, h->vae_enc_pe_rows);
   Plan* p = find_plan(h, 2, B, 0, T);
   if (!p) {
     p = add_plan(h, 2, B, 0, T);
-    TRY(alloc_stack_ws(h, h->venc, B, L, 0, &p->ws, h->venc.layers >= 3 ? G : 0));
+    // the last layer runs trimmed to the G distribution rows (ActorVae: always; MldVae: when it has skip blocks)
+    TRY(alloc_stack_ws(h, h->venc, B, L, 0, &p->ws, actor || h->venc.layers >= 3 ? G : 0));
     TRY(dev_alloc(h, (void**)&p->lengths, (size_t)B * sizeof(int32_t)));
     TRY(dev_alloc(h, (void**)&p->stage_f32, (size_t)B * G * d * sizeof(float)));
     if (h->skel_emb.K % 64 == 0) TRY(alloc_act(h, B * T, h->skel_emb.K, &p->in_split));
@@ -1709,11 +1767,19 @@ extern "C" int mldb_vae_encode(mldb_handle* h, const float* feats, const int32_t
     g.a_kind = A_F32; g.a_f32 = feats; g.lda = c.vae_nfeats;
   }
   op_gemm(h, g, st);
-  // global motion tokens (b, 0..G-1) = token + PE (mld_vae.py:146,157)
+  // global motion tokens (b, 0..G-1) = token + PE (mld_vae.py:146,157; actor_vae.py:144-165)
   k_rows_to_split<<<nblk((int64_t)B * G * d), 256, 0, st>>>(p->ws.x0, h->global_token, d, B * G, d, G, L, 0, 1, h->vae_enc_pe);
   kcount(h, MLDB_KSTAT_MISC);
   SeqInfo si; si.lengths = p->lengths; si.kv_prefix = G;
   ActBuf x = run_stack(h, h->venc, p->ws.x0, ActBuf{}, p->ws, si, st);
+  if (actor) {   // no final norm: the trimmed layer's (b, mu | logvar) rows are the distribution (actor_vae.py:169)
+    k_split_to_f32<<<nblk((int64_t)B * G * d), 256, 0, st>>>(x, p->stage_f32, (int64_t)B * G * d);
+    kcount(h, MLDB_KSTAT_MISC);
+    k_rows_out_permuted<<<nblk((int64_t)B * G * d), 256, 0, st>>>(p->stage_f32, mu, logvar, B, 1, d);
+    kcount(h, MLDB_KSTAT_MISC);
+    CK(cudaGetLastError());
+    return check_ops(h);
+  }
   LnArgs l; l.res = x; l.gamma = h->venc.norm.g; l.beta = h->venc.norm.b; l.M = B * G; l.d = d;
   if (p->ws.n_sel == 0) { l.sel_group = G; l.in_group = L; }
   l.out_f32 = p->stage_f32; l.ld_out = d;
@@ -2236,10 +2302,6 @@ extern "C" int mldb_t2m_text(mldb_handle* h, const float* word_embs, const float
 //   A [M,K] fp32 device; W [N,K], bias [N], gamma/beta [N] fp32 HOST (gamma == NULL: no LN);
 //   R [M,N] fp32 device or NULL; K1 < K splits A into two concatenated sources (skip connection);
 //   out [M,N] fp32 device.  use_tc: 1 tensor-core path, 0 CUDA-core path.  Synchronous.
-__global__ void k_split_to_f32(ActBuf X, float* __restrict__ out, int64_t n) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = join_f32(X.hi[i], X.lo()[i]);
-}
 extern "C" int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float* bias,
                                const float* gamma, const float* beta, const float* R, int32_t M, int32_t N,
                                int32_t K, int32_t K1, int32_t act, int32_t use_tc, int32_t split_out, float* out,

@@ -22,11 +22,13 @@ struct DecW {  // TransformerDecoderLayer (cross_attention.py:297-321)
   LinW sa_in, sa_out, ca_q, ca_kv, ca_v, ca_out, l1, l2;   // ca_v: rows [2d,3d) for the 1-memory-token collapse
   LnW n1, n2, n3;
 };
-enum StackKind { STACK_SKIP_ENC = 0, STACK_SKIP_DEC = 1, STACK_PLAIN_DEC = 2 };
+// STACK_PLAIN_ENC: torch nn.TransformerEncoder without a final norm (ActorVae's encoder); its last layer always
+// runs trimmed to the n_sel distribution rows
+enum StackKind { STACK_SKIP_ENC = 0, STACK_SKIP_DEC = 1, STACK_PLAIN_DEC = 2, STACK_PLAIN_ENC = 3 };
 struct StackW {
   int kind = STACK_SKIP_ENC;
   int d = 0, ff = 0, heads = 0, layers = 0;
-  std::vector<EncW> enc;   // input blocks, middle, output blocks (in execution order)
+  std::vector<EncW> enc;   // input blocks, middle, output blocks (in execution order); plain: layers in order
   std::vector<DecW> dec;
   std::vector<LinW> skip;  // linear_blocks (Linear(2d -> d))
   LnW norm;                // final norm (g == nullptr: none, ActorVae)
@@ -142,8 +144,9 @@ struct mldb_handle {
   float* mem_pe = nullptr;           // denoiser mem_pos.pe [500, d]
   float* vae_dec_pe = nullptr;       // [500 | 5000, d]
   int vae_dec_pe_rows = 0;
-  float* vae_enc_pe = nullptr;
-  float* global_token = nullptr;     // [2*n_lat, d]
+  float* vae_enc_pe = nullptr;       // MldVae [500, d] | ActorVae [5000, d]
+  int vae_enc_pe_rows = 0;
+  float* global_token = nullptr;     // [2*n_lat, d]; ActorVae: [mu_token; logvar_token]
   float* mean = nullptr; float* stdv = nullptr; int nstat = 0;
   TextW text;          // CLIP text tower (mldb_text_configure)
   T2mW t2m;            // T2M evaluator (mldb_t2m_configure)

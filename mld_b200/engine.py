@@ -364,13 +364,15 @@ class Engine:
         return out
 
     def vae_encode(self, feats: torch.Tensor, lengths):
+        """feats [B, T, vae_nfeats] -> (mu, logvar), each [n_lat, B, d] (MldVae) or [1, B, d] (ActorVae)."""
         f = _f32c(feats, self.device)
         ln = self._lengths(lengths)
         if f.dim() != 3 or f.shape[2] != self.cfg.vae_nfeats:
             raise ValueError(f"feats must be [B, T, {self.cfg.vae_nfeats}], got {tuple(f.shape)}")
         B, T = f.shape[0], f.shape[1]
         self._check_lengths(ln, B)
-        shape = (self.cfg.n_lat, B, self.cfg.latent_dim)
+        n_tok = 1 if self.cfg.vae_kind == _lib.VAE_ACTOR else self.cfg.n_lat
+        shape = (n_tok, B, self.cfg.latent_dim)
         mu = torch.empty(shape, dtype=torch.float32, device=self.device)
         logvar = torch.empty(shape, dtype=torch.float32, device=self.device)
         check(self.lib.mldb_vae_encode(self._h, _ptr(f), _ptr(ln), B, T, _ptr(mu), _ptr(logvar),

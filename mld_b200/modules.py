@@ -154,13 +154,15 @@ class B200MldVae(_EngineModule):
 
 
 class B200ActorVae(_EngineModule):
-    """``ActorVae`` decode path (mld/models/architectures/actor_vae.py:11-235)."""
+    """``ActorVae`` (mld/models/architectures/actor_vae.py:11-235).  A state dict without the ``encoder.*`` keys
+    still decodes; ``encode`` then raises."""
     _prefix = "vae."
 
     def __init__(self, ablation, nfeats: int, latent_dim: list = [1, 256], ff_size: int = 1024,
                  num_layers: int = 9, num_heads: int = 4, dropout: float = 0.1, is_vae: bool = True,
                  activation: str = "gelu", position_embedding: str = "learned", **kwargs) -> None:
         super().__init__()
+        self.is_vae = is_vae
         self.latent_size, self.latent_dim = latent_dim[0], latent_dim[-1]
         self._kw = dict(latent_dim=tuple(latent_dim), vae_ff=ff_size, vae_layers=num_layers,
                         vae_heads=num_heads, vae_nfeats=nfeats, nfeats=nfeats)
@@ -173,5 +175,21 @@ class B200ActorVae(_EngineModule):
     def decode(self, z: torch.Tensor, lengths: List[int]):
         return self.engine().vae_decode(z, lengths)
 
-    def encode(self, features, lengths=None):
-        raise NotImplementedError("ActorVae.encode is not on the sampling path (SURVEY.md section 8)")
+    def encode(self, features: torch.Tensor, lengths: Optional[List[int]] = None):
+        """(z [1, B, d], dist) with ``dist.loc`` / ``dist.scale`` [B, d] (actor_vae.py:62-75,120-170)."""
+        if not self.is_vae:
+            # the reference fails here too: its encoder always returns a Normal, which has no unsqueeze (:72)
+            raise NotImplementedError("B200ActorVae implements is_vae=True only")
+        if lengths is None:
+            lengths = [len(f) for f in features]
+        mu, logvar = self.engine().vae_encode(features, lengths)
+        dist = torch.distributions.Normal(mu[0], logvar[0].exp().pow(0.5))    # :169-172
+        z = dist.loc + 1.0 * (dist.rsample() - dist.loc)                       # sample_from_distribution, fact 1.0
+        return z.unsqueeze(0), dist
+
+    def forward(self, features: torch.Tensor, lengths: Optional[List[int]] = None):
+        print("Should Not enter here")                                         # actor_vae.py:58
+        if lengths is None:
+            lengths = [len(f) for f in features]
+        z, dist = self.encode(features, lengths)
+        return self.decode(z, lengths), z, dist
