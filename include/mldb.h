@@ -268,6 +268,18 @@ int mldb_debug_ffn(mldb_handle* h, const float* X, const float* W1, const float*
                    const float* b2, const float* gamma, const float* beta, int32_t M, int32_t d, int32_t ff,
                    int32_t mode, float* out, void* stream);
 
+/* Debug aid: an encoder layer after its attention, as the stacks run it:
+ *   x1 = LayerNorm1(att Wo^T + bo + X),  out = LayerNorm2(x1 + W2 gelu(W1 x1 + b1) + b2)
+ * att, X: [M, d] fp32 DEVICE; the weights HOST ([d,d], [ff,d], [d,ff]; biases nullable).  out: [out_rows, d] fp32
+ * DEVICE, out_rows >= M: rows >= M go into the output buffer's rows past M before the op and are read back after it
+ * (an op must leave them as they were).  mode 0 = CUDA cores, 1 = the two wgmma kernels (out-projection + LN GEMM,
+ * then the fused FFN), 2 = one fused launch (the fused FFN with its out-projection prefix; d = 256).  Synchronous
+ * on `stream`. */
+int mldb_debug_tail(mldb_handle* h, const float* att, const float* X, const float* Wo, const float* bo,
+                    const float* gamma1, const float* beta1, const float* W1, const float* b1, const float* W2,
+                    const float* b2, const float* gamma2, const float* beta2, int32_t M, int32_t d, int32_t ff,
+                    int32_t mode, int32_t out_rows, float* out, void* stream);
+
 /* Debug aid: the multi-head attention core softmax(Q K^T / sqrt(hd)) V per (sequence, head).
  *   KV == NULL: Q is a packed QKV [nseq*Lq, 3*heads*hd] fp32 DEVICE tensor (q | k | v column blocks, torch
  *               in_proj order; self-attention, Lk == Lq) - the layout the denoiser / VAE stacks use;
@@ -372,7 +384,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
  * (and the tests) assert that nothing fell back from the wgmma kernels to the CUDA-core kernels. */
 #define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue; k_proj_tc (its K = 256 split16 projections) */
 #define MLDB_KSTAT_GEMM_LN_TC 1   /* k_gemm_tc, fused residual + LayerNorm epilogue */
-#define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block) */
+#define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block; in the encoder layers it also runs the folded
+                                     out-projection + residual + LayerNorm in front of the FFN) */
 #define MLDB_KSTAT_ATTN_TC 3      /* k_attn_tc (wgmma attention) */
 #define MLDB_KSTAT_ATTN_MMA 4     /* k_attn_mma (mma.sync attention; option attn=mma) */
 #define MLDB_KSTAT_ATTN_SIMT 5    /* k_attn_simt (CUDA cores) */

@@ -94,6 +94,7 @@ _SIGNATURES = {
     "mldb_debug_gemm": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_debug_ffn": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_debug_tail": (C.c_int, [_P] * 13 + [C.c_int32] * 5 + [_P, _P]),
     "mldb_debug_attention": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_int32, _P, _P]),
     "mldb_debug_attention_causal": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -450,18 +450,51 @@ static void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st) {
     kcount(h, MLDB_KSTAT_ATTN_SIMT);
   }
 }
+// which stream's scratch / flags the fused FFN uses (branches run concurrently, each on its own pair)
+static int ffn_scratch_slot(const mldb_handle* h, cudaStream_t st) {
+  int k = 0;
+  for (int i = 0; i < mldb_handle::MAX_BRANCHES - 1; ++i) if (st == h->br_stream[i]) k = i + 1;
+  return k;
+}
 // the fused FFN block when the shape allows it, else the two GEMMs
 static void op_ffn(mldb_handle* h, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* cf32, cudaStream_t st) {
   if (h->use_tc && tc_ffn_supported(h->tc, g1, g2, l2)) {
     // one launch: the hidden activations stay in registers (gemm_tc.cu k_ffn_tc)
-    int k = 0;                                     // which stream: its own scratch (branches run concurrently)
-    for (int i = 0; i < mldb_handle::MAX_BRANCHES - 1; ++i) if (st == h->br_stream[i]) k = i + 1;
+    const int k = ffn_scratch_slot(h, st);
     if (!tc_ffn(h->tc, g1, g2, l2, h->ffn_scratch[k], h->ffn_flags[k], st)) h->op_failed = true;
     kcount(h, MLDB_KSTAT_FFN_TC);
     return;
   }
   op_gemm(h, g1, st);
   op_gemm_ln(h, g2, l2, cf32, st);
+}
+// An encoder layer after its attention: x1 = LN1(att W_o^T + b_o + x), then the FFN block on x1 into xout (x1 and
+// hbuf are workspaces).  The fused launch (k_ffn_tc with its out-projection prefix, which keeps x1 in shared memory
+// and does not write it) runs for at most FUSE_MAX_TILES m-tiles; else (or with fuse == 0: mldb_debug_tail's
+// two-kernel arm) the out-projection + LN GEMM and op_ffn, which write x1.  Measured on H100: at 2 m-tiles (one
+// prompt) the saved launch and x1 round trip make the whole sample 8 % faster than the two launches; at 24 m-tiles
+// (action512) and at 158 (the headline's sub-batches) the fused launch is 4-10 % slower end to end.  Its x tile holds
+// att, then x1, then y until the y store has read it, so a tile's loads are not overlapped with the previous tile's
+// work, and every ffn_split piece repeats the out-projection.  fuse: 0 never, 1 the size rule, 2 whenever the kernel
+// takes the shape (mldb_debug_tail, profile_op "tail_fused").
+static void op_tail(mldb_handle* h, const LinW& wo, const LnW& n1, const LinW& l1, const LinW& l2, const LnW& n2,
+                    ActBuf att, ActBuf x, ActBuf x1, ActBuf hbuf, ActBuf xout, int M, int d, int ff, float* cf32,
+                    cudaStream_t st, int fuse = 1) {
+  GemmArgs go; go.a1 = att; go.K1 = d; go.M = M; go.w = wo;
+  LnArgs ln1; ln1.res = x; ln1.gamma = n1.g; ln1.beta = n1.b; ln1.M = M; ln1.d = d; ln1.out = x1;
+  GemmArgs g1; g1.a1 = x1; g1.K1 = d; g1.M = M; g1.w = l1; g1.act = ACT_GELU; g1.out = hbuf;
+  GemmArgs g2; g2.a1 = hbuf; g2.K1 = ff; g2.M = M; g2.w = l2;
+  LnArgs ln2; ln2.res = x1; ln2.gamma = n2.g; ln2.beta = n2.b; ln2.M = M; ln2.d = d; ln2.out = xout;
+  constexpr int FUSE_MAX_TILES = 2;
+  const bool small = (M + 127) / 128 <= FUSE_MAX_TILES;
+  if (fuse && (fuse == 2 || small) && h->use_tc && tc_tail_supported(h->tc, go, ln1, g1, g2, ln2)) {
+    const int k = ffn_scratch_slot(h, st);
+    if (!tc_tail(h->tc, go, ln1, g1, g2, ln2, h->ffn_scratch[k], h->ffn_flags[k], st)) h->op_failed = true;
+    kcount(h, MLDB_KSTAT_FFN_TC);
+    return;
+  }
+  op_gemm_ln(h, go, ln1, cf32, st);
+  op_ffn(h, g1, g2, ln2, cf32, st);
 }
 
 // ----------------------------------------------------------------------------- workspaces
@@ -541,9 +574,9 @@ static void out_proj_ln(mldb_handle* h, const LinW& w, const LnW& n, ActBuf att,
   LnArgs l; l.res = res; l.gamma = n.g; l.beta = n.b; l.M = M; l.d = d; l.out = xout;
   op_gemm_ln(h, g, l, cf32, st);
 }
-static void self_attn_block(mldb_handle* h, const LinW& in_proj, const LinW& out_proj, const LnW& n,
-                            ActBuf xin, ActBuf xout, StackWs& ws, const SeqInfo& si, int heads,
-                            cudaStream_t st) {
+// QKV projection + self-attention of xin -> ws.att
+static void self_attn(mldb_handle* h, const LinW& in_proj, ActBuf xin, StackWs& ws, const SeqInfo& si, int heads,
+                      cudaStream_t st) {
   const int d = ws.d;
   GemmArgs g; g.a1 = xin; g.K1 = d; g.M = ws.M; g.w = in_proj; g.out = ws.qkv;
   op_gemm(h, g, st);
@@ -551,7 +584,12 @@ static void self_attn_block(mldb_handle* h, const LinW& in_proj, const LinW& out
   a.Lk = ws.L; a.nseq = ws.nseq; a.heads = heads; a.hd = d / heads;
   a.lengths = si.lengths; a.kv_prefix = si.kv_prefix; a.len_mod = si.len_mod; a.seq0 = 0; a.out = ws.att;
   op_attn(h, a, st);
-  out_proj_ln(h, out_proj, n, ws.att, xin, xout, ws.M, d, ws.cf32, st);
+}
+static void self_attn_block(mldb_handle* h, const LinW& in_proj, const LinW& out_proj, const LnW& n,
+                            ActBuf xin, ActBuf xout, StackWs& ws, const SeqInfo& si, int heads,
+                            cudaStream_t st) {
+  self_attn(h, in_proj, xin, ws, si, heads, st);
+  out_proj_ln(h, out_proj, n, ws.att, xin, xout, ws.M, ws.d, ws.cf32, st);
 }
 static void ffn_block(mldb_handle* h, const LinW& l1, const LinW& l2, const LnW& n, ActBuf xin,
                       ActBuf xout, StackWs& ws, int act, cudaStream_t st) {
@@ -563,8 +601,8 @@ static void ffn_block(mldb_handle* h, const LinW& l1, const LinW& l2, const LnW&
 // TransformerEncoderLayer.forward_post (cross_attention.py:259-272)
 static void enc_layer(mldb_handle* h, const StackW& sw, const EncW& w, ActBuf xin, ActBuf xout,
                       StackWs& ws, const SeqInfo& si, cudaStream_t st) {
-  self_attn_block(h, w.in_proj, w.out_proj, w.n1, xin, ws.x1, ws, si, sw.heads, st);
-  ffn_block(h, w.l1, w.l2, w.n2, ws.x1, xout, ws, ACT_GELU, st);
+  self_attn(h, w.in_proj, xin, ws, si, sw.heads, st);
+  op_tail(h, w.out_proj, w.n1, w.l1, w.l2, w.n2, ws.att, xin, ws.x1, ws.h, xout, ws.M, ws.d, ws.ff, ws.cf32, st);
 }
 // TransformerDecoderLayer.forward_post (cross_attention.py:323-345)
 static void dec_layer(mldb_handle* h, const StackW& sw, const DecW& w, ActBuf xin, ActBuf xout,
@@ -634,11 +672,7 @@ static ActBuf enc_layer_selected(mldb_handle* h, const StackW& sw, const EncW& w
   a.Lk = ws.L; a.nseq = ws.nseq; a.heads = sw.heads; a.hd = d / sw.heads; a.lengths = si.lengths;
   a.kv_prefix = si.kv_prefix; a.len_mod = si.len_mod; a.out = ws.satt;
   op_attn(h, a, st);
-  out_proj_ln(h, w.out_proj, w.n1, ws.satt, ws.sx, ws.sx1, R, d, ws.cf32, st);
-  GemmArgs g1; g1.a1 = ws.sx1; g1.K1 = d; g1.M = R; g1.w = w.l1; g1.act = ACT_GELU; g1.out = ws.sh;
-  GemmArgs g2; g2.a1 = ws.sh; g2.K1 = ws.ff; g2.M = R; g2.w = w.l2;
-  LnArgs l2; l2.res = ws.sx1; l2.gamma = w.n2.g; l2.beta = w.n2.b; l2.M = R; l2.d = d; l2.out = ws.sout;
-  op_ffn(h, g1, g2, l2, ws.cf32, st);
+  op_tail(h, w.out_proj, w.n1, w.l1, w.l2, w.n2, ws.satt, ws.sx, ws.sx1, ws.sh, ws.sout, R, d, ws.ff, ws.cf32, st);
   return ws.sout;
 }
 
@@ -1914,7 +1948,10 @@ extern "C" int mldb_sample_host(mldb_handle* h, const void* cond_host, const flo
 // ----------------------------------------------------------------------------- profiling aid
 // Time one operator of denoiser layer 0 in isolation on the real workspace of the (B, S_ctx)
 // reverse plan: `iters` back-to-back launches bracketed by CUDA events on `stream`.
-// op: "qkv" | "attn" | "outproj_ln" | "ffn1" | "ffn2_ln" | "layer".  avg_ms_out: HOST float.
+// op: "qkv" | "attn" | "outproj_ln" | "ffn1" | "ffn2_ln" | "ffn" | "tail" | "tail_fused" | "layer".  "outproj_ln" and
+// "ffn" time the standalone kernels; "tail" is both as the encoder layer runs them (op_tail), "tail_fused" the fused
+// launch at any row count.
+// avg_ms_out: HOST float.
 extern "C" int mldb_profile_op(mldb_handle* h, const char* op, int32_t B, int32_t S_ctx, int32_t iters,
                                float* avg_ms_out) {
   TRY(check_ready(h, false));
@@ -1946,6 +1983,10 @@ extern "C" int mldb_profile_op(mldb_handle* h, const char* op, int32_t B, int32_
       op_gemm_ln(h, g, l, ws.cf32, st);
     } else if (!strcmp(op, "ffn")) {             // FFN1 + FFN2 the way the stack runs them (pair mode or not)
       ffn_block(h, w.l1, w.l2, w.n2, ws.x1, ws.cur[0], ws, ACT_GELU, st);
+    } else if (!strcmp(op, "tail")) {            // out-projection + LN1 + FFN + LN2 the way the stack runs them
+      op_tail(h, w.out_proj, w.n1, w.l1, w.l2, w.n2, ws.att, ws.x0, ws.x1, ws.h, ws.cur[0], ws.M, d, ws.ff, ws.cf32, st);
+    } else if (!strcmp(op, "tail_fused")) {      // the same with the fused launch whatever the row count
+      op_tail(h, w.out_proj, w.n1, w.l1, w.l2, w.n2, ws.att, ws.x0, ws.x1, ws.h, ws.cur[0], ws.M, d, ws.ff, ws.cf32, st, 2);
     } else if (!strcmp(op, "layer")) {
       enc_layer(h, h->den, w, ws.x0, ws.cur[0], ws, si, st);
     } else {
@@ -2391,6 +2432,50 @@ extern "C" int mldb_debug_ffn(mldb_handle* h, const float* X, const float* W1, c
   if (e == cudaSuccess) e = cudaGetLastError();
   while (h->allocs.size() > n_alloc0) { cudaFree(h->allocs.back()); h->allocs.pop_back(); }
   if (e != cudaSuccess) FAIL(MLDB_ERR_CUDA, "debug ffn: %s", cudaGetErrorString(e));
+  return MLDB_OK;
+}
+
+extern "C" int mldb_debug_tail(mldb_handle* h, const float* att, const float* X, const float* Wo, const float* bo,
+                               const float* gamma1, const float* beta1, const float* W1, const float* b1,
+                               const float* W2, const float* b2, const float* gamma2, const float* beta2, int32_t M,
+                               int32_t d, int32_t ff, int32_t mode, int32_t out_rows, float* out, void* stream) {
+  if (!h || !att || !X || !Wo || !gamma1 || !beta1 || !W1 || !W2 || !gamma2 || !beta2 || !out || M <= 0 || d <= 0 ||
+      ff <= 0 || out_rows < M)
+    FAIL(MLDB_ERR_INVALID, "bad argument");
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t n_alloc0 = h->allocs.size();
+  LinW wo, l1, l2;
+  LnW n1, n2;
+  TRY(pack_linear(h, Wo, d, d, bo, &wo));
+  TRY(pack_linear(h, W1, ff, d, b1, &l1));
+  TRY(pack_linear(h, W2, d, ff, b2, &l2));
+  TRY(upload_f32(h, gamma1, d, &n1.g));
+  TRY(upload_f32(h, beta1, d, &n1.b));
+  TRY(upload_f32(h, gamma2, d, &n2.g));
+  TRY(upload_f32(h, beta2, d, &n2.b));
+  ActBuf a, x, x1, hb, o;
+  float* cf32 = nullptr;
+  TRY(alloc_act(h, M, d, &a));
+  TRY(alloc_act(h, M, d, &x));
+  TRY(alloc_act(h, M, d, &x1));
+  TRY(alloc_act(h, M, ff, &hb));
+  TRY(alloc_act(h, out_rows, d, &o));
+  TRY(dev_alloc(h, (void**)&cf32, (size_t)M * d * sizeof(float)));
+  k_rows_to_split<<<nblk((int64_t)out_rows * d), 256, 0, st>>>(o, out, d, out_rows, d, 1 << 30, 0, 0, 0, nullptr);
+  k_rows_to_split<<<nblk((int64_t)M * d), 256, 0, st>>>(a, att, d, M, d, 1 << 30, 0, 0, 0, nullptr);
+  k_rows_to_split<<<nblk((int64_t)M * d), 256, 0, st>>>(x, X, d, M, d, 1 << 30, 0, 0, 0, nullptr);
+  const bool saved = h->use_tc;
+  h->use_tc = mode != 0;
+  const int saved_fused = tc_set_ffn_fused(h->tc, 1);
+  op_tail(h, wo, n1, l1, l2, n2, a, x, x1, hb, o, M, d, ff, cf32, st, mode == 2 ? 2 : 0);
+  h->use_tc = saved;
+  tc_set_ffn_fused(h->tc, saved_fused);
+  k_split_to_f32<<<nblk((int64_t)out_rows * d), 256, 0, st>>>(o, out, (int64_t)out_rows * d);
+  cudaError_t e = cudaStreamSynchronize(st);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  while (h->allocs.size() > n_alloc0) { cudaFree(h->allocs.back()); h->allocs.pop_back(); }
+  if (e != cudaSuccess) FAIL(MLDB_ERR_CUDA, "debug tail: %s", cudaGetErrorString(e));
   return MLDB_OK;
 }
 

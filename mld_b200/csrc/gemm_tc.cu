@@ -115,36 +115,24 @@ __device__ __forceinline__ void ring_produce(int& q_next, int total, int need, c
 }
 
 // y = LayerNorm(acc * sc + bias + residual) * gamma + beta over the 256-wide rows of a [64 x 256] accumulator
-// fragment, eps 1e-5.  r_lo: this thread's first row (the second is r_lo + 8), cp: its column offset inside an
-// 8-column group.  The statistics are two exact passes over the registers; a row's four lanes are merged with
-// shuffles in a fixed order, so the result does not depend on which CTA ran the tile.
-__device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const float* bias, const __half* res_hi,
-                                            const __half* res_lo, int ld_res, const float* gamma, const float* beta,
-                                            __half* out_hi, __half* out_lo, int ld_out, int r_lo, int M, int cp) {
-  const bool ok0 = r_lo < M, ok1 = r_lo + 8 < M;
+// fragment, eps 1e-5.  cp: this thread's column offset inside an 8-column group.  The residual and the output go
+// through the caller: res(j, x) adds the residual of 8-column group j to x[0..1] (first row) and x[2..3] (second
+// row); out(j, y) stores group j's normalised values in the same layout.  The statistics are two exact passes over
+// the registers; a row's four lanes are merged with shuffles in a fixed order, so the result does not depend on
+// which CTA ran the tile, nor on where the residual came from.
+template <class Res, class Out>
+__device__ __forceinline__ void ln_rows(float (&d)[128], float sc, const float* bias, const float* gamma,
+                                        const float* beta, int cp, Res&& res, Out&& out) {
   float s0 = 0.0f, s1 = 0.0f;
 #pragma unroll
   for (int j = 0; j < 32; ++j) {
     const int n = 8 * j + cp;
     const float2 b = bias ? __ldg(reinterpret_cast<const float2*>(bias + n)) : make_float2(0.0f, 0.0f);
-    float x0 = fmaf(d[4 * j], sc, b.x), x1 = fmaf(d[4 * j + 1], sc, b.y);
-    float x2 = fmaf(d[4 * j + 2], sc, b.x), x3 = fmaf(d[4 * j + 3], sc, b.y);
-    if (res_hi) {
-      if (ok0) {
-        const int64_t o = (int64_t)r_lo * ld_res + n;
-        const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
-        const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
-        x0 = (x0 + h.x) + l.x; x1 = (x1 + h.y) + l.y;
-      }
-      if (ok1) {
-        const int64_t o = (int64_t)(r_lo + 8) * ld_res + n;
-        const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
-        const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
-        x2 = (x2 + h.x) + l.x; x3 = (x3 + h.y) + l.y;
-      }
-    }
-    d[4 * j] = x0; d[4 * j + 1] = x1; d[4 * j + 2] = x2; d[4 * j + 3] = x3;
-    s0 += x0 + x1; s1 += x2 + x3;
+    float x[4] = {fmaf(d[4 * j], sc, b.x), fmaf(d[4 * j + 1], sc, b.y), fmaf(d[4 * j + 2], sc, b.x),
+                  fmaf(d[4 * j + 3], sc, b.y)};
+    res(j, x);
+    d[4 * j] = x[0]; d[4 * j + 1] = x[1]; d[4 * j + 2] = x[2]; d[4 * j + 3] = x[3];
+    s0 += x[0] + x[1]; s1 += x[2] + x[3];
   }
   const float mean0 = quad_sum(s0) * (1.0f / 256), mean1 = quad_sum(s1) * (1.0f / 256);
   float q0 = 0.0f, q1 = 0.0f;
@@ -160,13 +148,70 @@ __device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const flo
   for (int j = 0; j < 32; ++j) {
     const int n = 8 * j + cp;
     const float2 g = __ldg(reinterpret_cast<const float2*>(gamma + n)), be = __ldg(reinterpret_cast<const float2*>(beta + n));
-    if (ok0)
-      store_split2(out_hi, out_lo, (int64_t)r_lo * ld_out + n, fmaf(d[4 * j] * rstd0, g.x, be.x),
-                   fmaf(d[4 * j + 1] * rstd0, g.y, be.y));
-    if (ok1)
-      store_split2(out_hi, out_lo, (int64_t)(r_lo + 8) * ld_out + n, fmaf(d[4 * j + 2] * rstd1, g.x, be.x),
-                   fmaf(d[4 * j + 3] * rstd1, g.y, be.y));
+    const float y[4] = {fmaf(d[4 * j] * rstd0, g.x, be.x), fmaf(d[4 * j + 1] * rstd0, g.y, be.y),
+                        fmaf(d[4 * j + 2] * rstd1, g.x, be.x), fmaf(d[4 * j + 3] * rstd1, g.y, be.y)};
+    out(j, y);
   }
+}
+
+// ln_rows with the residual read from and the output written to split16 planes in global memory (k_gemm_tc).
+// r_lo: this thread's first row (the second is r_lo + 8); rows >= M are neither read nor written.
+__device__ __forceinline__ void ln_epilogue(float (&d)[128], float sc, const float* bias, const __half* res_hi,
+                                            const __half* res_lo, int ld_res, const float* gamma, const float* beta,
+                                            __half* out_hi, __half* out_lo, int ld_out, int r_lo, int M, int cp) {
+  const bool ok0 = r_lo < M, ok1 = r_lo + 8 < M;
+  ln_rows(d, sc, bias, gamma, beta, cp,
+          [&](int j, float (&x)[4]) {
+            if (!res_hi) return;
+            const int n = 8 * j + cp;
+            if (ok0) {
+              const int64_t o = (int64_t)r_lo * ld_res + n;
+              const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
+              const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
+              x[0] = (x[0] + h.x) + l.x; x[1] = (x[1] + h.y) + l.y;
+            }
+            if (ok1) {
+              const int64_t o = (int64_t)(r_lo + 8) * ld_res + n;
+              const float2 h = __half22float2(*reinterpret_cast<const __half2*>(res_hi + o));
+              const float2 l = __half22float2(*reinterpret_cast<const __half2*>(res_lo + o));
+              x[2] = (x[2] + h.x) + l.x; x[3] = (x[3] + h.y) + l.y;
+            }
+          },
+          [&](int j, const float (&y)[4]) {
+            const int n = 8 * j + cp;
+            if (ok0) store_split2(out_hi, out_lo, (int64_t)r_lo * ld_out + n, y[0], y[1]);
+            if (ok1) store_split2(out_hi, out_lo, (int64_t)(r_lo + 8) * ld_out + n, y[2], y[3]);
+          });
+}
+
+// ln_rows in place on a [128 x 256] split16 tile in shared memory, laid out as TMA writes it with 128B swizzle:
+// [plane][k-block][row][128 B], 16-byte chunk c of row r at chunk c ^ (r & 7).  The residual is read from the tile
+// and the result written back over it; every thread touches only its own elements (rows rl, rl + 8 of the tile,
+// rl & 7 = lane / 4), and a warp's accesses of one group fall in 8 distinct 16-byte chunks: no bank conflicts.
+__device__ __forceinline__ void ln_tile(float (&d)[128], float sc, const float* bias, const float* gamma,
+                                        const float* beta, uint8_t* tile, int rl, int lane, int cp) {
+  uint8_t* const row0 = tile + rl * 128 + cp * 2;
+  const int sw = lane >> 2;
+  auto at = [&](int j, int h, int plane) {
+    return reinterpret_cast<__half2*>(row0 + plane * 65536 + h * 1024 + (j >> 3) * 16384 + (((j & 7) ^ sw) << 4));
+  };
+  ln_rows(d, sc, bias, gamma, beta, cp,
+          [&](int j, float (&x)[4]) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const float2 hi = __half22float2(*at(j, h, 0)), lo = __half22float2(*at(j, h, 1));
+              x[2 * h] = (x[2 * h] + hi.x) + lo.x; x[2 * h + 1] = (x[2 * h + 1] + hi.y) + lo.y;
+            }
+          },
+          [&](int j, const float (&y)[4]) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint32_t hi, lo;
+              split2(y[2 * h], y[2 * h + 1], hi, lo);
+              *reinterpret_cast<uint32_t*>(at(j, h, 0)) = hi;
+              *reinterpret_cast<uint32_t*>(at(j, h, 1)) = lo;
+            }
+          });
 }
 
 // ------------------------------------------------------------------------------ the kernel
@@ -367,7 +412,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
 }
 
 // ------------------------------------------------------------------------------ fused FFN
-// y = LayerNorm(res + W2 gelu(W1 x + b1) + b2) for d = 256 as ONE persistent launch in which the
+// y = LayerNorm(x + W2 gelu(W1 x + b1) + b2) for d = 256 as ONE persistent launch in which the
 // hidden activations never leave the register file (the unfused pair writes and re-reads 2 x 4 x ff
 // bytes per row through HBM, which is what bounds it).  A CTA owns 128-row m-tiles, 64 rows per
 // consumer warpgroup; the x tile (both planes, 128 KB) stays in shared memory while the warpgroup
@@ -376,9 +421,17 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
 //   E1(c): acc1 -> *s1 + b1 -> GELU -> split16 A fragments (the accumulator layout of 16 columns IS the
 //          register-operand layout of a 16-deep k-step, so the hidden chunk never touches shared memory)
 //   F2(c): acc2[64 x 256] += H[64 x 64] . W2[:, c*64..]^T                  (A from registers)
-// and finishes with the residual + LayerNorm epilogue on acc2.  W1 / W2 stream through a ring of three 32 KB
-// slots, four per chunk: W1 k-blocks 0-1, W1 k-blocks 2-3, W2 hi plane, W2 lo plane.  F2(c)'s last group stays in
-// flight under F1(c + 1); the other warpgroup's MMAs cover this one's GELU.
+// and finishes with the residual + LayerNorm epilogue on acc2: the residual is x, read from the x tile, and y is
+// written over it and leaves through one TMA store per warpgroup (64 rows, rows >= M clipped by the tensor map).
+// With FfnParams::prefix (tc_tail) the tile first holds the attention output `att` and the item begins with the
+// block's out-projection + residual + LayerNorm, so that x1 = LN1(att W_o^T + b_o + x) is produced in the x tile:
+//   P(kb): acc2 = sum over k-blocks kb of att . W_o^T   (kblock_ss<256> over k-blocks 0..3: k_gemm_tc<256, EPI_LN>'s
+//          order, so x1 has the bits of the two-kernel path)
+//   once att k-block kb has been read by both warpgroups, k-block kb of the layer input x is loaded over it;
+//   LN1:   acc2 * s0 + b_o + x -> LayerNorm -> x1 (split16, in place in the x tile), then the FFN as above.
+// W_o, W1 and W2 stream through a ring of three 32 KB slots: eight positions per item for W_o (k-block kb's hi /
+// lo plane at 2 kb / 2 kb + 1), then four per chunk: W1 k-blocks 0-1, W1 k-blocks 2-3, W2 hi plane, W2 lo plane.
+// F2(c)'s last group stays in flight under F1(c + 1); the other warpgroup's MMAs cover this one's GELU.
 // CTA = the two MMA warpgroups only, 256 threads, one CTA per SM.  ptxas compiles a kernel under 65536 / (threads
 // rounded up to whole warpgroups) registers per thread whatever setmaxnreg does at run time: 168 with a third
 // (producer) warpgroup, which this body (~208) does not fit - it spilled and had its wgmma serialised - and 255
@@ -391,11 +444,11 @@ struct FfnParams {
   float* scratch;              // [slot][128 rows][256] fp32 partial accumulators of the pieces
   int* flags;                  // [slot] 1 = partial written (reset by the reader)
   int reverse;                 // walk the tiles from the last one down (snake order, see tc_attention)
+  int prefix;                  // 1: every item (each piece too) starts with the out-projection + LN1 (tc_tail)
   long long* tl;
-  float inv_s1, inv_s2;
+  float inv_s0, inv_s1, inv_s2;
+  const float* b0; const float* gamma1; const float* beta1;   // the prefix's out-projection bias and LayerNorm
   const float* b1; const float* b2; const float* gamma; const float* beta;
-  const __half* res_hi; const __half* res_lo; int ld_res;
-  __half* out_hi; __half* out_lo; int ld_out;
 };
 struct FfnCfg {
   static constexpr int CHUNK = 64;                       // hidden columns per chunk
@@ -405,10 +458,15 @@ struct FfnCfg {
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
+// tmX: the FFN input x (with the prefix: the layer input, LN1's residual); tmA / tmWo: the attention output and
+// W_o (read with the prefix only); tmY: the output planes, 64-row boxes.
 __global__ void __launch_bounds__(MMA_THREADS, 1)
 k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
          const __grid_constant__ CUtensorMap tmW1h, const __grid_constant__ CUtensorMap tmW1l,
-         const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l, const FfnParams p) {
+         const __grid_constant__ CUtensorMap tmW2h, const __grid_constant__ CUtensorMap tmW2l,
+         const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
+         const __grid_constant__ CUtensorMap tmWoh, const __grid_constant__ CUtensorMap tmWol,
+         const __grid_constant__ CUtensorMap tmYh, const __grid_constant__ CUtensorMap tmYl, const FfnParams p) {
   using Cfg = FfnCfg;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
@@ -416,8 +474,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   uint8_t* ring = smem + Cfg::X_BYTES;
   uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
   uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
-  uint64_t* bar_xfull = bar_empty + STAGES;   // x tile landed
-  uint64_t* bar_xempty = bar_xfull + 1;       // ... and read by the tile's last F1
+  uint64_t* bar_xfull = bar_empty + STAGES;   // [4] k-block kb of the x tile landed
+  uint64_t* bar_xempty = bar_xfull + 4;       // [4] ... and no longer read (eight arrivals)
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   int tl_n = 0;
@@ -428,7 +486,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   // PIECE of a leftover tile: hidden chunks [c0, c1) of tile full * ncta + cid / parts.  Pieces 0 .. parts-2 are
   // contributors (their raw fp32 accumulator goes to `scratch`), the last piece is the finisher (adds the
   // contributors' accumulators in piece order, then bias + residual + LayerNorm as for a whole tile).
-  // Contributors have lower CTA ids than their finisher, so they are scheduled no later than it.
+  // Contributors have lower CTA ids than their finisher, so they are scheduled no later than it.  With the prefix
+  // every piece computes x1 itself (LN1 is deterministic: the same bits in every piece).
   struct Item { int mt, c0, c1, mode, piece0; };             // mode: 0 whole tile, 1 contributor, 2 finisher
   auto rev = [&](int t) { return p.reverse ? p.m_tiles - 1 - t : t; };
   const int nlocal = p.full + (cid < p.left * p.parts ? 1 : 0);
@@ -440,24 +499,32 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
     return Item{rev(p.full * ncta + t), c0, c1, p.parts == 1 ? 0 : (part == p.parts - 1 ? 2 : 1),
                 p.parts == 1 ? 0 : slot0 + (part == p.parts - 1 ? 0 : part)};
   };
-  // ring positions of this CTA: four per chunk of every item, in item order
-  const int per_tile = 4 * NC;
+  // ring positions of this CTA: PRE for the out-projection, then four per chunk, of every item in item order
+  const int PRE = p.prefix ? 8 : 0;
+  const int per_tile = PRE + 4 * NC;
   int total = p.full * per_tile;
   if (nlocal > p.full) {
     const Item it = item(p.full);
-    total += 4 * (it.c1 - it.c0);
+    total += PRE + 4 * (it.c1 - it.c0);
   }
+  // x-tile fills: XG per item and k-block ([att,] x), item after item; fill v is k-block v & 3's (v >> 2)-th
+  const int XG = p.prefix ? 2 : 1;
+  const int xtotal = nlocal * 4 * XG;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
       mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
     }
-    mbar_init(smem_u32(bar_xfull), 1);
-    mbar_init(smem_u32(bar_xempty), CONSUMER_WARPS);
+    for (int kb = 0; kb < 4; ++kb) {
+      mbar_init(smem_u32(&bar_xfull[kb]), 1);
+      mbar_init(smem_u32(&bar_xempty[kb]), CONSUMER_WARPS);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmXh); tma_prefetch_desc(&tmXl); tma_prefetch_desc(&tmW1h);
     tma_prefetch_desc(&tmW1l); tma_prefetch_desc(&tmW2h); tma_prefetch_desc(&tmW2l);
+    tma_prefetch_desc(&tmYh); tma_prefetch_desc(&tmYl);
+    if (p.prefix) { tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWoh); tma_prefetch_desc(&tmWol); }
   }
   pdl_trigger();
   __syncthreads();
@@ -465,64 +532,75 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
 
   // ---------------------------------------------------------------- TMA issue (warp 0, one elected lane)
-  // Ring position q holds, for chunk c of its item: q % 4 = 0 / 1: W1 rows [c*64, +64), k-blocks 0-1 / 2-3, hi
-  // then lo; 2 / 3: the hi / lo plane of W2[:, c*64 .. +64).  It is loaded once position q - 3 (same slot) has
-  // been freed by all eight warps.
-  int q_next = 0, x_next = 0;                      // next ring position / next item whose x tile is to be loaded
+  // Ring position q holds, for its item: q < PRE: plane q & 1 (hi, lo) of W_o's k-block q >> 1 (all 256 rows); then
+  // for chunk c, (q - PRE) % 4 = 0 / 1: W1 rows [c*64, +64), k-blocks 0-1 / 2-3, hi then lo; 2 / 3: the hi / lo
+  // plane of W2[:, c*64 .. +64).  It is loaded once position q - 3 (same slot) has been freed by all eight warps.
+  int q_next = 0, x_next = 0;                      // next ring position / next x-tile fill
   auto load_slot = [&](int q) {
     const int j = min(q / per_tile, p.full);
     const Item it = item(j);
-    const int r = q - j * per_tile, c = it.c0 + (r >> 2), k = r & 3;
+    const int r = q - j * per_tile;
     if (elect_one()) {
       const uint32_t full = smem_u32(&bar_full[q % STAGES]);
       const uint32_t dst = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES);
       mbar_expect_tx(full, Cfg::STAGE_BYTES);
-      if (k < 2) {
-        for (int kk = 0; kk < 2; ++kk) {
-          tma_load_2d(dst + kk * 8192, &tmW1h, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
-          tma_load_2d(dst + 16384 + kk * 8192, &tmW1l, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
-        }
+      if (r < PRE) {
+        tma_load_2d(dst, (r & 1) ? &tmWol : &tmWoh, full, (r >> 1) * BK, 0);
       } else {
-        tma_load_2d(dst, k == 3 ? &tmW2l : &tmW2h, full, c * Cfg::CHUNK, 0);
+        const int c = it.c0 + ((r - PRE) >> 2), k = (r - PRE) & 3;
+        if (k < 2) {
+          for (int kk = 0; kk < 2; ++kk) {
+            tma_load_2d(dst + kk * 8192, &tmW1h, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
+            tma_load_2d(dst + 16384 + kk * 8192, &tmW1l, full, (2 * k + kk) * BK, c * Cfg::CHUNK);
+          }
+        } else {
+          tma_load_2d(dst, k == 3 ? &tmW2l : &tmW2h, full, c * Cfg::CHUNK, 0);
+        }
       }
     }
     __syncwarp();
   };
-  auto load_x = [&](int j) {
+  auto load_x = [&](int v) {                       // fill v: k-block v & 3 of item v / (4 XG), both planes
     if (elect_one()) {
+      const int j = v / (4 * XG), kb = v & 3;
+      const bool att = p.prefix && (v >> 2) == j * XG;       // the item's first fill with the prefix: att
       const int m0 = item(j).mt * BM;
-      const uint32_t full = smem_u32(bar_xfull);
-      mbar_expect_tx(full, Cfg::X_BYTES);
-      for (int kb = 0; kb < 4; ++kb) {
-        tma_load_2d(smem_u32(smem + kb * 16384), &tmXh, full, kb * BK, m0);
-        tma_load_2d(smem_u32(smem + 65536 + kb * 16384), &tmXl, full, kb * BK, m0);
-      }
-      if (j + 1 < nlocal) {                        // next tile's x rows -> L2, a whole tile ahead
+      const uint32_t full = smem_u32(&bar_xfull[kb]);
+      mbar_expect_tx(full, 2 * BM * 128);
+      tma_load_2d(smem_u32(smem + kb * 16384), att ? &tmAh : &tmXh, full, kb * BK, m0);
+      tma_load_2d(smem_u32(smem + 65536 + kb * 16384), att ? &tmAl : &tmXl, full, kb * BK, m0);
+      if (att && kb == 0)                          // this item's residual rows -> L2 while att is consumed
+        for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m0); tma_prefetch_2d(&tmXl, k2 * BK, m0); }
+      if (v % (4 * XG) == 0 && j + 1 < nlocal) {   // the next item's rows -> L2, a whole item ahead
         const int m1 = item(j + 1).mt * BM;
-        for (int k2 = 0; k2 < 4; ++k2) { tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1); }
+        for (int k2 = 0; k2 < 4; ++k2) {
+          tma_prefetch_2d(&tmXh, k2 * BK, m1); tma_prefetch_2d(&tmXl, k2 * BK, m1);
+          if (p.prefix) { tma_prefetch_2d(&tmAh, k2 * BK, m1); tma_prefetch_2d(&tmAl, k2 * BK, m1); }
+        }
       }
     }
     __syncwarp();
   };
-  // Load every ring position up to `need` (waiting for its slot: warp 0 reads that position next), then those
-  // whose slot is already free, and the next x tile once the current one has been read.  Freeing position q
-  // never needs a load past q + 2, and the x tile of item j is loaded before any position of item j is waited
-  // for, so the other warpgroup can always free what warp 0 waits on.  Called by warp 0 only, warp-uniformly.
-  auto produce = [&](int need) {
+  // Load every x-tile fill up to `need_x` and ring position up to `need` (blocking: warp 0 reads them next), then
+  // those whose slot is already free.  Warp 0 blocks only where the other warpgroup can always make progress:
+  //   - on x fills at the start of an item (freed by the previous item's last reads of the tile: its y store, or a
+  //     contributor's last F1, which need nothing that has not been loaded) and, with the prefix, before LN1 (the
+  //     residual over att k-block kb, freed by the out-projection MMAs of kb, which need only att and W_o);
+  //   - on ring position q, whose slot frees when position q - 3 has been read.  Freeing position q never needs a
+  //     load past q + 2 (a W_o k-block's planes q, q + 1 retire before q + 2 is asked for; F1 / F2 as before), so
+  //     warp 0 never waits on its own warpgroup, and the other warpgroup's readers of q - 3 need at most positions
+  //     up to q - 1 and the x fills of their item.  Warp 0 has issued those fills itself before asking for any
+  //     position past the out-projection (it needs them for its own LN1 / F1).
+  // Called by warp 0 only, warp-uniformly.
+  auto produce = [&](int need, int need_x) {
+    ring_produce(x_next, xtotal, need_x, bar_xempty, 4, load_x);
     ring_produce(q_next, total, need, bar_empty, STAGES, load_slot);
-    if (x_next < nlocal && __shfl_sync(0xffffffffu, (int)mbar_test(smem_u32(bar_xempty), ((uint32_t)x_next & 1u) ^ 1u), 0))
-      load_x(x_next++);
-  };
-  auto produce_x = [&](int j) {                    // the x tile of item j, waiting for the previous one to be read
-    while (x_next <= j) {
-      mbar_wait(smem_u32(bar_xempty), ((uint32_t)x_next & 1u) ^ 1u);
-      load_x(x_next++);
-    }
   };
 
   // ------------------------------------------------------------------ both warpgroups: MMA + epilogue
   const int cw = warp >> 2;                        // which 64 rows of the tile
   const int cp = 2 * (lane & 3);
+  const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first row inside the tile
   const uint32_t sX = smem_u32(smem) + cw * (64 * 128);
   float acc2[128];
   float acc1[32];
@@ -530,18 +608,53 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   int rc = 0;
   auto slot_full = [&](int r) { mbar_wait(smem_u32(&bar_full[r % STAGES]), ((uint32_t)(r / STAGES)) & 1u); };
   auto slot_free = [&](int r) { if (lane == 0) mbar_arrive(smem_u32(&bar_empty[r % STAGES])); };
+  auto x_full = [&](int kb, uint32_t par) { mbar_wait(smem_u32(&bar_xfull[kb]), par); };
+  auto x_free = [&](int kb) { if (lane == 0) mbar_arrive(smem_u32(&bar_xempty[kb])); };
   for (int j = 0; j < nlocal; ++j) {
     const Item it = item(j);
     const int m0 = it.mt * BM;
-    if (warp == 0) produce_x(j);
-    mbar_wait(smem_u32(bar_xfull), (uint32_t)j & 1u);
-    tl_event(p.tl, tl_n, 2, j);                                      // x tile landed
+    const uint32_t xpar = (uint32_t)(j * XG) & 1u;               // parity of the item's first fill of each k-block
+    if (warp == 0) produce(-1, 4 * j * XG + 3);
+    if (p.prefix) {
+      // ---- P(kb): acc2 = att . W_o^T.  A k-block holds two of the three ring slots, so its MMAs retire (and free
+      // them, and the att k-block for the residual) before the next k-block's second plane is asked for: keeping
+      // two k-blocks in flight would need four slots, and warp 0 would wait on a slot only its own warpgroup frees.
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb) {
+        if (warp == 0) produce(rc + 1, -1);
+        x_full(kb, xpar);
+        slot_full(rc); slot_full(rc + 1);
+        const uint32_t wh = smem_u32(ring + (rc % STAGES) * Cfg::STAGE_BYTES);
+        const uint32_t wl = smem_u32(ring + ((rc + 1) % STAGES) * Cfg::STAGE_BYTES);
+        wg_fence();
+        kblock_ss<256>(acc2, sX + kb * 16384, sX + 65536 + kb * 16384, wh, wl, kb == 0);
+        wg_commit();
+        wg_wait<0>();
+        slot_free(rc); slot_free(rc + 1); x_free(kb);
+        rc += 2;
+        if (warp == 0) produce(-1, -1);            // the next k-block's hi plane goes into a slot freed earlier
+        tl_event(p.tl, tl_n, 60, kb);                                // out-projection k-block kb retired
+      }
+      acc_fence(acc2);
+      // ---- LN1: x1 = LN(acc2 * s0 + b_o + x) over the residual x, in place
+      if (warp == 0) produce(-1, 4 * j * XG + 7);
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb) x_full(kb, xpar ^ 1u);
+      ln_tile(acc2, p.inv_s0, p.b0, p.gamma1, p.beta1, smem, rl, lane, cp);
+      fence_async_smem();
+      named_bar_sync(2 + cw, 128);                 // this warpgroup's 64 rows of x1 are written: its F1 may read them
+      tl_event(p.tl, tl_n, 61, j);                                   // LN1 done
+    } else {
+#pragma unroll
+      for (int kb = 0; kb < 4; ++kb) x_full(kb, xpar);
+    }
+    tl_event(p.tl, tl_n, 2, j);                                      // x tile ready
     int pend = -1;                                   // ring position of the F2 group still in flight
     for (int c = it.c0; c < it.c1; ++c) {
       // ---- F1(c)
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
-        if (warp == 0) produce(rc + half);
+        if (warp == 0) produce(rc + half, -1);
         slot_full(rc + half);
         tl_event(p.tl, tl_n, 10 + half, c);                          // W1 k-blocks 2 * half, +1 landed
         const uint32_t w = smem_u32(ring + ((rc + half) % STAGES) * Cfg::STAGE_BYTES);
@@ -559,8 +672,9 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       if (pend >= 0) slot_free(pend);
       slot_free(rc); slot_free(rc + 1);
       rc += 2;
-      if (c == it.c1 - 1 && lane == 0) mbar_arrive(smem_u32(bar_xempty));     // the x tile may be overwritten
-      if (warp == 0) produce(-1);
+      if (c == it.c1 - 1 && it.mode == 1)          // a contributor does not read the x tile again
+        for (int kb = 0; kb < 4; ++kb) x_free(kb);
+      if (warp == 0) produce(-1, -1);
       // ---- E1(c): bias + GELU -> split16 A fragments
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
@@ -576,7 +690,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       }
       tl_event(p.tl, tl_n, 14, c);                                   // GELU done
       // ---- F2(c): H_lo.W2_hi + H_hi.W2_hi on the hi slot, H_hi.W2_lo on the lo slot
-      if (warp == 0) produce(rc);
+      if (warp == 0) produce(rc, -1);
       slot_full(rc);
       tl_event(p.tl, tl_n, 12, c);                                   // W2 hi plane landed
       wg_fence();
@@ -589,7 +703,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
         }
       }
       wg_commit();
-      if (warp == 0) produce(rc + 1);
+      if (warp == 0) produce(rc + 1, -1);
       slot_full(rc + 1);
       {
         const uint64_t wd = make_desc(smem_u32(ring + ((rc + 1) % STAGES) * Cfg::STAGE_BYTES));
@@ -601,14 +715,13 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       slot_free(rc);
       pend = rc + 1;
       rc += 2;
-      if (warp == 0) produce(-1);
+      if (warp == 0) produce(-1, -1);
     }
     wg_wait<0>();
     acc_fence(acc2);
     if (pend >= 0) slot_free(pend);
-    if (warp == 0) produce(-1);
+    if (warp == 0) produce(-1, -1);
     tl_event(p.tl, tl_n, 4, j);                                      // acc2 complete
-    const int rl = cw * 64 + (warp & 3) * 16 + (lane >> 2);          // this thread's first row inside the tile
     if (it.mode == 1) {
       // ---- contributor piece: the raw fp32 accumulator -> scratch, then the flag
       float* const dst = p.scratch + (size_t)it.piece0 * (BM * 256);
@@ -650,9 +763,31 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       if (threadIdx.x == 0)
         for (int pp = 0; pp < nparts; ++pp) p.flags[it.piece0 + pp] = 0;
     }
-    ln_epilogue(acc2, p.inv_s2, p.b2, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
-                m0 + rl, p.M, cp);
-    tl_event(p.tl, tl_n, 5, j);                                      // LN tail done
+    // ---- LN2: y = LN(acc2 * s2 + b2 + x) over the residual in the x tile, in place; then out through TMA
+    ln_tile(acc2, p.inv_s2, p.b2, p.gamma, p.beta, smem, rl, lane, cp);
+    fence_async_smem();
+    named_bar_sync(2 + cw, 128);                   // this warpgroup's 64 rows of y are in the tile
+    tl_event(p.tl, tl_n, 62, j);                                     // LN2 done
+    if ((warp & 3) == 0) {
+      // one thread per warpgroup stores its 64 rows and, once the stores have read the tile, frees it (4 arrivals
+      // per warpgroup) for the next item's fills
+      if (elect_one()) {
+        if (m0 + cw * 64 < p.M) {
+#pragma unroll
+          for (int kb = 0; kb < 4; ++kb) {
+            const uint32_t src = smem_u32(smem + kb * 16384 + cw * 8192);
+            tma_store_2d(&tmYh, src, kb * BK, m0 + cw * 64);
+            tma_store_2d(&tmYl, src + 65536, kb * BK, m0 + cw * 64);
+          }
+          bulk_commit();
+          bulk_wait_read<0>();
+        }
+#pragma unroll
+        for (int kb = 0; kb < 4; ++kb) mbar_arrive_cnt(smem_u32(&bar_xempty[kb]), 4);
+      }
+      __syncwarp();
+      tl_event(p.tl, tl_n, 63, j);                                   // the y store has read the tile
+    }
   }
   tl_event(p.tl, tl_n, 42);                       // kernel exit
 }
@@ -1015,6 +1150,9 @@ int tc_set_ffn_fused(TcCtx* c, int on) {
   c->ffn_fused = on;
   return old;
 }
+// both planes 16-byte aligned (TMA base addresses)
+static bool planes_aligned16(const ActBuf& b) { return ((uintptr_t)b.hi & 15) == 0 && ((uintptr_t)b.lo() & 15) == 0; }
+
 bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2) {
   if (!c || !c->ffn_fused) return false;
   if (!tc_gemm_supported(c, g1) || !tc_gemm_ln_supported(c, g2, l2)) return false;
@@ -1022,24 +1160,46 @@ bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, co
   if (g1.w.N % FfnCfg::CHUNK || g1.w.N > MAX_N || g1.w.N != g2.K1) return false;
   if (g1.act != ACT_GELU || g1.out_f32 || g1.addtab || g1.zero_lengths) return false;
   if (g1.in_group < g1.M || g1.out_group != 0 || g1.out_off != 0) return false;
+  // the residual is the FFN input itself (the kernel reads it from its x tile); y leaves through TMA stores
+  if (l2.res.hi != g1.a1.hi || l2.res.plane_stride != g1.a1.plane_stride) return false;
+  if (!planes_aligned16(g1.a1) || !planes_aligned16(l2.out)) return false;
   return true;
 }
-bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* scratch, int* flags, cudaStream_t st) {
-  CUtensorMap mXh, mXl, mW1h, mW1l, mW2h, mW2l;
-  const int m_tiles = (g1.M + BM - 1) / BM;
-  const bool ok = make_map(&mXh, g1.a1.hi, g1.M, g1.K1, BM) && make_map(&mXl, g1.a1.lo(), g1.M, g1.K1, BM) &&
-                  make_map(&mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
-                  make_map(&mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
-                  make_map(&mW2h, g2.w.w, g2.w.N, g2.w.K, 256) &&
-                  make_map(&mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256);
+bool tc_tail_supported(const TcCtx* c, const GemmArgs& go, const LnArgs& l1, const GemmArgs& g1, const GemmArgs& g2,
+                       const LnArgs& l2) {
+  if (!tc_gemm_ln_supported(c, go, l1) || !tc_ffn_supported(c, g1, g2, l2)) return false;
+  if (go.K1 != 256 || go.K2 > 0 || go.M != g1.M || !l1.res.hi) return false;
+  // the FFN's input is LN1's output (x1, which the fused kernel keeps in shared memory)
+  if (g1.a1.hi != l1.out.hi || g1.a1.plane_stride != l1.out.plane_stride) return false;
+  return planes_aligned16(go.a1) && planes_aligned16(l1.res);
+}
+
+// k_ffn_tc, standalone (go == nullptr: x = g1.a1) or with the out-projection prefix (x = l1->res, att = go->a1)
+static bool launch_ffn(TcCtx* c, const GemmArgs* go, const LnArgs* l1, const GemmArgs& g1, const GemmArgs& g2,
+                       const LnArgs& l2, float* scratch, int* flags, cudaStream_t st) {
+  CUtensorMap mXh, mXl, mW1h, mW1l, mW2h, mW2l, mAh, mAl, mWoh, mWol, mYh, mYl;
+  const int M = g1.M, m_tiles = (M + BM - 1) / BM;
+  const ActBuf x = go ? l1->res : g1.a1;
+  bool ok = make_map(&mXh, x.hi, M, 256, BM) && make_map(&mXl, x.lo(), M, 256, BM) &&
+            make_map(&mW1h, g1.w.w, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+            make_map(&mW1l, g1.w.w + g1.w.plane_stride, g1.w.N, g1.w.K, FfnCfg::CHUNK) &&
+            make_map(&mW2h, g2.w.w, g2.w.N, g2.w.K, 256) &&
+            make_map(&mW2l, g2.w.w + g2.w.plane_stride, g2.w.N, g2.w.K, 256) &&
+            make_map(&mYh, l2.out.hi, M, 256, 64) && make_map(&mYl, l2.out.lo(), M, 256, 64);
+  if (go) {
+    ok = ok && make_map(&mAh, go->a1.hi, M, 256, BM) && make_map(&mAl, go->a1.lo(), M, 256, BM) &&
+         make_map(&mWoh, go->w.w, go->w.N, go->w.K, 256) && make_map(&mWol, go->w.w + go->w.plane_stride, go->w.N, go->w.K, 256);
+  } else {
+    mAh = mXh; mAl = mXl; mWoh = mW2h; mWol = mW2l;   // not read
+  }
   if (!ok) return false;
   FfnParams p{};
-  p.M = g1.M; p.m_tiles = m_tiles; p.n_chunks = g1.w.N / FfnCfg::CHUNK;
+  p.M = M; p.m_tiles = m_tiles; p.n_chunks = g1.w.N / FfnCfg::CHUNK;
   p.tl = tc::mldb_timeline_buffer();
+  p.prefix = go ? 1 : 0;
+  if (go) { p.inv_s0 = go->w.inv_scale; p.b0 = go->w.bias; p.gamma1 = l1->gamma; p.beta1 = l1->beta; }
   p.inv_s1 = g1.w.inv_scale; p.inv_s2 = g2.w.inv_scale;
   p.b1 = g1.w.bias; p.b2 = g2.w.bias; p.gamma = l2.gamma; p.beta = l2.beta;
-  p.res_hi = l2.res.hi; p.res_lo = l2.res.hi ? l2.res.lo() : nullptr; p.ld_res = l2.res.cols;
-  p.out_hi = l2.out.hi; p.out_lo = l2.out.lo(); p.ld_out = l2.out.cols;
   const int ncta_max = c->sm_count;
   // whole rounds of tiles, then the leftover tiles cut along the hidden dimension so that the last round
   // uses (nearly) every SM instead of `left` of them (FfnParams).  scratch == nullptr, the ffn_split option
@@ -1052,6 +1212,14 @@ bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, 
   }
   const int ncta = p.full > 0 ? ncta_max : p.left * p.parts;
   p.reverse = tc::snake_order();
-  launch_pdl(k_ffn_tc, dim3(ncta), dim3(MMA_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, p);
+  launch_pdl(k_ffn_tc, dim3(ncta), dim3(MMA_THREADS), FfnCfg::SMEM_BYTES, st, mXh, mXl, mW1h, mW1l, mW2h, mW2l, mAh,
+             mAl, mWoh, mWol, mYh, mYl, p);
   return true;
+}
+bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* scratch, int* flags, cudaStream_t st) {
+  return launch_ffn(c, nullptr, nullptr, g1, g2, l2, scratch, flags, st);
+}
+bool tc_tail(TcCtx* c, const GemmArgs& go, const LnArgs& l1, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2,
+             float* scratch, int* flags, cudaStream_t st) {
+  return launch_ffn(c, &go, &l1, g1, g2, l2, scratch, flags, st);
 }

@@ -18,5 +18,11 @@ bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, co
 // that may run tc_ffn concurrently (flags zeroed once); nullptr = no hidden-dimension split of leftover tiles
 constexpr size_t TC_FFN_SCRATCH_BYTES = (size_t)160 * 128 * 256 * 4, TC_FFN_FLAG_BYTES = 160 * 4;
 bool tc_ffn(TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2, float* scratch, int* flags, cudaStream_t st);
+// The encoder layer's tail as one launch: out-projection go + residual + LayerNorm l1 (x1 = l1.out, which the
+// fused kernel keeps in shared memory and does not write), then the FFN block g1 / g2 / l2 on x1.
+bool tc_tail_supported(const TcCtx* c, const GemmArgs& go, const LnArgs& l1, const GemmArgs& g1, const GemmArgs& g2,
+                       const LnArgs& l2);
+bool tc_tail(TcCtx* c, const GemmArgs& go, const LnArgs& l1, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2,
+             float* scratch, int* flags, cudaStream_t st);
 int tc_set_ffn_split(TcCtx* c, int on);
 int tc_set_ffn_fused(TcCtx* c, int on);   // returns the previous setting

@@ -31,6 +31,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
+__device__ __forceinline__ void mbar_arrive_cnt(uint32_t bar, uint32_t n) {   // n arrivals at once
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(n) : "memory");
+}
 // A lost arrival must not hang the GPU: after ~2 s of spinning the kernel traps (the host sees a
 // launch failure instead of a dead box).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
@@ -86,6 +89,20 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
+// Store one box from shared memory into a tensor (elements outside the tensor are not written), as part of the
+// issuing thread's current bulk group.  The shared-memory source is reused only after bulk_wait_read.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+// close the issuing thread's bulk group / wait until at most N of its groups still read their shared memory
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// make this thread's shared-memory writes (generic proxy) visible to later TMA stores and wgmma operand reads
+// (async proxy); a barrier between the writers and the issuing thread follows
+__device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // one lane of a fully converged warp (elect.sync): lets ptxas keep the TMA operands in uniform
 // registers instead of emitting a per-instruction ELECT loop for a lane-id branch

@@ -116,6 +116,24 @@ class Engine:
                                       self._stream()), "mldb_debug_ffn")
         return out
 
+    def debug_tail(self, att, X, Wo, bo, g1, be1, W1, b1, W2, b2, g2, be2, mode=2, pad=None):
+        """Kernel unit-test hook (mldb_debug_tail): x1 = LayerNorm1(att Wo^T + bo + X), then
+        LayerNorm2(x1 + W2 gelu(W1 x1 + b1) + b2); mode 0 CUDA-core, 1 the two wgmma kernels (out-projection + LN
+        GEMM, fused FFN), 2 one fused launch.  att, X [M,d] (device), the rest host; biases may be None.
+        pad: optional [P, d] rows placed in the output buffer past row M before the op; the result is then
+        [M + P, d], its last P rows read back from that buffer after the op."""
+        att, X = _f32c(att, self.device), _f32c(X, self.device)
+        host = [None if t is None else t.detach().float().contiguous().cpu()
+                for t in (Wo, bo, g1, be1, W1, b1, W2, b2, g2, be2)]
+        M, d = X.shape
+        ff = host[4].shape[0]
+        out = torch.empty((M, d), dtype=torch.float32, device=self.device)
+        if pad is not None:
+            out = torch.cat([out, _f32c(pad, self.device)]).contiguous()
+        check(self.lib.mldb_debug_tail(self._h, _ptr(att), _ptr(X), *[_ptr(t) for t in host], M, d, ff, int(mode),
+                                       out.shape[0], _ptr(out), self._stream()), "mldb_debug_tail")
+        return out
+
     def debug_attention(self, q, nseq, Lq, heads, lengths=None, mode=2, kv=None, Lk=None, kv_prefix=0,
                         causal=False):
         """Kernel unit-test hook (mldb_debug_attention).  ``kv is None``: ``q`` is a packed qkv

@@ -1,4 +1,4 @@
-"""In-kernel timeline of one operator (CTA 0): python scripts/timeline.py qkv|attn|outproj_ln|ffn [max_events]
+"""In-kernel timeline of one operator (CTA 0): python scripts/timeline.py qkv|attn|outproj_ln|ffn|tail|tail_fused [max_events]
 Prints, per warp, the sequence of pipeline events with SM-clock deltas (cycles) from the kernel's first event."""
 import ctypes as C, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -11,6 +11,7 @@ TAGS = {1: "prod:tile", 2: "mma:tile_begin", 3: "mma:tile_issued", 4: "epi:acc_r
         20: "prod:Q", 21: "prod:Vslot", 22: "mma:S_go", 23: "mma:K_landed", 24: "mma:S_issued", 25: "mma:P_written", 26: "mma:V_landed",
         40: "entry", 41: "pdl_waited", 42: "exit",
         50: "proj:item", 51: "proj:A_landed", 52: "proj:epi_begin", 53: "proj:epi_stored",
+        60: "tail:outproj_kb", 61: "tail:ln1_done", 62: "tail:ln2_done", 63: "tail:y_store_read",
         30: "sm:wait_S", 31: "sm:S_ready", 32: "sm:pass1", 33: "sm:pass2", 34: "sm:O_ready", 35: "sm:epi_done"}
 op = sys.argv[1] if len(sys.argv) > 1 else "attn"
 maxe = int(sys.argv[2]) if len(sys.argv) > 2 else 400
