@@ -192,14 +192,18 @@ static const RawTensor& rt(mldb_handle* h, const std::string& k) { return h->raw
 
 // Pack a host [N, K] fp32 matrix into split fp16 planes scaled by 2^s.  Kpad > K zero-pads the rows
 // (odd K such as the 263 motion features: the tensor-core GEMM wants K % 64 == 0).
+// The scale comes from the finite elements only, so an inf or NaN element poisons its own output column (as in
+// torch) and not the precision of every other one; an all-zero or all non-finite W packs at s = 0.
 static int pack_linear(mldb_handle* h, const float* W, int N, int K, const float* bias, LinW* out, int Kpad = 0) {
   if (Kpad < K) Kpad = K;
   float mx = 0.0f;
-  for (int64_t i = 0; i < (int64_t)N * K; ++i) mx = std::max(mx, fabsf(W[i]));
+  for (int64_t i = 0; i < (int64_t)N * K; ++i)
+    if (std::isfinite(W[i])) mx = std::max(mx, fabsf(W[i]));
   int s = 0;
   if (mx > 0.0f) {
-    s = (int)floorf(log2f(16384.0f / mx));
-    s = std::max(-14, std::min(14, s));
+    // clamp before the conversion to int: below mx ~ 5e-35, 16384 / mx overflows to inf
+    const float e = floorf(log2f(16384.0f / mx));
+    s = (int)std::max(-14.0f, std::min(14.0f, e));
   }
   const float sc = ldexpf(1.0f, s);
   std::vector<__half> buf((size_t)2 * N * Kpad, __float2half_rn(0.0f));
