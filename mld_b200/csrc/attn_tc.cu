@@ -325,9 +325,6 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   tl_event(p.tl, tl_n, 42);                       // kernel exit
 }
 
-int g_sm_count = 132;
-bool g_ready = false;
-
 // launch geometry for a shape; false when it does not fit
 bool plan_shape(const AttnArgs& a, AtcParams* p) {
   const int npad = (a.Lk + 15) & ~15;
@@ -343,20 +340,17 @@ auto pick_kernel(int nkb) { return nkb <= 2 ? k_attn_tc<HD, CAUSAL, 2> : k_attn_
 
 }  // namespace
 
-bool tc_attention_init(int device) {
-  if (g_ready) return true;
-  cudaDeviceGetAttribute(&g_sm_count, cudaDevAttrMultiProcessorCount, device);
+bool tc_attention_init() {
   using Kernel = void (*)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, AtcParams);
   const Kernel kernels[] = {k_attn_tc<64, false, 2>, k_attn_tc<64, false, 4>, k_attn_tc<64, true, 2>, k_attn_tc<64, true, 4>,
                             k_attn_tc<128, false, 2>, k_attn_tc<128, false, 4>, k_attn_tc<128, true, 2>, k_attn_tc<128, true, 4>};
   for (Kernel k : kernels)
     if (!smem_opt_in(k, SMEM_BYTES, "k_attn_tc")) return false;
-  g_ready = true;
   return true;
 }
 
 bool tc_attention_supported(const AttnArgs& a) {
-  if (!g_ready || (a.hd != 64 && a.hd != 128) || a.Lq < 1 || a.Lk < 1 || a.Lk > 256 || a.nseq < 1) return false;
+  if ((a.hd != 64 && a.hd != 128) || a.Lq < 1 || a.Lk < 1 || a.Lk > 256 || a.nseq < 1) return false;
   if (a.causal && a.Lq != a.Lk) return false;
   if ((a.q.cols % 8) || (a.kv.cols % 8) || (a.q_col0 % 8) || (a.k_col0 % 8) || (a.v_col0 % 8)) return false;
   if ((a.out.cols % 8) || ((uintptr_t)a.q.hi & 15) || ((uintptr_t)a.kv.hi & 15) || ((uintptr_t)a.out.hi & 15)) return false;
@@ -365,7 +359,7 @@ bool tc_attention_supported(const AttnArgs& a) {
   return plan_shape(a, &p);
 }
 
-bool tc_attention(const AttnArgs& a, cudaStream_t st) {
+bool tc_attention(const AttnArgs& a, int sm_count, cudaStream_t st) {
   AtcParams p{};
   if (!plan_shape(a, &p)) return false;
   CUtensorMap mQh, mQl, mKh, mKl, mRh, mRl;
@@ -385,7 +379,7 @@ bool tc_attention(const AttnArgs& a, cudaStream_t st) {
   p.heads_log2 = -1;
   for (int k = 0; k < 8; ++k) if ((1 << k) == p.heads) p.heads_log2 = k;
   const int pairs = (p.items + 1) / 2;                 // two pipelines per CTA
-  const int grid = pairs < g_sm_count ? pairs : g_sm_count;
+  const int grid = pairs < sm_count ? pairs : sm_count;
   auto kernel = a.hd == 64 ? (a.causal ? pick_kernel<64, true>(p.nkb) : pick_kernel<64, false>(p.nkb))
                            : (a.causal ? pick_kernel<128, true>(p.nkb) : pick_kernel<128, false>(p.nkb));
   launch_pdl(kernel, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);

@@ -1,15 +1,74 @@
-// Internal engine types of libmldb200 (not part of the C ABI).
+// Internal engine types of libmldb200 (not part of the C ABI), and what the engine sources share: the error macros,
+// the operator dispatch, the workspace and plan helpers.
 #pragma once
 #include <cuda_runtime.h>
+#include <stdio.h>
 
+#include <functional>
 #include <map>
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "../../include/mldb.h"
-#include "misc_kernels.cuh"
 #include "ops.cuh"
+
+#define CK(call)                                                                      \
+  do {                                                                                \
+    cudaError_t e__ = (call);                                                         \
+    if (e__ != cudaSuccess) {                                                         \
+      char buf__[512];                                                                \
+      snprintf(buf__, sizeof buf__, "%s:%d: %s failed: %s", __FILE__, __LINE__, #call, \
+               cudaGetErrorString(e__));                                              \
+      mldb_set_err(buf__);                                                            \
+      return MLDB_ERR_CUDA;                                                           \
+    }                                                                                 \
+  } while (0)
+
+#define FAIL(code, ...)                         \
+  do {                                          \
+    char buf__[512];                            \
+    snprintf(buf__, sizeof buf__, __VA_ARGS__); \
+    mldb_set_err(buf__);                        \
+    return (code);                              \
+  } while (0)
+
+#define TRY(expr)                 \
+  do {                            \
+    int rc__ = (expr);            \
+    if (rc__ != MLDB_OK) return rc__; \
+  } while (0)
+
+// Every ABI call runs on the handle's device and restores the caller's current device afterwards
+// (a single-process multi-GPU program must not find torch.cuda.current_device() changed under it).
+struct DeviceGuard {
+  int prev = -1;
+  explicit DeviceGuard(int dev) {
+    if (cudaGetDevice(&prev) != cudaSuccess) prev = -1;
+    if (prev != dev) cudaSetDevice(dev); else prev = -1;
+  }
+  ~DeviceGuard() { if (prev >= 0) cudaSetDevice(prev); }
+  DeviceGuard(const DeviceGuard&) = delete;
+  DeviceGuard& operator=(const DeviceGuard&) = delete;
+};
+
+// The split16 layout (common.cuh) of a [rows, cols] activation at p: each plane padded to whole 128-row tiles.
+inline ActBuf split16_at(void* p, int rows, int cols) {
+  const int64_t rp = ((int64_t)rows + 127) / 128 * 128;
+  return ActBuf{(__half*)p, rp * cols, rows, cols};
+}
+inline size_t split16_bytes(int rows, int cols) { return 2 * sizeof(__half) * split16_at(nullptr, rows, cols).plane_stride; }
+inline ActBuf rows_of(ActBuf b, int64_t row0, int rows) { b.hi += row0 * b.cols; b.rows = rows; return b; }
+inline unsigned nblk(int64_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
+
+// A device buffer of the eager entry points, grown on demand and freed with the handle.
+struct GrowBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  GrowBuf() = default;
+  GrowBuf(const GrowBuf&) = delete;
+  GrowBuf& operator=(const GrowBuf&) = delete;
+  ~GrowBuf() { cudaFree(p); }
+};
 
 struct LnW { float* g = nullptr; float* b = nullptr; };
 
@@ -47,12 +106,10 @@ struct TextW {
   LinW proj;                      // text_projection, no bias
   float* tok = nullptr;           // token_embedding [vocab, hidden] fp32
   float* pos = nullptr;           // position_embedding [max_positions, hidden] fp32
-  // workspace for `rows` tokens (grown on demand by mldb_text_encode)
-  int rows = 0, seqs = 0;
-  float* x = nullptr;             // [rows, hidden] fp32 residual stream
-  ActBuf a{}, qkv{}, att{}, h{};  // LN output, q|k|v, attention output, fc1 output (split16)
-  ActBuf pooled{};                // [seqs, hidden] final LN of the eos rows (split16, A of text_projection)
-  std::vector<void*> ws_allocs;
+  // workspace of mldb_text_encode
+  GrowBuf x;                      // [rows, hidden] fp32 residual stream
+  GrowBuf a, qkv, att, h;         // LN output, q|k|v, attention output, fc1 output (split16)
+  GrowBuf pooled;                 // [seqs, hidden] final LN of the eos rows (split16, A of text_projection)
 };
 
 // T2M evaluator (mldb_t2m_configure): bidirectional GRU + BiGRUCo head, the movement convolutions
@@ -73,9 +130,14 @@ struct T2mW {
   LinW motion_in;                 // motion: input_emb
   GruW text_gru, motion_gru;
   int chunk = 0;                  // option t2m_chunk (0: from the workspace budget)
-  static constexpr int NBUF = 10;
-  void* buf[NBUF] = {};           // workspace slots, grown on demand
-  size_t cap[NBUF] = {};
+  // workspace; the encoders run one at a time, so buffers that are never live together are shared
+  GrowBuf in;                     // split16 A of the first GEMM: movement im2col of the poses, motion rows, text pos_ohot
+  GrowBuf f32;                    // fp32: the GRU's x W_ih^T + b_ih, movement conv1 output
+  GrowBuf emb;                    // split16: the GRU input rows, movement im2col of the conv1 output
+  GrowBuf mid;                    // movement conv2 output (split16), text word_embs + pos_emb (fp32)
+  GrowBuf words;                  // text word_embs + pos_emb (split16, K padded)
+  GrowBuf h_split, h_f32, gh;     // GRU state ping-pong (split16, fp32), CUDA-core h W_hh^T
+  GrowBuf head_f32, head_ln;      // GRU head: first Linear, LayerNorm + LeakyReLU
 };
 
 struct RawTensor {
@@ -100,8 +162,18 @@ struct StackWs {
 
 struct TcCtx;
 
+// A plan's workspace serves one entry point at one shape; the kind is part of the plan key.
+enum PlanKind {
+  PLAN_REVERSE = 0,       // reverse diffusion, trans_enc denoiser (mldb_diffusion_reverse, mldb_sample)
+  PLAN_VAE_DECODE = 1,
+  PLAN_VAE_ENCODE = 2,
+  PLAN_DENOISE = 3,       // one trans_enc denoiser pass (mldb_denoise)
+  PLAN_DENOISE_DEC = 4,   // one trans_dec (no-VAE) denoiser pass (mldb_denoise)
+  PLAN_REVERSE_DEC = 5,   // reverse diffusion, trans_dec denoiser
+};
+
 struct Plan {
-  int kind = 0;       // 0 reverse (denoiser), 1 vae decode, 2 vae encode, 3 single denoise
+  int kind = PLAN_REVERSE;
   int B = 0, S = 0, T = 0, Bx = 0, Ntok = 0;
   StackWs ws;
   ActBuf mem;         // memory tokens for decoder stacks
@@ -194,6 +266,80 @@ struct mldb_handle {
   cudaEvent_t ev_local_done = nullptr, ev_gather_done[2] = {};
   int64_t gather_count = 0;
 };
+
+struct SeqInfo {
+  const int32_t* lengths = nullptr;  // key-padding: valid keys = kv_prefix + lengths[s % len_mod]
+  int kv_prefix = 0;
+  int len_mod = 0;
+};
+
+// engine.cu
+inline void kcount(mldb_handle* h, int kind) {
+  h->kstat[kind]++;
+  if (h->capturing) h->capture_nodes++; else h->launches++;
+}
+int check_ready(mldb_handle* h, bool need_sched);
+int check_ops(mldb_handle* h);
+// The exit of an eager entry point that enqueued operators: a launch error or an operator that could not be
+// enqueued fails the call.
+inline int ops_done(mldb_handle* h) {
+  CK(cudaGetLastError());
+  return check_ops(h);
+}
+int dev_alloc(mldb_handle* h, void** p, size_t bytes);
+int grow(GrowBuf& b, size_t bytes);
+int grow_act(GrowBuf& b, int rows, int cols, ActBuf* out);
+int upload_f32(mldb_handle* h, const float* src, size_t n, float** out);
+int upload_pe(mldb_handle* h, const std::string& key, float** out, int* rows = nullptr);
+const RawTensor& rt(mldb_handle* h, const std::string& k);
+void spec_add(mldb_handle* h, const std::string& key, std::vector<int64_t> shape);
+void spec_ln(mldb_handle* h, const std::string& p, int d);
+int pack_linear(mldb_handle* h, const float* W, int N, int K, const float* bias, LinW* out, int Kpad = 0);
+int pack_named(mldb_handle* h, const std::string& wkey, const std::string& bkey, LinW* out, int row0 = 0,
+               int nrows = -1, bool pad_k = false);
+int pack_ln(mldb_handle* h, const std::string& p, int d, LnW* out);
+int time_tokens(mldb_handle* h, const int64_t* d_ts, int64_t t_scalar, int n, const float* pe_row, float* out,
+                float* scratch_feats, float* scratch_h, cudaStream_t st);
+Plan* find_plan(mldb_handle* h, PlanKind kind, int B, int S, int T);
+Plan* add_plan(mldb_handle* h, PlanKind kind, int B, int S, int T);
+// Run `record` either directly on `st` or as a (cached) CUDA graph.
+int run_graphed(mldb_handle* h, Plan* p, cudaStream_t st, const std::function<void(cudaStream_t)>& record);
+
+// stack.cu: operators (each picks its kernel and counts it in kstat), workspaces, transformer stacks
+void op_gemm(mldb_handle* h, const GemmArgs& g, cudaStream_t st);
+void op_gemm_ln(mldb_handle* h, GemmArgs g, LnArgs l, float* cf32, cudaStream_t st);
+void op_ln(mldb_handle* h, const LnArgs& l, cudaStream_t st);
+void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st);
+void op_tail(mldb_handle* h, const LinW& wo, const LnW& n1, const LinW& l1, const LinW& l2, const LnW& n2, ActBuf att,
+             ActBuf x, ActBuf x1, ActBuf hbuf, ActBuf xout, int M, int d, int ff, float* cf32, cudaStream_t st,
+             int fuse = 1);
+void rows_to_split(mldb_handle* h, ActBuf X, const float* src, int ld_src, int M, int d, int in_group, int out_group,
+                   int out_off, int src_bcast, const float* tab, int relu, cudaStream_t st);
+int alloc_act(mldb_handle* h, int rows, int cols, ActBuf* out);
+int alloc_stack_ws(mldb_handle* h, const StackW& sw, int nseq, int L, int Lmem, StackWs* ws, int n_sel = 0);
+StackWs ws_slice(const StackWs& ws, int s0, int n);
+void out_proj_ln(mldb_handle* h, const LinW& w, const LnW& n, ActBuf att, ActBuf res, ActBuf xout, int M, int d,
+                 float* cf32, cudaStream_t st);
+void ffn_block(mldb_handle* h, const LinW& l1, const LinW& l2, const LnW& n, ActBuf xin, ActBuf xout, StackWs& ws,
+               int act, cudaStream_t st);
+void enc_layer(mldb_handle* h, const StackW& sw, const EncW& w, ActBuf xin, ActBuf xout, StackWs& ws,
+               const SeqInfo& si, cudaStream_t st);
+ActBuf run_stack(mldb_handle* h, const StackW& sw, ActBuf x0, ActBuf mem, StackWs& ws, const SeqInfo& si,
+                 cudaStream_t st);
+
+// denoiser.cu
+int enc_plan(mldb_handle* h, PlanKind kind, int B, int Bx, int S, Plan** out);
+int place_condition(mldb_handle* h, Plan* p, const void* cond, cudaStream_t st);
+void denoiser_pass(mldb_handle* h, Plan* p, const float* latents, int lat_mod, const float* tt, float* eps_out,
+                   cudaStream_t st);
+// vae.cu
+int dec_plan(mldb_handle* h, int B, int T, Plan** out);
+int run_decode(mldb_handle* h, const float* z, const int32_t* lengths, int B, int T, float* feats_out, cudaStream_t st,
+               Plan** plan_out);
+int run_f2j(mldb_handle* h, const float* feats, int B, int T, float* joints, cudaStream_t st);
+// text_tower.cu, t2m.cu
+int pack_text(mldb_handle* h);
+int pack_t2m(mldb_handle* h);
 
 // comm.cu
 void mldb_comm_release(mldb_handle* h);

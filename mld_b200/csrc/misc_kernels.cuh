@@ -1,7 +1,7 @@
 // Small elementwise / scan kernels of the sampling path (token assembly, timestep features,
 // classifier-free guidance + scheduler update, feats2joints).
 #pragma once
-#include "common.cuh"
+#include "ops.cuh"
 
 // get_timestep_embedding (mld/models/architectures/tools/embeddings.py:245-285) for a list of
 // integer timesteps: out[i, :] = [cos | sin] (flip_sin_to_cos) of t_i * exp(-ln(1e4) k/(half-shift)).
@@ -130,6 +130,12 @@ static __global__ void k_f32_to_split_pad(ActBuf X, const float* __restrict__ sr
   }
 }
 
+// the first n elements of a split16 buffer whose rows are contiguous (cols == leading dimension), widened to fp32
+static __global__ void k_split_to_f32(ActBuf X, float* __restrict__ out, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = join_f32(X.hi[i], X.lo()[i]);
+}
+
 // device-side step counter of a replayed single-step graph (the 1000-step DDPM loop of the no-VAE model)
 static __global__ void k_step_set(int* step, int v) { *step = v; }
 static __global__ void k_step_inc(int* step) { *step += 1; }
@@ -143,17 +149,6 @@ static __global__ void k_permute_01(const float* __restrict__ src, float* __rest
   const int a = (int)(idx / ((int64_t)d * B));
   dst[((int64_t)b * A + a) * d + n] = src[idx];
 }
-
-// Scheduler coefficients for one step, computed on the host in fp32 exactly as diffusers does
-// (0-d fp32 tensor arithmetic; x ** 0.5 == sqrtf).
-struct StepCoef {
-  float c0, c1, c2, c3;  // DDIM: sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-std^2)
-                         // DDPM: sqrt(a_t), sqrt(1-a_t), x0 coeff, sample coeff
-  float sigma;           // scale of the injected N(0,1) noise; 0 = the step adds none (and reads none)
-                         // DDIM: std_dev_t = eta * sqrt(variance); DDPM: sqrt(clamp(var, 1e-20)) when t > 0
-  int kind;              // 0 DDIM, 1 DDPM
-  int clip;              // clip_sample: x0 clamped to [-1, 1] (clip_sample_range 1.0)
-};
 
 __device__ __forceinline__ float sched_update(const StepCoef& k, float x, float e, float nz) {
   // pred_original_sample = (sample - beta_prod_t ** 0.5 * model_output) / alpha_prod_t ** 0.5

@@ -73,6 +73,17 @@ struct AttnArgs {
   ActBuf out{};                       // [nseq*Lq, heads*hd]
 };
 
+// Scheduler coefficients for one step, computed on the host in fp32 exactly as diffusers does
+// (0-d fp32 tensor arithmetic; x ** 0.5 == sqrtf).
+struct StepCoef {
+  float c0, c1, c2, c3;  // DDIM: sqrt(a_t), sqrt(1-a_t), sqrt(a_prev), sqrt(1-a_prev-std^2)
+                         // DDPM: sqrt(a_t), sqrt(1-a_t), x0 coeff, sample coeff
+  float sigma;           // scale of the injected N(0,1) noise; 0 = the step adds none (and reads none)
+                         // DDIM: std_dev_t = eta * sqrt(variance); DDPM: sqrt(clamp(var, 1e-20)) when t > 0
+  int kind;              // 0 DDIM, 1 DDPM
+  int clip;              // clip_sample: x0 clamped to [-1, 1] (clip_sample_range 1.0)
+};
+
 // --- SIMT implementations (simt.cu) ---
 void simt_gemm(const GemmArgs& a, cudaStream_t st);
 void simt_ln(const LnArgs& a, cudaStream_t st);
@@ -82,13 +93,14 @@ bool simt_attention(const AttnArgs& a, cudaStream_t st);
 bool simt_attention_supported(int hd);
 // --- mma.sync tensor-core attention (attn_mma.cu) ---
 bool mma_attention_supported(const AttnArgs& a);
-bool mma_attention_init();                                // outside stream capture
+bool mma_attention_init();                                // per device, outside stream capture
 void mma_attention(const AttnArgs& a, cudaStream_t st);
 // attn_tc.cu: wgmma attention core (Lk <= 256, head_dim 64 / 128)
-bool tc_attention_init(int device);                       // once per process, outside stream capture
+bool tc_attention_init();                                 // per device, outside stream capture
 bool tc_attention_supported(const AttnArgs& a);
-bool tc_attention(const AttnArgs& a, cudaStream_t st);    // false: tensor-map encoding failed, nothing launched
-bool simt_init();                                         // reads MLDB_PDL; outside stream capture
+// at most sm_count CTAs; false: tensor-map encoding failed, nothing launched
+bool tc_attention(const AttnArgs& a, int sm_count, cudaStream_t st);
+bool simt_init();                                         // reads MLDB_PDL; per device, outside stream capture
 // --- CLIP text tower row kernels (text_ln.cu) ---
 // One warp per row, d a multiple of 128 up to 1024, exact two-pass statistics, no shared memory.
 //   TEXT_LN_ROWS:  out = LN(x[r])                                   (pre-norm LN1 / LN2, final LN of every row)
@@ -129,7 +141,7 @@ __host__ __device__ __forceinline__ int gru_packed_col(int g, int u) {
   const int t = u >> 5, uu = u & 31;
   return t * 96 + (3 * (uu >> 3) + g) * 8 + (uu & 7);
 }
-bool gru_tc_init();                                              // once per process, outside stream capture
+bool gru_tc_init();                                              // per device, outside stream capture
 bool gru_shape_supported(int H);                                 // 64 <= H <= 1024, H % 64 == 0
 bool gru_step_tc(const GruStepArgs& a, cudaStream_t st);         // false: tensor-map encoding failed, nothing launched
 void gru_gate_simt(const GruStepArgs& a, cudaStream_t st);       // the gate update from a.gh (CUDA cores)

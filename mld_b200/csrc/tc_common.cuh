@@ -340,7 +340,7 @@ __device__ __forceinline__ void tl_event(long long* tl, int& n, int tag, int aux
     ++n;
   }
 }
-long long* mldb_timeline_buffer();   // engine.cu: the device buffer while a timeline is being recorded, else nullptr
+long long* mldb_timeline_buffer();   // debug.cu: the device buffer while a timeline is being recorded, else nullptr
 
 // ---------------------------------------------------------------------------------- host: tensor maps
 typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
