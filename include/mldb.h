@@ -374,6 +374,36 @@ int mldb_t2m_text(mldb_handle* h, const float* word_embs, const float* pos_ohot,
  * of the chunking.  The GEMMs count under MLDB_KSTAT_GEMM_TC (GEMM_SIMT with gemm=simt), the recurrent steps under
  * MLDB_KSTAT_GRU_TC (with gemm=simt: two GEMM_SIMT and one MISC gate kernel per step). */
 
+/* ---- HumanAct12 action classifier (HUMANACTMetrics, mld/models/metrics/gru.py): MotionDiscriminator and
+ * MotionDiscriminatorForFID (mld/models/architectures/humanact12_gru.py), whose logits feed the action model's accuracy
+ * and whose tanh(linear1) features feed its FID, diversity and multimodality.  nn.GRU(input_size, hidden_size,
+ * hidden_layer) -> the output at lengths - 1 -> Linear(hidden_size, 30) -> tanh -> Linear(30, output_size).
+ * Keys (strict) under "gru_classifier.": recurrent.{weight_ih,weight_hh,bias_ih,bias_hh}_l{k}, linear1.weight /
+ * .bias [30, hidden_size] / [30], linear2.weight / .bias [output_size, 30] / [output_size]. */
+#define MLDB_A2M_ABI_VERSION 1
+typedef struct mldb_a2m_config {
+  int32_t abi_version;        /* must be MLDB_A2M_ABI_VERSION */
+  int32_t input_size;         /* 72 (24 joints x 3) */
+  int32_t hidden_size;        /* 128; 64 or 128: the layer's split16 W_hh must fit in shared memory */
+  int32_t hidden_layer;       /* 2; 1 .. 8 */
+  int32_t output_size;        /* 12 action classes */
+} mldb_a2m_config;
+void mldb_default_a2m_config(mldb_a2m_config* cfg);
+/* Add the classifier's keys to the strict key spec; after mldb_create, before mldb_finalize_weights. */
+int mldb_a2m_configure(mldb_handle* h, const mldb_a2m_config* cfg);
+/* Replaces: MotionDiscriminator.forward / MotionDiscriminatorForFID.forward with an explicit hidden_unit.
+ *   x        [B, input_size, T] fp32 (the reference's motion_sequence.reshape(bs, njoints * nfeats, T))
+ *   lengths  device int32 [B], each in [1, T]; frames t >= lengths[b] are never read
+ *   h0       [hidden_layer, B, hidden_size] fp32, each sequence's own initial state
+ *   logits   [B, output_size] (may be NULL);  features  [B, 30] tanh(linear1) (may be NULL)
+ * The lengths are copied to the host and checked before anything is launched (the call synchronises `stream`).
+ * Runs eagerly on `stream` in batch chunks that bound the workspace (which grows on demand, outside any capture, and
+ * synchronises the device when it does); every sequence is computed independently of the others and of the chunking.
+ * Each layer is one k_gru_seq_tc launch per chunk (MLDB_KSTAT_GRU_TC) behind its input GEMM (MLDB_KSTAT_GEMM_TC); with
+ * gemm=simt, every step is one GEMM_SIMT and one MISC gate kernel. */
+int mldb_a2m_classify(mldb_handle* h, const float* x, const int32_t* lengths, const float* h0, int32_t B, int32_t T,
+                      float* logits, float* features, void* stream);
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);
@@ -394,7 +424,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
 #define MLDB_KSTAT_LN_UNFUSED 8   /* k_ln behind a GEMM whose LayerNorm could NOT be fused (a fallback) */
 #define MLDB_KSTAT_MISC 9         /* token assembly, scheduler step, feats2joints, ... */
 #define MLDB_KSTAT_TEXT_LN 10     /* k_text_ln: the text tower's row LayerNorm (+ embedding / eos gather) */
-#define MLDB_KSTAT_GRU_TC 11      /* k_gru_step_tc: one recurrent step of the T2M evaluator's bidirectional GRU */
+#define MLDB_KSTAT_GRU_TC 11      /* k_gru_step_tc: one recurrent step of the T2M evaluator's bidirectional GRU;
+                                     k_gru_seq_tc: one whole layer of the action classifier's GRU */
 #define MLDB_KSTAT_COUNT 12
 int mldb_kernel_stats(const mldb_handle* h, int64_t* out, int32_t n);
 int mldb_reset_kernel_stats(mldb_handle* h);
@@ -411,6 +442,7 @@ int mldb_reset_kernel_stats(mldb_handle* h);
  *   "branches"   1..4                   concurrent sub-batch branches inside a denoiser step (2)      MLDB_BRANCHES
  *   "graph"      0 | 1                  CUDA-graph replay of the step loop (1)                        MLDB_GRAPH
  *   "t2m_chunk"  0 | n                  T2M evaluator: sequences per batch chunk (0: sized from the workspace budget)
+ *   "a2m_chunk"  0 | n                  action classifier: sequences per batch chunk (0: from the workspace budget)
  * Environment only: MLDB_PDL (programmatic dependent launch, 1); MLDB_SNAKE (1: attention and the fused FFN walk
  * the token tiles downwards, the GEMMs upwards, so every kernel starts on the rows its producer wrote last). */
 int mldb_set_option(mldb_handle* h, const char* name, const char* value);

@@ -29,6 +29,8 @@ TEXT_HIDDEN, TEXT_POOLED = 0, 1
 # T2M evaluator (mldb_t2m_config, mldb_t2m_*)
 MLDB_T2M_ABI_VERSION = 1
 T2M_TEXT, T2M_MOVEMENT, T2M_MOTION = 1, 2, 4
+# HumanAct12 action classifier (mldb_a2m_config, mldb_a2m_classify)
+MLDB_A2M_ABI_VERSION = 1
 
 
 class MldbConfig(C.Structure):
@@ -65,6 +67,14 @@ class MldbT2mConfig(C.Structure):
         ("dim_text_hidden", C.c_int32), ("dim_coemb_hidden", C.c_int32), ("dim_pose", C.c_int32),
         ("dim_move_hidden", C.c_int32), ("dim_move_latent", C.c_int32), ("dim_motion_hidden", C.c_int32),
         ("dim_motion_latent", C.c_int32),
+    ]
+
+
+class MldbA2mConfig(C.Structure):
+    """``mldb_a2m_config`` (include/mldb.h)."""
+    _fields_ = [
+        ("abi_version", C.c_int32), ("input_size", C.c_int32), ("hidden_size", C.c_int32),
+        ("hidden_layer", C.c_int32), ("output_size", C.c_int32),
     ]
 
 
@@ -107,6 +117,9 @@ _SIGNATURES = {
     "mldb_t2m_movement": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_t2m_motion": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
     "mldb_t2m_text": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_default_a2m_config": (None, [C.POINTER(MldbA2mConfig)]),
+    "mldb_a2m_configure": (C.c_int, [_P, C.POINTER(MldbA2mConfig)]),
+    "mldb_a2m_classify": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
@@ -165,4 +178,10 @@ def default_text_config() -> MldbTextConfig:
 def default_t2m_config() -> MldbT2mConfig:
     cfg = MldbT2mConfig()
     lib().mldb_default_t2m_config(C.byref(cfg))
+    return cfg
+
+
+def default_a2m_config() -> MldbA2mConfig:
+    cfg = MldbA2mConfig()
+    lib().mldb_default_a2m_config(C.byref(cfg))
     return cfg

@@ -1,6 +1,6 @@
 // libmldb200 engine: handles and their options, the state-dict spec and weight packing of the sampling models,
 // scheduler tables, plans and CUDA-graph capture.  The models' forward passes live in stack.cu (transformer stacks),
-// denoiser.cu, vae.cu, text_tower.cu and t2m.cu.
+// denoiser.cu, vae.cu, text_tower.cu, t2m.cu and a2m.cu.
 #include "engine.h"
 
 #include <math.h>
@@ -486,6 +486,8 @@ extern "C" int mldb_set_option(mldb_handle* h, const char* name, const char* val
     h->use_graph = strcmp(value, "0") != 0;
   } else if (!strcmp(name, "t2m_chunk")) {
     h->t2m.chunk = std::max(atoi(value), 0);
+  } else if (!strcmp(name, "a2m_chunk")) {
+    h->a2m.chunk = std::max(atoi(value), 0);
   } else {
     FAIL(MLDB_ERR_INVALID, "unknown option %s", name);
   }
@@ -585,6 +587,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
   }
   if (h->text.on) TRY(pack_text(h));
   if (h->t2m.on) TRY(pack_t2m(h));
+  if (h->a2m.on) TRY(pack_a2m(h));
   for (auto& kv : h->raw) { kv.second.host.clear(); kv.second.host.shrink_to_fit(); }
   h->finalized = true;
   return MLDB_OK;

@@ -140,6 +140,26 @@ struct T2mW {
   GrowBuf head_f32, head_ln;      // GRU head: first Linear, LayerNorm + LeakyReLU
 };
 
+// HumanAct12 action classifier (mldb_a2m_configure): nn.GRU(input, H, layers) + Linear(H, 30), tanh, Linear(30, out)
+struct A2mLayerW {
+  LinW w_ih;                      // [3H, in] (K padded to a multiple of 64), gates r | z | n, bias b_ih
+  LinW w_hh;                      // [3H, H], rows in gru_packed_col order, no bias
+  float* b_hh = nullptr;          // [3H] fp32
+};
+struct A2mW {
+  bool on = false;
+  mldb_a2m_config cfg{};
+  std::vector<A2mLayerW> layers;
+  float *l1w = nullptr, *l1b = nullptr, *l2w = nullptr, *l2b = nullptr;   // the fp32 head: linear1, linear2
+  int chunk = 0;                  // option a2m_chunk (0: from the workspace budget)
+  // workspace of mldb_a2m_classify
+  GrowBuf x;                      // split16 frames [n * T, input_size padded to 64]
+  GrowBuf gi;                     // fp32 [n * T, 3H]: x_t W_ih^T + b_ih of the running layer
+  GrowBuf seq;                    // split16 [n * T, H]: a layer's h_t, the A operand of the next layer's input GEMM
+  GrowBuf h_last;                 // fp32 [n, H]: the last layer's h at t = len - 1
+  GrowBuf h_split, h_f32, gh;     // gemm=simt: state ping-pong (split16, fp32), h W_hh^T
+};
+
 struct RawTensor {
   std::vector<float> host;
   std::vector<int64_t> shape;
@@ -222,6 +242,7 @@ struct mldb_handle {
   float* mean = nullptr; float* stdv = nullptr; int nstat = 0;
   TextW text;          // CLIP text tower (mldb_text_configure)
   T2mW t2m;            // T2M evaluator (mldb_t2m_configure)
+  A2mW a2m;            // HumanAct12 action classifier (mldb_a2m_configure)
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;
@@ -337,9 +358,10 @@ int dec_plan(mldb_handle* h, int B, int T, Plan** out);
 int run_decode(mldb_handle* h, const float* z, const int32_t* lengths, int B, int T, float* feats_out, cudaStream_t st,
                Plan** plan_out);
 int run_f2j(mldb_handle* h, const float* feats, int B, int T, float* joints, cudaStream_t st);
-// text_tower.cu, t2m.cu
+// text_tower.cu, t2m.cu, a2m.cu
 int pack_text(mldb_handle* h);
 int pack_t2m(mldb_handle* h);
+int pack_a2m(mldb_handle* h);   // a2m.cu
 
 // comm.cu
 void mldb_comm_release(mldb_handle* h);

@@ -120,20 +120,37 @@ struct TextLnArgs {
 };
 bool text_ln_supported(int d);
 void text_ln(const TextLnArgs& a, cudaStream_t st);
-// --- bidirectional GRU of the T2M evaluator (gru_tc.cu) ---
-// State buffers are [2 * rows_pad, H]: direction d's row m at d * rows_pad + m (rows_pad a multiple of 128).
+// --- the GRUs of the T2M evaluator (bidirectional) and of the action classifier (unidirectional, gru_tc.cu) ---
+// State buffers are [dirs * rows_pad, H]: direction d's row m at d * rows_pad + m (rows_pad a multiple of 128).
 struct GruStepArgs {
   ActBuf h_in{}, h_out{};              // split16 state h_{s-1} (the MMA operand) / h_s
   const float* hf_in = nullptr;        // fp32 state h_{s-1} (the z * h term and the copy-through)
   float* hf_out = nullptr;
-  const float* gi = nullptr;           // [rows * L, 6H]: x_t W_ih^T + b_ih, forward then backward, gates r | z | n
-  const float* gh = nullptr;           // CUDA-core path: [2 * rows_pad, 3H] h W_hh^T in the packed column order
-  const float* b_hh = nullptr;         // [2][3H] fp32, gates r | z | n
+  const float* gi = nullptr;           // [rows * L, dirs * 3H]: x_t W_ih^T + b_ih, forward then backward, gates r | z | n
+  const float* gh = nullptr;           // CUDA-core path: [dirs * rows_pad, 3H] h W_hh^T in the packed column order
+  const float* b_hh = nullptr;         // [dirs][3H] fp32, gates r | z | n
   const int32_t* lengths = nullptr;    // [rows] valid steps per sequence (clamped to [0, L])
-  const __half* w_hh = nullptr;        // packed W_hh planes [2][2 * 3H][H] (gru_packed_col order)
+  const __half* w_hh = nullptr;        // packed W_hh planes [2][dirs * 3H][H] (gru_packed_col order)
   int64_t w_plane_stride = 0;
   float w_inv_scale = 1.0f;
   int rows = 0, rows_pad = 0, L = 0, H = 0, step = 0;
+  int dirs = 2;                        // 2: bidirectional (k_gru_step_tc's only layout); 1: forward only
+  int64_t h0_ld = 0;                   // initial state of (dir, row m) at h0[dir * H + m * h0_ld]: 0 broadcasts one vector
+  ActBuf seq_out{};                    // CUDA-core gates, dirs == 1: h_s also goes to split16 row m * L + t (hi null: not)
+};
+// One unidirectional layer of the action classifier over every step (k_gru_seq_tc).  The split16 W_hh of the layer
+// stays in shared memory for the whole launch; each warpgroup carries a 64-row tile through all L steps.
+struct GruSeqArgs {
+  const float* gi = nullptr;           // [rows * L, 3H]: x_t W_ih^T + b_ih, gates r | z | n; only t < len is read
+  const float* b_hh = nullptr;         // [3H] fp32, gates r | z | n
+  const float* h0 = nullptr;           // [rows, H] fp32, each row's own initial state
+  const int32_t* lengths = nullptr;    // [rows], each in [1, L] (clamped to [0, L])
+  const __half* w_hh = nullptr;        // packed W_hh planes [2][3H][H] (gru_packed_col order)
+  int64_t w_plane_stride = 0;
+  float w_inv_scale = 1.0f;
+  ActBuf seq_out{};                    // not the last layer: h_t (t < len) as split16 row m * L + t (hi null: not written)
+  float* h_last = nullptr;             // the last layer: [rows, H] fp32 h at t = len - 1 (null: not written)
+  int rows = 0, L = 0, H = 0;
 };
 // column of gate g (0 r, 1 z, 2 n) of hidden unit u inside one direction's 3H packed rows: 32-unit tiles of 96 rows,
 // 8-row group 3 * jj + g holds units 8 * jj .. 8 * jj + 7 of the tile
@@ -145,7 +162,10 @@ bool gru_tc_init();                                              // per device, 
 bool gru_shape_supported(int H);                                 // 64 <= H <= 1024, H % 64 == 0
 bool gru_step_tc(const GruStepArgs& a, cudaStream_t st);         // false: tensor-map encoding failed, nothing launched
 void gru_gate_simt(const GruStepArgs& a, cudaStream_t st);       // the gate update from a.gh (CUDA cores)
-void gru_init_state(const GruStepArgs& a, const float* h0, cudaStream_t st);   // h_out / hf_out = h0 [2][H] per row
+void gru_init_state(const GruStepArgs& a, const float* h0, cudaStream_t st);   // h_out / hf_out = h0 (see h0_ld)
+bool gru_seq_supported(int H);                                   // H = 64 or 128: W_hh fits in shared memory
+// at most sm_count CTAs; false: tensor-map encoding failed, nothing launched
+bool gru_seq_tc(const GruSeqArgs& a, int sm_count, cudaStream_t st);
 // Conv1d(k = 4, stride 2, padding 1) im2col: src [rows / T_out sequences][T_in][ld] fp32 -> X [rows, 4 * Cp] split16
 void im2col_k4s2(ActBuf X, const float* src, int64_t ld, int T_in, int C, int Cp, int T_out, int rows, cudaStream_t st);
 // --- wgmma implementations (gemm_tc.cu) ---

@@ -245,6 +245,34 @@ class Engine:
               "mldb_t2m_text")
         return out
 
+    # ------------------------------------------------------------------ HumanAct12 action classifier
+    def a2m_configure(self, acfg):
+        """Add the classifier's keys (``gru_classifier.`` prefix) to the strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_a2m_configure(self._h, C.byref(acfg)), "mldb_a2m_configure")
+        self.a2m_cfg = acfg
+
+    def a2m_classify(self, x: torch.Tensor, lengths, h0: torch.Tensor):
+        """MotionDiscriminator with an explicit initial state: x [B, input_size, T] (or [B, njoints, nfeats, T]),
+        lengths (each in [1, T]), h0 [hidden_layer, B, hidden_size] -> (logits [B, output_size], features [B, 30])."""
+        ac = getattr(self, "a2m_cfg", None)
+        if ac is None:
+            raise RuntimeError("the action classifier was not configured (a2m_configure) before finalize()")
+        if x.dim() == 4:
+            x = x.reshape(x.shape[0], x.shape[1] * x.shape[2], x.shape[3])
+        if x.dim() != 3 or x.shape[1] != ac.input_size or x.shape[0] < 1 or x.shape[2] < 1:
+            raise ValueError(f"x must be [B >= 1, {ac.input_size}, T >= 1], got {tuple(x.shape)}")
+        xd = _f32c(x, self.device)
+        B, T = xd.shape[0], xd.shape[2]
+        if tuple(h0.shape) != (ac.hidden_layer, B, ac.hidden_size):
+            raise ValueError(f"h0 must be [{ac.hidden_layer}, {B}, {ac.hidden_size}], got {tuple(h0.shape)}")
+        ln = self._t2m_lengths(lengths, B, T)
+        hd = _f32c(h0, self.device)
+        logits = torch.empty((B, ac.output_size), dtype=torch.float32, device=self.device)
+        feats = torch.empty((B, 30), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_a2m_classify(self._h, _ptr(xd), _ptr(ln), _ptr(hd), B, T, _ptr(logits), _ptr(feats),
+                                         self._stream()), "mldb_a2m_classify")
+        return logits, feats
+
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:
         """Which kernel each operator was enqueued on since the last reset (mldb_kernel_stats)."""
         arr = (C.c_int64 * len(_lib.KSTAT_NAMES))()

@@ -9,6 +9,12 @@ MultiModality:
 Same ctor kwargs, same ``state_dict`` keys and shapes (``hidden`` included, so finest.tar's dicts load with
 ``strict=True``), same forward signatures and return shapes; the math runs in ``libmldb200.so``.  Inference only.
 Like ``pack_padded_sequence``, the GRU encoders refuse lengths that are zero or not in decreasing order.
+
+And for the HumanAct12 action classifier of ``HUMANACTMetrics`` (mld/models/metrics/gru.py:32-36), whose logits feed
+the action model's accuracy and whose features feed its FID, diversity and multimodality:
+
+    gru_classifier:         mld_b200.evaluator.B200MotionDiscriminator        (was humanact12_gru.MotionDiscriminator)
+    gru_classifier_for_fid: mld_b200.evaluator.B200MotionDiscriminatorForFID  (was ...MotionDiscriminatorForFID)
 """
 from __future__ import annotations
 
@@ -88,3 +94,61 @@ class B200MotionEncoderBiGRUCo(_T2mModule):
     def forward(self, inputs: torch.Tensor, m_lens) -> torch.Tensor:
         _lengths(m_lens, inputs.shape[0], inputs.shape[1])
         return self.engine().t2m_motion(inputs, m_lens)
+
+
+class B200MotionDiscriminator(_EngineModule):
+    """``MotionDiscriminator`` (mld/models/architectures/humanact12_gru.py:6-55): nn.GRU(input_size, hidden_size,
+    hidden_layer), the output at ``lengths - 1``, Linear(hidden_size, 30), tanh, Linear(30, output_size).
+
+    ``hidden_unit=None`` draws the initial state exactly as the reference does (``torch.randn(layer, bs, H)`` on the
+    CPU default generator, then ``.to(device)``), so a seeded caller draws the same states in the same order.
+    Every length must lie in [1, T]: the reference wraps a zero length around to the last frame (``gru_o[-1]``),
+    which is not reproduced; such lengths raise before anything runs.  ``use_noise`` is kept and unused, as there."""
+    _prefix = "gru_classifier."
+
+    def __init__(self, input_size: int, hidden_size: int, hidden_layer: int, output_size: int = 12, use_noise=None):
+        super().__init__()
+        self.input_size = input_size
+        self.hidden_size = hidden_size
+        self.hidden_layer = hidden_layer
+        self.use_noise = use_noise
+        cfg = _lib.default_a2m_config()
+        cfg.input_size, cfg.hidden_size, cfg.hidden_layer, cfg.output_size = input_size, hidden_size, hidden_layer, output_size
+        self._a2m_cfg = cfg
+        _register_tree(self, synth.a2m_state_dict(seed=0, input_size=input_size, hidden_size=hidden_size,
+                                                   hidden_layer=hidden_layer, output_size=output_size))
+
+    def _make_config(self):
+        return make_config(num_layers=0, vae="none")            # a handle that holds only the classifier
+
+    def _configure_engine(self, eng):
+        eng.a2m_configure(self._a2m_cfg)
+
+    def initHidden(self, num_samples: int, layer: int) -> torch.Tensor:
+        return torch.randn(layer, num_samples, self.hidden_size, requires_grad=False)
+
+    def _classify(self, motion_sequence: torch.Tensor, lengths, hidden_unit):
+        bs, njoints, nfeats, num_frames = motion_sequence.shape
+        if lengths is None:
+            raise ValueError("lengths is required (the reference indexes the GRU output with lengths - 1)")
+        ln = torch.as_tensor(lengths).reshape(-1)
+        if ln.numel() != bs:
+            raise ValueError(f"expected {bs} lengths, got {ln.numel()}")
+        if ln.dtype.is_floating_point or ln.dtype == torch.bool:
+            raise ValueError("lengths must be integers")
+        if int(ln.min()) < 1 or int(ln.max()) > num_frames:
+            raise ValueError(f"lengths must lie in [1, {num_frames}] (a zero length is not wrapped to the last frame)")
+        x = motion_sequence.reshape(bs, njoints * nfeats, num_frames)
+        if hidden_unit is None:
+            hidden_unit = self.initHidden(bs, self.hidden_layer).to(motion_sequence.device)
+        return self.engine().a2m_classify(x, ln, hidden_unit)
+
+    def forward(self, motion_sequence: torch.Tensor, lengths=None, hidden_unit=None) -> torch.Tensor:
+        return self._classify(motion_sequence, lengths, hidden_unit)[0]
+
+
+class B200MotionDiscriminatorForFID(B200MotionDiscriminator):
+    """``MotionDiscriminatorForFID`` (humanact12_gru.py:58-85): the 30-d ``tanh(linear1)`` features."""
+
+    def forward(self, motion_sequence: torch.Tensor, lengths=None, hidden_unit=None) -> torch.Tensor:
+        return self._classify(motion_sequence, lengths, hidden_unit)[1]

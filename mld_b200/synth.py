@@ -322,3 +322,40 @@ def renorm4t2m(feats: Tensor, mean: Tensor, std: Tensor, mean_eval: Tensor, std_
     """HumanML3DDataModule.renorm4t2m (mld/data/HumanML3D.py:54-62)."""
     feats = feats * std.to(feats) + mean.to(feats)
     return (feats - mean_eval.to(feats)) / std_eval.to(feats)
+
+
+A2M_DIMS = {"input_size": 72, "hidden_size": 128, "hidden_layer": 2, "output_size": 12}   # metrics/gru.py:32-36
+
+
+def a2m_state_dict(seed: int = 1357, **dims) -> Dict[str, Tensor]:
+    """``MotionDiscriminator``'s state dict (the keys of HumanAct12's ``a2m_checkpoint["model"]``), shaped by
+    ``A2M_DIMS``, with torch's default init: GRU weights and biases U(-1/sqrt(H), 1/sqrt(H)), Linear
+    U(-1/sqrt(fan_in), 1/sqrt(fan_in))."""
+    d = {**A2M_DIMS, **dims}
+    g = _Gen(seed)
+    H = d["hidden_size"]
+    b = 1.0 / math.sqrt(H)
+    sd: Dict[str, Tensor] = {}
+    for k in range(d["hidden_layer"]):
+        sd[f"recurrent.weight_ih_l{k}"] = _t2m_uniform(g, b, 3 * H, d["input_size"] if k == 0 else H)
+        sd[f"recurrent.weight_hh_l{k}"] = _t2m_uniform(g, b, 3 * H, H)
+        sd[f"recurrent.bias_ih_l{k}"] = _t2m_uniform(g, b, 3 * H)
+        sd[f"recurrent.bias_hh_l{k}"] = _t2m_uniform(g, b, 3 * H)
+    _t2m_linear(sd, g, "linear1.", 30, H)
+    _t2m_linear(sd, g, "linear2.", d["output_size"], 30)
+    return sd
+
+
+def a2m_motions(B: int, T: int = 60, seed: int = 21, njoints: int = 24, nfeats: int = 3) -> Tensor:
+    """Smooth synthetic joint trajectories ``[B, njoints, nfeats, T]`` (what ``feats2joints_eval`` hands the
+    classifier): a per-joint offset of ~0.5 m plus three sinusoids per coordinate with random frequency and phase."""
+    g = torch.Generator().manual_seed(seed)
+    t = torch.arange(T, dtype=torch.float32) / 30.0                          # 30 fps
+    base = torch.randn(B, njoints, nfeats, 1, generator=g) * 0.5
+    x = base.expand(B, njoints, nfeats, T).clone()
+    for _ in range(3):
+        amp = torch.rand(B, njoints, nfeats, 1, generator=g) * 0.2
+        freq = 0.2 + torch.rand(B, njoints, nfeats, 1, generator=g) * 2.0
+        phase = torch.rand(B, njoints, nfeats, 1, generator=g) * 2 * math.pi
+        x = x + amp * torch.sin(2 * math.pi * freq * t + phase)
+    return x
