@@ -404,6 +404,38 @@ int mldb_a2m_configure(mldb_handle* h, const mldb_a2m_config* cfg);
 int mldb_a2m_classify(mldb_handle* h, const float* x, const int32_t* lengths, const float* h0, int32_t B, int32_t T,
                       float* logits, float* features, void* stream);
 
+/* ---- UESTC action classifier (UESTCMetrics, mld/models/metrics/stgcn.py): STGCN (mld/models/architectures/
+ * uestc_stgcn.py) with layout "smpl", strategy "spatial" and edge importance weighting, whose yhat feeds the action
+ * model's accuracy and whose pooled features feed its FID, diversity and multimodality.  data_bn -> ten st_gcn blocks
+ * (64, 64, 64, 64, 128/s2, 128, 128, 256/s2, 256, 256 channels) -> the mean over (T_out, 24) -> fcn (1 x 1 conv).
+ * Keys (strict, 172 with the defaults) under "stgcn_classifier.": A [3, 24, 24]; edge_importance.{0..9} [3, 24, 24];
+ * data_bn.{weight,bias,running_mean,running_var} [24 in_channels] and data_bn.num_batches_tracked (0-d, value
+ * ignored); for each block i, st_gcn_networks.{i}.gcn.conv.weight [3 C_out, C_in, 1, 1] / .bias [3 C_out],
+ * .tcn.0.* and .tcn.3.* (BatchNorm2d(C_out), the same five keys), .tcn.2.weight [C_out, C_out, 9, 1] / .bias [C_out],
+ * and for i = 4, 7 .residual.0.weight [C_out, C_in, 1, 1] / .bias [C_out] and .residual.1.* (BatchNorm2d(C_out));
+ * fcn.weight [num_class, 256, 1, 1], fcn.bias [num_class].  Every BatchNorm is applied in eval mode (eps 1e-5). */
+#define MLDB_STGCN_ABI_VERSION 1
+typedef struct mldb_stgcn_config {
+  int32_t abi_version;        /* must be MLDB_STGCN_ABI_VERSION */
+  int32_t in_channels;        /* 6 (rot6d); 1 .. 64 */
+  int32_t num_class;          /* 40 UESTC actions; 1 .. 4096 */
+} mldb_stgcn_config;
+void mldb_default_stgcn_config(mldb_stgcn_config* cfg);
+/* Add the classifier's keys to the strict key spec; after mldb_create, before mldb_finalize_weights. */
+int mldb_stgcn_configure(mldb_handle* h, const mldb_stgcn_config* cfg);
+/* Replaces: STGCN.forward.
+ *   x         [B, 24, in_channels, T] fp32, contiguous (the reference's `motion`)
+ *   yhat      [B, num_class] (may be NULL);  features  [B, 256], the pooled features (may be NULL)
+ * Padding frames are computed like any other frame (there is no mask, as in the reference).  Runs eagerly on
+ * `stream` in batch chunks that bound the workspace (which grows on demand, outside any capture, and synchronises
+ * the device when it does); every sequence is computed independently of the others and of the chunking.
+ * Kernels per chunk: for each of the ten blocks one graph mix (MLDB_KSTAT_MISC), one gcn GEMM and one k_tconv_tc
+ * temporal convolution (both MLDB_KSTAT_GEMM_TC), then one head (MISC): 20 GEMM_TC + 11 MISC.  With gemm=simt, each
+ * block runs the mix, the gcn GEMM, an im2col, the temporal-convolution GEMM and a residual + ReLU kernel: 20
+ * GEMM_SIMT + 31 MISC per chunk. */
+int mldb_stgcn_classify(mldb_handle* h, const float* x, int32_t B, int32_t T, float* yhat, float* features,
+                        void* stream);
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);
@@ -412,7 +444,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
 /* Which kernel every operator of the path was ENQUEUED on since the last reset (recorded launches: a CUDA
  * graph counts once, at capture).  out: HOST int64[MLDB_KSTAT_COUNT], index = MLDB_KSTAT_*.  Lets a caller
  * (and the tests) assert that nothing fell back from the wgmma kernels to the CUDA-core kernels. */
-#define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue; k_proj_tc (its K = 256 split16 projections) */
+#define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue; k_proj_tc (its K = 256 split16 projections);
+                                     k_tconv_tc (the UESTC classifier's temporal convolutions) */
 #define MLDB_KSTAT_GEMM_LN_TC 1   /* k_gemm_tc, fused residual + LayerNorm epilogue */
 #define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block; in the encoder layers it also runs the folded
                                      out-projection + residual + LayerNorm in front of the FFN) */
@@ -443,6 +476,7 @@ int mldb_reset_kernel_stats(mldb_handle* h);
  *   "graph"      0 | 1                  CUDA-graph replay of the step loop (1)                        MLDB_GRAPH
  *   "t2m_chunk"  0 | n                  T2M evaluator: sequences per batch chunk (0: sized from the workspace budget)
  *   "a2m_chunk"  0 | n                  action classifier: sequences per batch chunk (0: from the workspace budget)
+ *   "stgcn_chunk" 0 | n                 UESTC classifier: sequences per batch chunk (0: from the workspace budget)
  * Environment only: MLDB_PDL (programmatic dependent launch, 1); MLDB_SNAKE (1: attention and the fused FFN walk
  * the token tiles downwards, the GEMMs upwards, so every kernel starts on the rows its producer wrote last). */
 int mldb_set_option(mldb_handle* h, const char* name, const char* value);

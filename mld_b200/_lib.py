@@ -31,6 +31,8 @@ MLDB_T2M_ABI_VERSION = 1
 T2M_TEXT, T2M_MOVEMENT, T2M_MOTION = 1, 2, 4
 # HumanAct12 action classifier (mldb_a2m_config, mldb_a2m_classify)
 MLDB_A2M_ABI_VERSION = 1
+# UESTC action classifier (mldb_stgcn_config, mldb_stgcn_classify)
+MLDB_STGCN_ABI_VERSION = 1
 
 
 class MldbConfig(C.Structure):
@@ -78,6 +80,11 @@ class MldbA2mConfig(C.Structure):
     ]
 
 
+class MldbStgcnConfig(C.Structure):
+    """``mldb_stgcn_config`` (include/mldb.h)."""
+    _fields_ = [("abi_version", C.c_int32), ("in_channels", C.c_int32), ("num_class", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/mldb.h declares
 _P = C.c_void_p
 _SIGNATURES = {
@@ -120,6 +127,9 @@ _SIGNATURES = {
     "mldb_default_a2m_config": (None, [C.POINTER(MldbA2mConfig)]),
     "mldb_a2m_configure": (C.c_int, [_P, C.POINTER(MldbA2mConfig)]),
     "mldb_a2m_classify": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
+    "mldb_default_stgcn_config": (None, [C.POINTER(MldbStgcnConfig)]),
+    "mldb_stgcn_configure": (C.c_int, [_P, C.POINTER(MldbStgcnConfig)]),
+    "mldb_stgcn_classify": (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
@@ -184,4 +194,10 @@ def default_t2m_config() -> MldbT2mConfig:
 def default_a2m_config() -> MldbA2mConfig:
     cfg = MldbA2mConfig()
     lib().mldb_default_a2m_config(C.byref(cfg))
+    return cfg
+
+
+def default_stgcn_config() -> MldbStgcnConfig:
+    cfg = MldbStgcnConfig()
+    lib().mldb_default_stgcn_config(C.byref(cfg))
     return cfg

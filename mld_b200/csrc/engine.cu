@@ -1,6 +1,6 @@
 // libmldb200 engine: handles and their options, the state-dict spec and weight packing of the sampling models,
 // scheduler tables, plans and CUDA-graph capture.  The models' forward passes live in stack.cu (transformer stacks),
-// denoiser.cu, vae.cu, text_tower.cu, t2m.cu and a2m.cu.
+// denoiser.cu, vae.cu, text_tower.cu, t2m.cu, a2m.cu and stgcn.cu.
 #include "engine.h"
 
 #include <math.h>
@@ -413,7 +413,8 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   if (e != cudaSuccess) { delete h; FAIL(MLDB_ERR_CUDA, "cudaStreamCreate: %s", cudaGetErrorString(e)); }
   // kernel setup, on this handle's device (the shared-memory opt-ins apply per device): each step records its own
   // message in mldb_last_error() when it fails
-  if (!simt_init() || !mma_attention_init() || !tc_attention_init() || !gru_tc_init()) { delete h; return MLDB_ERR_CUDA; }
+  if (!simt_init() || !mma_attention_init() || !tc_attention_init() || !gru_tc_init() ||
+      !tconv_tc_init()) { delete h; return MLDB_ERR_CUDA; }
   h->tc = tc_create(device);
   if (!h->tc) { delete h; return MLDB_ERR_CUDA; }
   const char* env = getenv("MLDB_GEMM");
@@ -488,6 +489,8 @@ extern "C" int mldb_set_option(mldb_handle* h, const char* name, const char* val
     h->t2m.chunk = std::max(atoi(value), 0);
   } else if (!strcmp(name, "a2m_chunk")) {
     h->a2m.chunk = std::max(atoi(value), 0);
+  } else if (!strcmp(name, "stgcn_chunk")) {
+    h->stgcn.chunk = std::max(atoi(value), 0);
   } else {
     FAIL(MLDB_ERR_INVALID, "unknown option %s", name);
   }
@@ -503,7 +506,7 @@ extern "C" int64_t mldb_launch_count(const mldb_handle* h) { return h ? h->launc
 // ----------------------------------------------------------------------------- weights
 extern "C" int mldb_load_tensor(mldb_handle* h, const char* key, const void* data,
                                 const int64_t* shape, int32_t ndim, int32_t dtype) {
-  if (!h || !key || !data || !shape) FAIL(MLDB_ERR_INVALID, "null argument");
+  if (!h || !key || !data || (!shape && ndim != 0)) FAIL(MLDB_ERR_INVALID, "null argument");
   if (dtype != MLDB_DTYPE_F32) FAIL(MLDB_ERR_UNSUPPORTED, "only fp32 tensors are accepted");
   if (h->finalized) FAIL(MLDB_ERR_STATE, "weights already finalized");
   auto it = h->raw.find(key);
@@ -588,6 +591,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
   if (h->text.on) TRY(pack_text(h));
   if (h->t2m.on) TRY(pack_t2m(h));
   if (h->a2m.on) TRY(pack_a2m(h));
+  if (h->stgcn.on) TRY(pack_stgcn(h));
   for (auto& kv : h->raw) { kv.second.host.clear(); kv.second.host.shrink_to_fit(); }
   h->finalized = true;
   return MLDB_OK;

@@ -160,6 +160,30 @@ struct A2mW {
   GrowBuf h_split, h_f32, gh;     // gemm=simt: state ping-pong (split16, fp32), h W_hh^T
 };
 
+// UESTC action classifier (mldb_stgcn_configure): STGCN (uestc_stgcn.py), ten st_gcn blocks
+constexpr int kStgcnBlocks = 10;
+struct StgcnBlockW {
+  LinW gcn;                       // [C_out, 3 C_in] (K padded to 64): the 1 x 1 conv with BN1 folded, column k C_in + ci
+  float* gcn_tab = nullptr;       // [24, C_out] fp32: the gcn bias through the graph, + BN1's shift, per joint
+  LinW tcn;                       // [C_out, 9 C_out (+ C_in)]: the (9, 1) conv tap-major with BN2 folded (+ the
+                                  // residual 1 x 1 conv with its BN folded); bias: both biases and shifts
+};
+struct StgcnW {
+  bool on = false;
+  mldb_stgcn_config cfg{};
+  StgcnBlockW blocks[kStgcnBlocks];
+  float* adj = nullptr;           // [10][3][24][24] fp32: A * edge_importance[i]
+  float *bn_scale = nullptr, *bn_shift = nullptr;   // data_bn [24 * in_channels], channel v * in_channels + c
+  float *fcn_w = nullptr, *fcn_b = nullptr;         // [num_class, 256], [num_class]
+  int chunk = 0;                  // option stgcn_chunk (0: from the workspace budget)
+  // workspace of mldb_stgcn_classify
+  GrowBuf z;                      // split16 [n * T * 24, 3 C_in (padded to 64)]: the graph mix, the gcn GEMM's A
+  GrowBuf y;                      // split16 [n * T * 24, C_out]: the gcn output, the temporal convolution's input
+  GrowBuf x[2];                   // split16 block outputs (ping-pong)
+  GrowBuf last;                   // fp32 [n * T_out * 24, 256]: the last block's output
+  GrowBuf col, acc;               // gemm=simt: the temporal convolution's im2col (split16) and its fp32 GEMM output
+};
+
 struct RawTensor {
   std::vector<float> host;
   std::vector<int64_t> shape;
@@ -243,6 +267,7 @@ struct mldb_handle {
   TextW text;          // CLIP text tower (mldb_text_configure)
   T2mW t2m;            // T2M evaluator (mldb_t2m_configure)
   A2mW a2m;            // HumanAct12 action classifier (mldb_a2m_configure)
+  StgcnW stgcn;        // UESTC action classifier (mldb_stgcn_configure)
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;
@@ -358,10 +383,11 @@ int dec_plan(mldb_handle* h, int B, int T, Plan** out);
 int run_decode(mldb_handle* h, const float* z, const int32_t* lengths, int B, int T, float* feats_out, cudaStream_t st,
                Plan** plan_out);
 int run_f2j(mldb_handle* h, const float* feats, int B, int T, float* joints, cudaStream_t st);
-// text_tower.cu, t2m.cu, a2m.cu
+// text_tower.cu, t2m.cu, a2m.cu, stgcn.cu
 int pack_text(mldb_handle* h);
 int pack_t2m(mldb_handle* h);
 int pack_a2m(mldb_handle* h);   // a2m.cu
+int pack_stgcn(mldb_handle* h); // stgcn.cu
 
 // comm.cu
 void mldb_comm_release(mldb_handle* h);

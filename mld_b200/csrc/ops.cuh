@@ -168,5 +168,25 @@ bool gru_seq_supported(int H);                                   // H = 64 or 12
 bool gru_seq_tc(const GruSeqArgs& a, int sm_count, cudaStream_t st);
 // Conv1d(k = 4, stride 2, padding 1) im2col: src [rows / T_out sequences][T_in][ld] fp32 -> X [rows, 4 * Cp] split16
 void im2col_k4s2(ActBuf X, const float* src, int64_t ld, int T_in, int C, int Cp, int T_out, int rows, cudaStream_t st);
+// --- the ST-GCN's temporal convolution (tconv_tc.cu) ---
+// One st_gcn block's tcn + residual + ReLU over activations laid out [nseq][T][24 joints][C] (split16 rows
+// (n * T + t) * 24 + v), as an implicit GEMM with K = 9 taps x C (+ C_res for a residual convolution):
+//   out[(n, t, v), c] = relu( sum_{tap, ci} x[(n, s t + tap - 4, v), ci] W[c, tap C + ci] * inv_scale
+//                             (+ sum_cr res[(n, s t, v), cr] W[c, 9 C + cr] * inv_scale) + bias[c] (+ res[(n, t, v), c]) )
+// Frames outside [0, T_in) read as zero (the convolution's padding).
+struct TconvArgs {
+  ActBuf x{};                          // split16 [nseq * T_in * 24, C]: the block's gcn output
+  ActBuf res{};                        // split16 [nseq * T_in * 24, C_res]: the block input (hi null: no residual)
+  int res_conv = 0;                    // 1: res goes through the 1 x 1 stride-s convolution (W's tenth K segment);
+                                       // 0: res is added as it is (C_res == C, stride 1)
+  LinW w{};                            // [C, 9 C (+ C_res)] tap-major, every BatchNorm folded; bias [C]
+  int nseq = 0, T_in = 0, T_out = 0, C = 0, C_res = 0, stride = 1;
+  ActBuf out{};                        // split16 [nseq * T_out * 24, C] (hi null: out_f32)
+  float* out_f32 = nullptr;            // fp32 [nseq * T_out * 24, C]
+};
+bool tconv_tc_init();                                            // per device, outside stream capture
+bool tconv_tc_supported(const TconvArgs& a);                     // C in {64, 128, 256}, C_res % 64 == 0, stride 1 | 2
+// at most sm_count CTAs; false: tensor-map encoding failed, nothing launched
+bool tconv_tc(const TconvArgs& a, int sm_count, cudaStream_t st);
 // --- wgmma implementations (gemm_tc.cu) ---
 struct TcCtx;

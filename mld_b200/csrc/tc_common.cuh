@@ -80,6 +80,13 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2,
+                                            int c3) {
+  asm volatile(
+      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+      : "memory");
+}
 // pull one box of a tensor into L2 (no shared-memory destination, no barrier): issued one tile ahead so that
 // the real TMA loads of a shallow ring hit L2 instead of paying the HBM latency
 __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, int c1) {
@@ -378,14 +385,16 @@ inline PFN_tmapEncodeTiled tmap_encoder() {
 // A tensor map of one split16 plane (fp16, columns contiguous): boxes of 64 columns (one 128B swizzle row) x
 // box[1] rows, SWIZZLE_128B, L2 256B promotion, and elements outside the plane zero-filled - so M and N need not
 // be tile multiples, and a box never brings in rows of another sequence (DESIGN §2).  dims / strides / box are
-// innermost first.  false: encoding failed and mldb_last_error() names the plane.
+// innermost first; rank <= 5.  estr: the traversal stride of each dimension (nullptr: all 1); a box then holds
+// ceil(box[i] / estr[i]) elements along dimension i, every estr[i]-th one from the load's start coordinate.
+// false: encoding failed and mldb_last_error() names the plane.
 inline bool encode_plane_map(CUtensorMap* m, const __half* base, int rank, const cuuint64_t* dims,
-                             const cuuint64_t* strides, const cuuint32_t* box) {
+                             const cuuint64_t* strides, const cuuint32_t* box, const cuuint32_t* estr = nullptr) {
   const PFN_tmapEncodeTiled encode = tmap_encoder();
   if (!encode) return false;
-  const cuuint32_t estr[3] = {1, 1, 1};
+  const cuuint32_t ones[5] = {1, 1, 1, 1, 1};
   const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, (void*)base, dims, strides, box,
-                            estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+                            estr ? estr : ones, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                             CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     std::string shape;

@@ -273,6 +273,28 @@ class Engine:
                                          self._stream()), "mldb_a2m_classify")
         return logits, feats
 
+    # ------------------------------------------------------------------ UESTC action classifier
+    def stgcn_configure(self, scfg):
+        """Add the classifier's keys (``stgcn_classifier.`` prefix) to the strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_stgcn_configure(self._h, C.byref(scfg)), "mldb_stgcn_configure")
+        self.stgcn_cfg = scfg
+
+    def stgcn_classify(self, motion: torch.Tensor):
+        """STGCN: motion [B, 24, in_channels, T] -> (yhat [B, num_class], features [B, 256])."""
+        sc = getattr(self, "stgcn_cfg", None)
+        if sc is None:
+            raise RuntimeError("the UESTC classifier was not configured (stgcn_configure) before finalize()")
+        if motion.dim() != 4 or motion.shape[0] < 1 or motion.shape[1] != 24 or motion.shape[2] != sc.in_channels \
+                or motion.shape[3] < 1:
+            raise ValueError(f"motion must be [B >= 1, 24, {sc.in_channels}, T >= 1], got {tuple(motion.shape)}")
+        xd = _f32c(motion, self.device)
+        B, T = xd.shape[0], xd.shape[3]
+        yhat = torch.empty((B, sc.num_class), dtype=torch.float32, device=self.device)
+        feats = torch.empty((B, 256), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_stgcn_classify(self._h, _ptr(xd), B, T, _ptr(yhat), _ptr(feats), self._stream()),
+              "mldb_stgcn_classify")
+        return yhat, feats
+
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:
         """Which kernel each operator was enqueued on since the last reset (mldb_kernel_stats)."""
         arr = (C.c_int64 * len(_lib.KSTAT_NAMES))()

@@ -15,6 +15,11 @@ the action model's accuracy and whose features feed its FID, diversity and multi
 
     gru_classifier:         mld_b200.evaluator.B200MotionDiscriminator        (was humanact12_gru.MotionDiscriminator)
     gru_classifier_for_fid: mld_b200.evaluator.B200MotionDiscriminatorForFID  (was ...MotionDiscriminatorForFID)
+
+And for the UESTC action classifier of ``UESTCMetrics`` (mld/models/metrics/stgcn.py:32), whose yhat feeds the action
+model's accuracy and whose pooled features feed its FID, diversity and multimodality:
+
+    stgcn_classifier:       mld_b200.evaluator.B200STGCN                      (was uestc_stgcn.STGCN)
 """
 from __future__ import annotations
 
@@ -152,3 +157,68 @@ class B200MotionDiscriminatorForFID(B200MotionDiscriminator):
 
     def forward(self, motion_sequence: torch.Tensor, lengths=None, hidden_unit=None) -> torch.Tensor:
         return self._classify(motion_sequence, lengths, hidden_unit)[1]
+
+
+class B200STGCN(_EngineModule):
+    """``STGCN`` (mld/models/architectures/uestc_stgcn.py:8-130), the UESTC action classifier of ``UESTCMetrics``
+    (mld/models/metrics/stgcn.py:32-40): data_bn, ten st_gcn blocks over the SMPL graph, a global average pool and a
+    1 x 1 convolution head.  Same constructor kwargs; ``A`` is built from ``kintree_path`` with the same spatial
+    partition, so a fresh module equals the reference before loading.  Same 172 state-dict keys, shapes and dtypes
+    (``A``, the running statistics and ``num_batches_tracked`` are buffers), so ``uestc_rot6d_stgcn.tar`` loads with
+    ``strict=True``.  ``forward`` returns ``{"output", "features", "yhat"}`` with the reference's squeeze.  Only the
+    ``smpl`` layout, the ``spatial`` strategy and edge importance weighting are implemented; anything else raises
+    ``ValueError`` at construction, as does a motion of another joint or channel count, or with no frame."""
+    _prefix = "stgcn_classifier."
+    _BUFFERS = ("A", "running_mean", "running_var", "num_batches_tracked")
+
+    def __init__(self, in_channels, num_class, kintree_path, graph_args, edge_importance_weighting, **kwargs):
+        super().__init__()
+        ga = dict(graph_args)
+        if ga.get("layout", "openpose") != "smpl" or ga.get("strategy", "uniform") != "spatial":
+            raise ValueError(f"only graph_args layout='smpl', strategy='spatial' is implemented, got {ga}")
+        if ga.get("max_hop", 1) != 1 or ga.get("dilation", 1) != 1:
+            raise ValueError(f"only max_hop = dilation = 1 is implemented, got {ga}")
+        if not edge_importance_weighting:
+            raise ValueError("only edge_importance_weighting=True is implemented")
+        from .graph import smpl_adjacency
+        A = smpl_adjacency(kintree_path)                 # ValueError unless the table describes SMPL's 24 joints
+        self.num_class = num_class
+        self.in_channels = in_channels
+        cfg = _lib.default_stgcn_config()
+        cfg.in_channels, cfg.num_class = in_channels, num_class
+        self._stgcn_cfg = cfg
+        sd = synth.stgcn_state_dict(seed=0, in_channels=in_channels, num_class=num_class)
+        sd["A"] = A
+        bn_init = {"running_mean": 0.0, "running_var": 1.0, "num_batches_tracked": 0}
+        for k in sd:                                     # as the reference initialises them: unit edge importances,
+            if k.startswith("edge_importance."):         # identity BatchNorms
+                sd[k] = torch.ones(3, 24, 24)
+            elif k.rsplit(".", 1)[-1] in bn_init:
+                sd[k] = torch.full_like(sd[k], bn_init[k.rsplit(".", 1)[-1]])
+                if "num_batches_tracked" not in k:
+                    w = k.rsplit(".", 1)[0]
+                    sd[w + ".weight"], sd[w + ".bias"] = torch.ones_like(sd[k]), torch.zeros_like(sd[k])
+        for key, value in sd.items():
+            parts = key.split(".")
+            m = self
+            for p in parts[:-1]:
+                if p not in m._modules:
+                    m.add_module(p, torch.nn.Module())
+                m = m._modules[p]
+            if parts[-1] in self._BUFFERS:
+                m.register_buffer(parts[-1], value.clone())
+            else:
+                m.register_parameter(parts[-1], torch.nn.Parameter(value.clone(), requires_grad=False))
+
+    def _make_config(self):
+        return make_config(num_layers=0, vae="none")            # a handle that holds only the classifier
+
+    def _configure_engine(self, eng):
+        eng.stgcn_configure(self._stgcn_cfg)
+
+    def forward(self, motion: torch.Tensor):
+        if motion.dim() != 4 or motion.shape[1] != 24 or motion.shape[2] != self.in_channels or motion.shape[3] < 1 \
+                or motion.shape[0] < 1:
+            raise ValueError(f"motion must be [B >= 1, 24, {self.in_channels}, T >= 1], got {tuple(motion.shape)}")
+        yhat, features = self.engine().stgcn_classify(motion.contiguous())
+        return {"output": motion, "features": features.squeeze(), "yhat": yhat}

@@ -359,3 +359,79 @@ def a2m_motions(B: int, T: int = 60, seed: int = 21, njoints: int = 24, nfeats: 
         phase = torch.rand(B, njoints, nfeats, 1, generator=g) * 2 * math.pi
         x = x + amp * torch.sin(2 * math.pi * freq * t + phase)
     return x
+
+
+# ---------------------------------------------------------------------------- UESTC action classifier (STGCN)
+STGCN_DIMS = {"in_channels": 6, "num_class": 40}                              # metrics/stgcn.py:32-40
+STGCN_CHANNELS = (64, 64, 64, 64, 128, 128, 128, 256, 256, 256)
+STGCN_STRIDES = (1, 1, 1, 1, 2, 1, 1, 2, 1, 1)
+
+
+def stgcn_residual(i: int, in_channels: int = 6) -> str:
+    """The residual of st_gcn block i: "none" (block 0), "identity", or "conv" (1 x 1 stride-s conv + BN)."""
+    if i == 0:
+        return "none"
+    cin = STGCN_CHANNELS[i - 1]
+    return "identity" if cin == STGCN_CHANNELS[i] and STGCN_STRIDES[i] == 1 else "conv"
+
+
+def _stgcn_bn(sd, g: _Gen, p: str, n: int):
+    """Eval-mode BatchNorm with non-trivial statistics: running_var spread over two decades."""
+    sd[p + "weight"] = 0.5 + g.uniform(n)
+    sd[p + "bias"] = g.normal(n, std=0.1)
+    sd[p + "running_mean"] = g.normal(n, std=0.2)
+    sd[p + "running_var"] = 10.0 ** (g.uniform(n) * 2 - 1)
+    sd[p + "num_batches_tracked"] = torch.tensor(1000, dtype=torch.int64)
+
+
+def stgcn_state_dict(seed: int = 2025, **dims) -> Dict[str, Tensor]:
+    """``STGCN``'s state dict (the keys of ``uestc_rot6d_stgcn.tar``), shaped by ``STGCN_DIMS``: convolutions with
+    torch's default init U(-1/sqrt(fan_in), 1/sqrt(fan_in)), BatchNorms with spread statistics, edge importances in
+    [0.8, 1.2] and ``A`` from SMPL's parent table."""
+    from .graph import smpl_adjacency
+    d = {**STGCN_DIMS, **dims}
+    g = _Gen(seed)
+    cin0 = d["in_channels"]
+    sd: Dict[str, Tensor] = {"A": smpl_adjacency()}
+    _stgcn_bn(sd, g, "data_bn.", 24 * cin0)
+    for i, co in enumerate(STGCN_CHANNELS):
+        ci = STGCN_CHANNELS[i - 1] if i else cin0
+        p = f"st_gcn_networks.{i}."
+        _t2m_linear(sd, g, p + "gcn.conv.", 3 * co, ci)
+        sd[p + "gcn.conv.weight"] = sd[p + "gcn.conv.weight"].reshape(3 * co, ci, 1, 1)
+        _stgcn_bn(sd, g, p + "tcn.0.", co)
+        b = 1.0 / math.sqrt(co * 9)
+        sd[p + "tcn.2.weight"] = _t2m_uniform(g, b, co, co, 9, 1)
+        sd[p + "tcn.2.bias"] = _t2m_uniform(g, b, co)
+        _stgcn_bn(sd, g, p + "tcn.3.", co)
+        if stgcn_residual(i, cin0) == "conv":
+            _t2m_linear(sd, g, p + "residual.0.", co, ci)
+            sd[p + "residual.0.weight"] = sd[p + "residual.0.weight"].reshape(co, ci, 1, 1)
+            _stgcn_bn(sd, g, p + "residual.1.", co)
+    for i in range(len(STGCN_CHANNELS)):
+        sd[f"edge_importance.{i}"] = 0.8 + 0.4 * g.uniform(3, 24, 24)
+    _t2m_linear(sd, g, "fcn.", d["num_class"], 256)
+    sd["fcn.weight"] = sd["fcn.weight"].reshape(d["num_class"], 256, 1, 1)
+    return sd
+
+
+def uestc_motions(B: int, T: int = 60, seed: int = 31, njoints: int = 24) -> Tensor:
+    """Smooth rot6d-like motions ``[B, njoints, 6, T]`` (what ``UESTCMetrics.update`` hands the classifier): per joint,
+    the first two columns of a rotation about a fixed random axis whose angle is an offset plus three sinusoids."""
+    g = torch.Generator().manual_seed(seed)
+    t = torch.arange(T, dtype=torch.float64) / 30.0                          # 30 fps
+    axis = torch.randn(B, njoints, 3, 1, generator=g, dtype=torch.float64)
+    axis = axis / axis.norm(dim=2, keepdim=True)
+    ang = (torch.rand(B, njoints, 1, generator=g, dtype=torch.float64) * 2 - 1) * math.pi
+    for _ in range(3):
+        amp = torch.rand(B, njoints, 1, generator=g, dtype=torch.float64) * 0.5
+        freq = 0.2 + torch.rand(B, njoints, 1, generator=g, dtype=torch.float64) * 2.0
+        phase = torch.rand(B, njoints, 1, generator=g, dtype=torch.float64) * 2 * math.pi
+        ang = ang + amp * torch.sin(2 * math.pi * freq * t + phase)
+    kx, ky, kz = axis[:, :, 0], axis[:, :, 1], axis[:, :, 2]             # [B, J, 1]
+    c, s = torch.cos(ang), torch.sin(ang)                                # [B, J, T]
+    C1 = 1 - c
+    # Rodrigues: the first two columns of R = cI + s[k]x + (1 - c) k k^T
+    col0 = torch.stack([c + kx * kx * C1, kz * s + ky * kx * C1, -ky * s + kz * kx * C1], 2)
+    col1 = torch.stack([-kz * s + kx * ky * C1, c + ky * ky * C1, kx * s + kz * ky * C1], 2)
+    return torch.cat([col0, col1], 2).float()                          # [B, J, 6, T]
