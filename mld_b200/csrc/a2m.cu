@@ -17,9 +17,7 @@ extern "C" void mldb_default_a2m_config(mldb_a2m_config* c) {
 
 extern "C" int mldb_a2m_configure(mldb_handle* h, const mldb_a2m_config* cfg) {
   if (!h || !cfg) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (cfg->abi_version != MLDB_A2M_ABI_VERSION) FAIL(MLDB_ERR_INVALID, "mldb_a2m_config abi_version mismatch");
-  if (h->finalized) FAIL(MLDB_ERR_STATE, "mldb_a2m_configure must precede mldb_finalize_weights");
-  if (h->a2m.on) FAIL(MLDB_ERR_STATE, "the action classifier is already configured");
+  TRY(may_configure(h, cfg->abi_version, MLDB_A2M_ABI_VERSION, h->a2m.on, "a2m", "the action classifier"));
   const mldb_a2m_config& c = *cfg;
   if (c.input_size < 1 || c.input_size > 4096) FAIL(MLDB_ERR_INVALID, "input_size must be in [1, 4096], got %d", c.input_size);
   if (c.output_size < 1 || c.output_size > 4096) FAIL(MLDB_ERR_INVALID, "output_size must be in [1, 4096], got %d", c.output_size);
@@ -126,19 +124,10 @@ __global__ void __launch_bounds__(128) k_a2m_head(const float* __restrict__ hl, 
   }
 }
 
-// sequences per chunk: the option, else what keeps the chunk's workspace near 1 GiB (whole 64-row tiles when > 64)
-static int a2m_chunk(const mldb_handle* h, int B, size_t per_seq) {
-  if (h->a2m.chunk > 0) return std::min(B, h->a2m.chunk);
-  int c = (int)std::max<size_t>(1, ((size_t)1 << 30) / per_seq);
-  if (c > 64) c = c / 64 * 64;
-  return std::min(B, c);
-}
-
 extern "C" int mldb_a2m_classify(mldb_handle* h, const float* x, const int32_t* lengths, const float* h0, int32_t B,
                                  int32_t T, float* logits, float* features, void* stream) {
   if (!h || !x || !lengths || !h0) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (!h->a2m.on) FAIL(MLDB_ERR_STATE, "the action classifier is not configured (mldb_a2m_configure)");
-  if (!h->finalized) FAIL(MLDB_ERR_STATE, "finalize weights first");
+  TRY(check_configured(h, h->a2m.on, "a2m", "the action classifier"));
   const mldb_a2m_config& c = h->a2m.cfg;
   if (B < 1 || T < 1 || (int64_t)B * T > (1 << 26))
     FAIL(MLDB_ERR_INVALID, "classifier input must be [B >= 1, %d, T >= 1] with B * T <= 2^26, got B=%d T=%d", c.input_size, B, T);
@@ -154,61 +143,20 @@ extern "C" int mldb_a2m_classify(mldb_handle* h, const float* x, const int32_t* 
   A2mW& a = h->a2m;
   const int In = c.input_size, Kp = (In + 63) / 64 * 64, H = c.hidden_size, NL = c.hidden_layer;
   const size_t per_seq = (size_t)T * (4 * Kp + 12 * H + (NL > 1 ? 4 * H : 0)) + (size_t)(h->use_tc ? 4 : 40) * H;
-  const int Bc = a2m_chunk(h, B, per_seq);
+  const int Bc = eval_chunk(a.chunk, B, per_seq, 64);
   for (int b0 = 0; b0 < B; b0 += Bc) {
     const int n = std::min(Bc, B - b0), M = n * T;
     ActBuf xs, seq;
     TRY(grow_act(a.x, M, Kp, &xs));
-    TRY(grow(a.gi, (size_t)M * 3 * H * sizeof(float)));
     if (NL > 1) TRY(grow_act(a.seq, M, H, &seq));
-    float* gi = (float*)a.gi.p;
     k_a2m_frames<<<dim3((unsigned)((T + 31) / 32), (unsigned)n), 256, 0, st>>>(xs, x + (int64_t)b0 * In * T, lengths + b0, In, T);
     kcount(h, MLDB_KSTAT_MISC);
     const float* hl = nullptr;                       // the last layer's h at t = len - 1, rows H floats apart
-    for (int l = 0; l < NL; ++l) {
+    for (int l = 0; l < NL; ++l) {                   // each layer but the last writes its h_t into seq
       const A2mLayerW& w = a.layers[l];
       const bool last = l == NL - 1;
-      GemmArgs g; g.a1 = l ? seq : xs; g.K1 = l ? H : Kp; g.M = M; g.w = w.w_ih; g.out_f32 = gi; g.ldc = 3 * H;
-      g.wide_n = 1; g.vec_f32 = 1;
-      op_gemm(h, g, st);                             // gi = x_t W_ih^T + b_ih for every step
-      const float* h0l = h0 + ((int64_t)l * B + b0) * H;
-      if (h->use_tc) {
-        TRY(grow(a.h_last, (size_t)n * H * sizeof(float)));
-        GruSeqArgs s;
-        s.gi = gi; s.b_hh = w.b_hh; s.h0 = h0l; s.lengths = lengths + b0; s.w_hh = w.w_hh.w;
-        s.w_plane_stride = w.w_hh.plane_stride; s.w_inv_scale = w.w_hh.inv_scale; s.rows = n; s.L = T; s.H = H;
-        if (last) s.h_last = (float*)a.h_last.p; else s.seq_out = seq;
-        if (!gru_seq_tc(s, h->sm_count, st)) h->op_failed = true;
-        kcount(h, MLDB_KSTAT_GRU_TC);
-        hl = (float*)a.h_last.p;
-        continue;
-      }
-      // gemm=simt: h W_hh^T on CUDA cores and the gate kernel, one step at a time
-      const int rows_pad = (n + 127) / 128 * 128;
-      const size_t plane = (size_t)rows_pad * H, state_bytes = split16_bytes(rows_pad, H);
-      TRY(grow(a.h_split, 2 * state_bytes));
-      TRY(grow(a.h_f32, 2 * plane * sizeof(float)));
-      TRY(grow(a.gh, plane * 3 * sizeof(float)));
-      float* hf = (float*)a.h_f32.p;
-      auto state = [&](int i) { return split16_at((char*)a.h_split.p + i * state_bytes, rows_pad, H); };
-      GruStepArgs s;
-      s.gi = gi; s.gh = (float*)a.gh.p; s.b_hh = w.b_hh; s.lengths = lengths + b0; s.rows = n; s.rows_pad = rows_pad;
-      s.L = T; s.H = H; s.dirs = 1; s.h0_ld = H;
-      if (!last) s.seq_out = seq;
-      s.h_out = state(0); s.hf_out = hf;
-      gru_init_state(s, h0l, st);
-      kcount(h, MLDB_KSTAT_MISC);
-      for (int t = 0; t < T; ++t) {
-        s.step = t;
-        s.h_in = state(t & 1); s.hf_in = hf + (t & 1) * plane;
-        s.h_out = state((t + 1) & 1); s.hf_out = hf + ((t + 1) & 1) * plane;
-        GemmArgs gg; gg.a1 = rows_of(s.h_in, 0, n); gg.K1 = H; gg.M = n; gg.w = w.w_hh;
-        gg.out_f32 = (float*)a.gh.p; gg.ldc = 3 * H; gg.wide_n = 1;
-        op_gemm(h, gg, st);
-        gru_gate_simt(s, st);
-        kcount(h, MLDB_KSTAT_MISC);
-      }
-      hl = hf + (T & 1) * plane;
+      TRY(op_gru(h, l ? seq : xs, &w.w_ih, w.w_hh, w.b_hh, h0 + ((int64_t)l * B + b0) * H, H, lengths + b0, n, T, H, 1,
+                 a.gi, a.gru, last ? ActBuf{} : seq, nullptr, last ? &hl : nullptr, st));
     }
     k_a2m_head<<<(unsigned)n, 128, 0, st>>>(hl, H, H, a.l1w, a.l1b, a.l2w, a.l2b, c.output_size,
                                             features ? features + (int64_t)b0 * kA2mFeat : nullptr,

@@ -143,6 +143,23 @@ int dev_alloc(mldb_handle* h, void** p, size_t bytes) {
 }
 // Grow b to at least `bytes`, zero-filled (outside any capture).  Synchronises the device first: enqueued work may
 // still use the old buffer.
+int may_configure(const mldb_handle* h, int abi_version, int expected, bool on, const char* name, const char* what) {
+  if (abi_version != expected) FAIL(MLDB_ERR_INVALID, "mldb_%s_config abi_version mismatch", name);
+  if (h->finalized) FAIL(MLDB_ERR_STATE, "mldb_%s_configure must precede mldb_finalize_weights", name);
+  if (on) FAIL(MLDB_ERR_STATE, "%s is already configured", what);
+  return MLDB_OK;
+}
+int check_configured(const mldb_handle* h, bool on, const char* name, const char* what) {
+  if (!on) FAIL(MLDB_ERR_STATE, "%s is not configured (mldb_%s_configure)", what, name);
+  if (!h->finalized) FAIL(MLDB_ERR_STATE, "finalize weights first");
+  return MLDB_OK;
+}
+int eval_chunk(int option, int B, size_t per_seq, int round) {
+  if (option > 0) return std::min(B, option);
+  int c = (int)std::max<size_t>(1, ((size_t)1 << 30) / per_seq);
+  if (c > round) c = c / round * round;
+  return std::min(B, c);
+}
 int grow(GrowBuf& b, size_t bytes) {
   if (bytes <= b.cap) return MLDB_OK;
   CK(cudaDeviceSynchronize());

@@ -70,6 +70,10 @@ struct GrowBuf {
   ~GrowBuf() { cudaFree(p); }
 };
 
+// op_gru's state, one per model: two models' calls may run on different streams.  h_split / h_f32: the split16 /
+// fp32 state ping-pong (k_gru_seq_tc: h_f32 holds the final state); gh: h W_hh^T under gemm=simt.
+struct GruState { GrowBuf h_split, h_f32, gh; };
+
 struct LnW { float* g = nullptr; float* b = nullptr; };
 
 struct EncW {  // TransformerEncoderLayer (cross_attention.py:236-257)
@@ -136,7 +140,7 @@ struct T2mW {
   GrowBuf emb;                    // split16: the GRU input rows, movement im2col of the conv1 output
   GrowBuf mid;                    // movement conv2 output (split16), text word_embs + pos_emb (fp32)
   GrowBuf words;                  // text word_embs + pos_emb (split16, K padded)
-  GrowBuf h_split, h_f32, gh;     // GRU state ping-pong (split16, fp32), CUDA-core h W_hh^T
+  GruState gru;
   GrowBuf head_f32, head_ln;      // GRU head: first Linear, LayerNorm + LeakyReLU
 };
 
@@ -156,8 +160,7 @@ struct A2mW {
   GrowBuf x;                      // split16 frames [n * T, input_size padded to 64]
   GrowBuf gi;                     // fp32 [n * T, 3H]: x_t W_ih^T + b_ih of the running layer
   GrowBuf seq;                    // split16 [n * T, H]: a layer's h_t, the A operand of the next layer's input GEMM
-  GrowBuf h_last;                 // fp32 [n, H]: the last layer's h at t = len - 1
-  GrowBuf h_split, h_f32, gh;     // gemm=simt: state ping-pong (split16, fp32), h W_hh^T
+  GruState gru;
 };
 
 // UESTC action classifier (mldb_stgcn_configure): STGCN (uestc_stgcn.py), ten st_gcn blocks
@@ -332,6 +335,13 @@ inline int ops_done(mldb_handle* h) {
   CK(cudaGetLastError());
   return check_ops(h);
 }
+// mldb_<name>_configure after its null check: the config's abi_version, before finalize, not yet configured (`on`)
+int may_configure(const mldb_handle* h, int abi_version, int expected, bool on, const char* name, const char* what);
+// an entry point of a model configured by mldb_<name>_configure: configured (`on`) and finalized
+int check_configured(const mldb_handle* h, bool on, const char* name, const char* what);
+// sequences per chunk of an eager evaluator: the option, else what keeps the chunk's workspace near 1 GiB (whole
+// `round`-row tiles when more than one)
+int eval_chunk(int option, int B, size_t per_seq, int round);
 int dev_alloc(mldb_handle* h, void** p, size_t bytes);
 int grow(GrowBuf& b, size_t bytes);
 int grow_act(GrowBuf& b, int rows, int cols, ActBuf* out);
@@ -356,6 +366,16 @@ void op_gemm(mldb_handle* h, const GemmArgs& g, cudaStream_t st);
 void op_gemm_ln(mldb_handle* h, GemmArgs g, LnArgs l, float* cf32, cudaStream_t st);
 void op_ln(mldb_handle* h, const LnArgs& l, cudaStream_t st);
 void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st);
+// One GRU layer over n sequences of L steps, x [n * L, in] split16 (row b * L + t): gi = x W_ih^T + b_ih (grown
+// here), then the recurrence on k_gru_seq_tc (dirs == 1, H = 64 or 128 as mldb_a2m_configure enforces), on
+// k_gru_step_tc per step (dirs == 2), or under gemm=simt on CUDA-core GEMMs and k_gru_gate_simt per step.
+// w_hh: the directions' packed [3H, H] stacked; b_hh [dirs][3H]; h0 of (dir, row m) at h0[dir * H + m * h0_ld]
+// (k_gru_seq_tc: h0_ld == H).  seq_out (dirs == 1; hi null: none) gets h_t as split16 row m * L + t.  The final
+// states at t = len - 1 (null: not wanted), direction d's row m at row d * rows_pad + m (n rounded up to 128):
+// *fin split16 (not from k_gru_seq_tc), *fin_f32 fp32 with rows H floats apart.
+int op_gru(mldb_handle* h, ActBuf x, const LinW* w_ih, const LinW& w_hh, const float* b_hh, const float* h0,
+           int64_t h0_ld, const int32_t* lengths, int n, int L, int H, int dirs, GrowBuf& gi, GruState& ws,
+           ActBuf seq_out, ActBuf* fin, const float** fin_f32, cudaStream_t st);
 void op_tail(mldb_handle* h, const LinW& wo, const LnW& n1, const LinW& l1, const LinW& l2, const LnW& n2, ActBuf att,
              ActBuf x, ActBuf x1, ActBuf hbuf, ActBuf xout, int M, int d, int ff, float* cf32, cudaStream_t st,
              int fuse = 1);

@@ -43,6 +43,66 @@ void op_attn(mldb_handle* h, const AttnArgs& a, cudaStream_t st) {
     kcount(h, MLDB_KSTAT_ATTN_SIMT);
   }
 }
+int op_gru(mldb_handle* h, ActBuf x, const LinW* w_ih, const LinW& w_hh, const float* b_hh, const float* h0,
+           int64_t h0_ld, const int32_t* lengths, int n, int L, int H, int dirs, GrowBuf& gi, GruState& ws,
+           ActBuf seq_out, ActBuf* fin, const float** fin_f32, cudaStream_t st) {
+  TRY(grow(gi, (size_t)n * L * dirs * 3 * H * sizeof(float)));
+  float* gif = (float*)gi.p;
+  for (int d = 0; d < dirs; ++d) {                 // gi = x W_ih^T + b_ih, every step of every direction
+    GemmArgs g; g.a1 = x; g.K1 = x.cols; g.M = n * L; g.w = w_ih[d]; g.out_f32 = gif + (size_t)d * 3 * H;
+    g.ldc = dirs * 3 * H; g.wide_n = 1; g.vec_f32 = 1;
+    op_gemm(h, g, st);
+  }
+  if (h->use_tc && dirs == 1) {
+    GruSeqArgs s;
+    s.gi = gif; s.b_hh = b_hh; s.h0 = h0; s.lengths = lengths; s.w_hh = w_hh.w; s.w_plane_stride = w_hh.plane_stride;
+    s.w_inv_scale = w_hh.inv_scale; s.rows = n; s.L = L; s.H = H; s.seq_out = seq_out;
+    if (fin_f32) {
+      TRY(grow(ws.h_f32, (size_t)n * H * sizeof(float)));
+      *fin_f32 = s.h_last = (float*)ws.h_f32.p;
+    }
+    // mldb_a2m_configure refuses other H: k_gru_step_tc, the kernel for larger H, runs two directions only
+    if (!gru_seq_supported(H) || !gru_seq_tc(s, h->sm_count, st)) h->op_failed = true;
+    kcount(h, MLDB_KSTAT_GRU_TC);
+    return MLDB_OK;
+  }
+  const int rows_pad = (n + 127) / 128 * 128;
+  const size_t plane = (size_t)dirs * rows_pad * H, state_bytes = split16_bytes(dirs * rows_pad, H);
+  TRY(grow(ws.h_split, 2 * state_bytes));
+  TRY(grow(ws.h_f32, 2 * plane * sizeof(float)));
+  if (!h->use_tc) TRY(grow(ws.gh, plane * 3 * sizeof(float)));
+  float *hf = (float*)ws.h_f32.p, *gh = (float*)ws.gh.p;
+  auto state = [&](int b) { return split16_at((char*)ws.h_split.p + b * state_bytes, dirs * rows_pad, H); };
+  GruStepArgs a;
+  a.gi = gif; a.gh = gh; a.b_hh = b_hh; a.lengths = lengths; a.w_hh = w_hh.w; a.w_plane_stride = w_hh.plane_stride;
+  a.w_inv_scale = w_hh.inv_scale; a.rows = n; a.rows_pad = rows_pad; a.L = L; a.H = H; a.dirs = dirs; a.h0_ld = h0_ld;
+  a.seq_out = seq_out;
+  a.h_out = state(0); a.hf_out = hf;
+  gru_init_state(a, h0, st);
+  kcount(h, MLDB_KSTAT_MISC);
+  for (int s = 0; s < L; ++s) {
+    a.step = s;
+    a.h_in = state(s & 1); a.hf_in = hf + (s & 1) * plane;
+    a.h_out = state((s + 1) & 1); a.hf_out = hf + ((s + 1) & 1) * plane;
+    if (h->use_tc) {
+      if (!gru_step_tc(a, st)) h->op_failed = true;
+      kcount(h, MLDB_KSTAT_GRU_TC);
+    } else {
+      for (int d = 0; d < dirs; ++d) {
+        LinW w = w_hh;
+        w.w += (size_t)d * 3 * H * H; w.N = 3 * H;
+        GemmArgs g; g.a1 = rows_of(a.h_in, (int64_t)d * rows_pad, n); g.K1 = H; g.M = n; g.w = w;
+        g.out_f32 = gh + (size_t)d * rows_pad * 3 * H; g.ldc = 3 * H; g.wide_n = 1;
+        op_gemm(h, g, st);
+      }
+      gru_gate_simt(a, st);
+      kcount(h, MLDB_KSTAT_MISC);
+    }
+  }
+  if (fin) *fin = state(L & 1);
+  if (fin_f32) *fin_f32 = hf + (L & 1) * plane;
+  return MLDB_OK;
+}
 // which stream's scratch / flags the fused FFN uses (branches run concurrently, each on its own pair)
 static int ffn_scratch_slot(const mldb_handle* h, cudaStream_t st) {
   int k = 0;

@@ -37,9 +37,7 @@ static void spec_bn(mldb_handle* h, const std::string& p, int n) {
 
 extern "C" int mldb_stgcn_configure(mldb_handle* h, const mldb_stgcn_config* cfg) {
   if (!h || !cfg) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (cfg->abi_version != MLDB_STGCN_ABI_VERSION) FAIL(MLDB_ERR_INVALID, "mldb_stgcn_config abi_version mismatch");
-  if (h->finalized) FAIL(MLDB_ERR_STATE, "mldb_stgcn_configure must precede mldb_finalize_weights");
-  if (h->stgcn.on) FAIL(MLDB_ERR_STATE, "the UESTC classifier is already configured");
+  TRY(may_configure(h, cfg->abi_version, MLDB_STGCN_ABI_VERSION, h->stgcn.on, "stgcn", "the UESTC classifier"));
   const mldb_stgcn_config& c = *cfg;
   if (c.in_channels < 1 || c.in_channels > 64) FAIL(MLDB_ERR_INVALID, "in_channels must be in [1, 64], got %d", c.in_channels);
   if (c.num_class < 1 || c.num_class > 4096) FAIL(MLDB_ERR_INVALID, "num_class must be in [1, 4096], got %d", c.num_class);
@@ -284,17 +282,10 @@ static StgcnSizes stgcn_sizes(const mldb_stgcn_config& c, int n, int T, bool tc)
   return s;
 }
 
-// sequences per chunk: the option, else what keeps the chunk's workspace near 1 GiB
-static int stgcn_chunk(const mldb_handle* h, int B, size_t per_seq) {
-  if (h->stgcn.chunk > 0) return std::min(B, h->stgcn.chunk);
-  return std::min(B, (int)std::max<size_t>(1, ((size_t)1 << 30) / per_seq));
-}
-
 extern "C" int mldb_stgcn_classify(mldb_handle* h, const float* x, int32_t B, int32_t T, float* yhat, float* features,
                                    void* stream) {
   if (!h || !x) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (!h->stgcn.on) FAIL(MLDB_ERR_STATE, "the UESTC classifier is not configured (mldb_stgcn_configure)");
-  if (!h->finalized) FAIL(MLDB_ERR_STATE, "finalize weights first");
+  TRY(check_configured(h, h->stgcn.on, "stgcn", "the UESTC classifier"));
   StgcnW& s = h->stgcn;
   const mldb_stgcn_config& c = s.cfg;
   if (B < 1 || T < 1 || (int64_t)B * T > (1 << 22))
@@ -303,7 +294,7 @@ extern "C" int mldb_stgcn_classify(mldb_handle* h, const float* x, int32_t B, in
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const bool tc = h->use_tc;
-  const int Bc = stgcn_chunk(h, B, stgcn_sizes(c, 1, T, tc).sum());
+  const int Bc = eval_chunk(s.chunk, B, stgcn_sizes(c, 1, T, tc).sum(), 1);
   const int mix_smem = (kK * kJ * kJ + kJ * std::max(c.in_channels, kFeat)) * (int)sizeof(float);
   for (int b0 = 0; b0 < B; b0 += Bc) {
     const int n = std::min(Bc, B - b0);

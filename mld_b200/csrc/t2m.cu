@@ -40,9 +40,7 @@ static void spec_gru(mldb_handle* h, const std::string& p, int in, int H, int ou
 
 extern "C" int mldb_t2m_configure(mldb_handle* h, const mldb_t2m_config* cfg) {
   if (!h || !cfg) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (cfg->abi_version != MLDB_T2M_ABI_VERSION) FAIL(MLDB_ERR_INVALID, "mldb_t2m_config abi_version mismatch");
-  if (h->finalized) FAIL(MLDB_ERR_STATE, "mldb_t2m_configure must precede mldb_finalize_weights");
-  if (h->t2m.on) FAIL(MLDB_ERR_STATE, "the T2M evaluator is already configured");
+  TRY(may_configure(h, cfg->abi_version, MLDB_T2M_ABI_VERSION, h->t2m.on, "t2m", "the T2M evaluator"));
   const mldb_t2m_config& c = *cfg;
   if (c.parts < 1 || c.parts > 7) FAIL(MLDB_ERR_INVALID, "parts must be a non-empty MLDB_T2M_* mask");
   if (c.dim_word < 1 || c.dim_pos_ohot < 1 || c.dim_coemb_hidden < 1 || c.dim_pose < 1 || c.dim_motion_latent < 1)
@@ -141,20 +139,11 @@ int pack_t2m(mldb_handle* h) {
 // The workspace buffers (T2mW) are shared between encoders and grow to the largest use; every kernel that writes one
 // writes all of the region it later reads.
 
-// sequences per chunk: the option, else what keeps the chunk's workspace near 1 GiB (whole 128-row tiles when > 128)
-static int t2m_chunk(const mldb_handle* h, int B, size_t per_seq) {
-  if (h->t2m.chunk > 0) return std::min(B, h->t2m.chunk);
-  int c = (int)std::max<size_t>(1, ((size_t)1 << 30) / per_seq);
-  if (c > 128) c = c / 128 * 128;
-  return std::min(B, c);
-}
 static size_t gru_bytes_per_seq(int L, int in, int H) {
   return (size_t)L * (4 * in + 24 * H) + (size_t)40 * H;   // x (split16), gi (fp32), state and head
 }
-static int t2m_ready(mldb_handle* h, int part, const char* name) {
-  if (!h->t2m.on || !(h->t2m.cfg.parts & part)) FAIL(MLDB_ERR_STATE, "the T2M %s encoder is not configured (mldb_t2m_configure)", name);
-  if (!h->finalized) FAIL(MLDB_ERR_STATE, "finalize weights first");
-  return MLDB_OK;
+static int t2m_ready(mldb_handle* h, int part, const char* what) {
+  return check_configured(h, h->t2m.on && (h->t2m.cfg.parts & part), "t2m", what);
 }
 
 // Bidirectional GRU over x [n * L, in] (split16, row b * L + t) and the BiGRUCo head -> out [n, out_dim] fp32.
@@ -162,50 +151,10 @@ static int gru_forward(mldb_handle* h, const GruW& g, ActBuf x, const int32_t* l
                        int out_dim, cudaStream_t st) {
   T2mW& t = h->t2m;
   const int H = g.H, rows_pad = (n + 127) / 128 * 128;
-  TRY(grow(t.f32, (size_t)n * L * 6 * H * sizeof(float)));
-  float* gi = (float*)t.f32.p;
-  for (int d = 0; d < 2; ++d) {                    // gi = x W_ih^T + b_ih, every step of both directions
-    GemmArgs ga; ga.a1 = x; ga.K1 = x.cols; ga.M = n * L; ga.w = g.w_ih[d]; ga.out_f32 = gi + (size_t)d * 3 * H;
-    ga.ldc = 6 * H; ga.wide_n = 1; ga.vec_f32 = 1;
-    op_gemm(h, ga, st);
-  }
-  const size_t plane = (size_t)2 * rows_pad * H, state_bytes = split16_bytes(2 * rows_pad, H);
-  TRY(grow(t.h_split, 2 * state_bytes));           // ping-pong split16 state
-  TRY(grow(t.h_f32, 2 * plane * sizeof(float)));   // ping-pong fp32 state
-  float* hf = (float*)t.h_f32.p;
-  float* gh = nullptr;
-  if (!h->use_tc) {
-    TRY(grow(t.gh, plane * 3 * sizeof(float)));
-    gh = (float*)t.gh.p;
-  }
-  auto state = [&](int b) { return split16_at((char*)t.h_split.p + b * state_bytes, 2 * rows_pad, H); };
-  GruStepArgs a;
-  a.gi = gi; a.gh = gh; a.b_hh = g.b_hh; a.lengths = lengths; a.w_hh = g.w_hh.w; a.w_plane_stride = g.w_hh.plane_stride;
-  a.w_inv_scale = g.w_hh.inv_scale; a.rows = n; a.rows_pad = rows_pad; a.L = L; a.H = H;
-  a.h_out = state(0); a.hf_out = hf;
-  gru_init_state(a, g.h0, st);
-  kcount(h, MLDB_KSTAT_MISC);
-  for (int s = 0; s < L; ++s) {
-    a.step = s;
-    a.h_in = state(s & 1); a.hf_in = hf + (s & 1) * plane;
-    a.h_out = state((s + 1) & 1); a.hf_out = hf + ((s + 1) & 1) * plane;
-    if (h->use_tc) {
-      if (!gru_step_tc(a, st)) h->op_failed = true;
-      kcount(h, MLDB_KSTAT_GRU_TC);
-    } else {                                       // gemm=simt: h W_hh^T per direction on CUDA cores, then the gates
-      for (int d = 0; d < 2; ++d) {
-        LinW w = g.w_hh;
-        w.w += (size_t)d * 3 * H * H; w.N = 3 * H;
-        GemmArgs gg; gg.a1 = rows_of(a.h_in, (int64_t)d * rows_pad, n); gg.K1 = H; gg.M = n; gg.w = w;
-        gg.out_f32 = gh + (size_t)d * rows_pad * 3 * H; gg.ldc = 3 * H; gg.wide_n = 1;
-        op_gemm(h, gg, st);
-      }
-      gru_gate_simt(a, st);
-      kcount(h, MLDB_KSTAT_MISC);
-    }
-  }
+  ActBuf fin;
+  // h0_ld = 0: the learned `hidden` is the initial state of every row
+  TRY(op_gru(h, x, g.w_ih, g.w_hh, g.b_hh, g.h0, 0, lengths, n, L, H, 2, t.f32, t.gru, ActBuf{}, &fin, nullptr, st));
   // head: cat(h_fwd final, h_bwd final) -> Linear -> LayerNorm -> LeakyReLU -> Linear
-  const ActBuf fin = state(L & 1);
   TRY(grow(t.head_f32, (size_t)n * H * sizeof(float)));
   float* cf = (float*)t.head_f32.p;
   ActBuf ln_out;
@@ -224,7 +173,7 @@ static int gru_forward(mldb_handle* h, const GruW& g, ActBuf x, const int32_t* l
 extern "C" int mldb_t2m_movement(mldb_handle* h, const float* x, int32_t ld, int32_t B, int32_t T, float* out,
                                  void* stream) {
   if (!h || !x || !out) FAIL(MLDB_ERR_INVALID, "null argument");
-  TRY(t2m_ready(h, MLDB_T2M_MOVEMENT, "movement"));
+  TRY(t2m_ready(h, MLDB_T2M_MOVEMENT, "the T2M movement encoder"));
   const mldb_t2m_config& c = h->t2m.cfg;
   if (B < 1 || T < 4) FAIL(MLDB_ERR_INVALID, "movement encoder input must be [B >= 1, T >= 4, %d], got B=%d T=%d", c.dim_pose, B, T);
   if (ld < c.dim_pose) FAIL(MLDB_ERR_INVALID, "row stride ld=%d is smaller than dim_pose=%d", ld, c.dim_pose);
@@ -235,7 +184,7 @@ extern "C" int mldb_t2m_movement(mldb_handle* h, const float* x, int32_t ld, int
   const int C = c.dim_pose, Cp = (C + 15) / 16 * 16, hid = c.dim_move_hidden, lat = c.dim_move_latent;
   const int T1 = T / 2, T2 = T1 / 2;
   const size_t per_seq = (size_t)T1 * (16 * Cp + 4 * hid) + (size_t)T2 * (16 * hid + 4 * lat);
-  const int Bc = t2m_chunk(h, B, per_seq);
+  const int Bc = eval_chunk(t.chunk, B, per_seq, 128);
   for (int b0 = 0; b0 < B; b0 += Bc) {
     const int n = std::min(Bc, B - b0);
     ActBuf a1, a2, z;
@@ -264,14 +213,14 @@ extern "C" int mldb_t2m_movement(mldb_handle* h, const float* x, int32_t ld, int
 extern "C" int mldb_t2m_motion(mldb_handle* h, const float* x, const int32_t* lengths, int32_t B, int32_t L, float* out,
                                void* stream) {
   if (!h || !x || !lengths || !out) FAIL(MLDB_ERR_INVALID, "null argument");
-  TRY(t2m_ready(h, MLDB_T2M_MOTION, "motion"));
+  TRY(t2m_ready(h, MLDB_T2M_MOTION, "the T2M motion encoder"));
   const mldb_t2m_config& c = h->t2m.cfg;
   if (B < 1 || L < 1 || (int64_t)B * L > (1 << 26)) FAIL(MLDB_ERR_INVALID, "motion encoder input must be [B >= 1, L >= 1, %d], got B=%d L=%d", c.dim_move_latent, B, L);
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   T2mW& t = h->t2m;
   const int In = c.dim_move_latent, H = c.dim_motion_hidden;
-  const int Bc = t2m_chunk(h, B, gru_bytes_per_seq(L, In + H, H));
+  const int Bc = eval_chunk(t.chunk, B, gru_bytes_per_seq(L, In + H, H), 128);
   for (int b0 = 0; b0 < B; b0 += Bc) {
     const int n = std::min(Bc, B - b0);
     ActBuf xs, e;
@@ -290,14 +239,14 @@ extern "C" int mldb_t2m_motion(mldb_handle* h, const float* x, const int32_t* le
 extern "C" int mldb_t2m_text(mldb_handle* h, const float* word_embs, const float* pos_ohot, const int32_t* lengths,
                              int32_t B, int32_t L, float* out, void* stream) {
   if (!h || !word_embs || !pos_ohot || !lengths || !out) FAIL(MLDB_ERR_INVALID, "null argument");
-  TRY(t2m_ready(h, MLDB_T2M_TEXT, "text"));
+  TRY(t2m_ready(h, MLDB_T2M_TEXT, "the T2M text encoder"));
   const mldb_t2m_config& c = h->t2m.cfg;
   if (B < 1 || L < 1 || (int64_t)B * L > (1 << 26)) FAIL(MLDB_ERR_INVALID, "text encoder input must be [B >= 1, L >= 1, *], got B=%d L=%d", B, L);
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   T2mW& t = h->t2m;
   const int W = c.dim_word, P = c.dim_pos_ohot, H = c.dim_text_hidden;
-  const int Bc = t2m_chunk(h, B, gru_bytes_per_seq(L, pad64(P) + 2 * W + pad64(W) + H, H));
+  const int Bc = eval_chunk(t.chunk, B, gru_bytes_per_seq(L, pad64(P) + 2 * W + pad64(W) + H, H), 128);
   for (int b0 = 0; b0 < B; b0 += Bc) {
     const int n = std::min(Bc, B - b0), M = n * L;
     ActBuf ps, xs, e;

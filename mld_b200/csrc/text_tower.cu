@@ -17,9 +17,7 @@ extern "C" void mldb_default_text_config(mldb_text_config* c) {
 
 extern "C" int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg) {
   if (!h || !cfg) FAIL(MLDB_ERR_INVALID, "null argument");
-  if (cfg->abi_version != MLDB_TEXT_ABI_VERSION) FAIL(MLDB_ERR_INVALID, "mldb_text_config abi_version mismatch");
-  if (h->finalized) FAIL(MLDB_ERR_STATE, "mldb_text_configure must precede mldb_finalize_weights");
-  if (h->text.on) FAIL(MLDB_ERR_STATE, "the text tower is already configured");
+  TRY(may_configure(h, cfg->abi_version, MLDB_TEXT_ABI_VERSION, h->text.on, "text", "the text tower"));
   const mldb_text_config& c = *cfg;
   if (c.vocab_size < 1 || c.layers < 1 || c.heads < 1 || c.ff < 1 || c.projection_dim < 1 || !(c.ln_eps > 0.0f))
     FAIL(MLDB_ERR_INVALID, "bad text config");
@@ -91,8 +89,7 @@ extern "C" int mldb_text_encode(mldb_handle* h, const int64_t* ids, int32_t n, i
                                 void* stream) {
   if (!h || !ids || !out) FAIL(MLDB_ERR_INVALID, "null argument");
   TextW& tw = h->text;
-  if (!tw.on) FAIL(MLDB_ERR_STATE, "the text tower is not configured (mldb_text_configure)");
-  if (!h->finalized) FAIL(MLDB_ERR_STATE, "finalize weights first");
+  TRY(check_configured(h, tw.on, "text", "the text tower"));
   const mldb_text_config& c = tw.cfg;
   if (n < 1 || L < 1 || L > c.max_positions) FAIL(MLDB_ERR_INVALID, "ids must be [n >= 1, 1 <= L <= %d]", c.max_positions);
   if ((int64_t)n * L > (1 << 30)) FAIL(MLDB_ERR_INVALID, "too many tokens");

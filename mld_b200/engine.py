@@ -163,9 +163,7 @@ class Engine:
     def text_encode(self, ids: torch.Tensor, mode: int = _lib.TEXT_POOLED) -> torch.Tensor:
         """int64 token ids [n, L] -> last_hidden_state [n, L, hidden] (TEXT_HIDDEN) or get_text_features [n, proj]
         (TEXT_POOLED), on the current stream.  Ids outside the vocabulary are rejected here, before the launch."""
-        tc = getattr(self, "text_cfg", None)
-        if tc is None:
-            raise RuntimeError("text_configure() was not called before finalize()")
+        tc = self._configured("text_cfg", "text_configure() was not called before finalize()")
         if ids.dim() != 2 or ids.shape[0] < 1 or not 1 <= ids.shape[1] <= tc.max_positions:
             raise ValueError(f"ids must be [n, L] with 1 <= L <= {tc.max_positions}, got {tuple(ids.shape)}")
         if ids.numel() and (int(ids.min()) < 0 or int(ids.max()) >= tc.vocab_size):
@@ -186,12 +184,21 @@ class Engine:
         self.t2m_cfg = tcfg
 
     def _t2m(self, part: int, name: str):
-        tc = getattr(self, "t2m_cfg", None)
-        if tc is None or not tc.parts & part:
-            raise RuntimeError(f"the T2M {name} encoder was not configured (t2m_configure) before finalize()")
+        msg = f"the T2M {name} encoder was not configured (t2m_configure) before finalize()"
+        tc = self._configured("t2m_cfg", msg)
+        if not tc.parts & part:
+            raise RuntimeError(msg)
         return tc
 
-    def _t2m_lengths(self, lengths, B: int, L: int) -> torch.Tensor:
+    def _configured(self, attr: str, msg: str):
+        """The config that ``*_configure`` stored as ``attr``; RuntimeError(msg) if it was not called."""
+        cfg = getattr(self, attr, None)
+        if cfg is None:
+            raise RuntimeError(msg)
+        return cfg
+
+    def _seq_lengths(self, lengths, B: int, L: int) -> torch.Tensor:
+        """B integer sequence lengths, each in [1, L], as a contiguous int32 tensor on the device."""
         ln = torch.as_tensor(lengths).reshape(-1)
         if ln.numel() != B:
             raise ValueError(f"lengths must hold {B} values, got {ln.numel()}")
@@ -223,7 +230,7 @@ class Engine:
             raise ValueError(f"x must be [B >= 1, L >= 1, {tc.dim_move_latent}], got {tuple(x.shape)}")
         xd = _f32c(x, self.device)
         B, L = xd.shape[:2]
-        ln = self._t2m_lengths(lengths, B, L)
+        ln = self._seq_lengths(lengths, B, L)
         out = torch.empty((B, tc.dim_motion_latent), dtype=torch.float32, device=self.device)
         check(self.lib.mldb_t2m_motion(self._h, _ptr(xd), _ptr(ln), B, L, _ptr(out), self._stream()), "mldb_t2m_motion")
         return out
@@ -239,7 +246,7 @@ class Engine:
                              f"got {tuple(pos_ohot.shape)}")
         w, p = _f32c(word_embs, self.device), _f32c(pos_ohot, self.device)
         B, L = w.shape[:2]
-        ln = self._t2m_lengths(lengths, B, L)
+        ln = self._seq_lengths(lengths, B, L)
         out = torch.empty((B, tc.dim_coemb_hidden), dtype=torch.float32, device=self.device)
         check(self.lib.mldb_t2m_text(self._h, _ptr(w), _ptr(p), _ptr(ln), B, L, _ptr(out), self._stream()),
               "mldb_t2m_text")
@@ -254,9 +261,7 @@ class Engine:
     def a2m_classify(self, x: torch.Tensor, lengths, h0: torch.Tensor):
         """MotionDiscriminator with an explicit initial state: x [B, input_size, T] (or [B, njoints, nfeats, T]),
         lengths (each in [1, T]), h0 [hidden_layer, B, hidden_size] -> (logits [B, output_size], features [B, 30])."""
-        ac = getattr(self, "a2m_cfg", None)
-        if ac is None:
-            raise RuntimeError("the action classifier was not configured (a2m_configure) before finalize()")
+        ac = self._configured("a2m_cfg", "the action classifier was not configured (a2m_configure) before finalize()")
         if x.dim() == 4:
             x = x.reshape(x.shape[0], x.shape[1] * x.shape[2], x.shape[3])
         if x.dim() != 3 or x.shape[1] != ac.input_size or x.shape[0] < 1 or x.shape[2] < 1:
@@ -265,7 +270,7 @@ class Engine:
         B, T = xd.shape[0], xd.shape[2]
         if tuple(h0.shape) != (ac.hidden_layer, B, ac.hidden_size):
             raise ValueError(f"h0 must be [{ac.hidden_layer}, {B}, {ac.hidden_size}], got {tuple(h0.shape)}")
-        ln = self._t2m_lengths(lengths, B, T)
+        ln = self._seq_lengths(lengths, B, T)
         hd = _f32c(h0, self.device)
         logits = torch.empty((B, ac.output_size), dtype=torch.float32, device=self.device)
         feats = torch.empty((B, 30), dtype=torch.float32, device=self.device)
@@ -281,9 +286,7 @@ class Engine:
 
     def stgcn_classify(self, motion: torch.Tensor):
         """STGCN: motion [B, 24, in_channels, T] -> (yhat [B, num_class], features [B, 256])."""
-        sc = getattr(self, "stgcn_cfg", None)
-        if sc is None:
-            raise RuntimeError("the UESTC classifier was not configured (stgcn_configure) before finalize()")
+        sc = self._configured("stgcn_cfg", "the UESTC classifier was not configured (stgcn_configure) before finalize()")
         if motion.dim() != 4 or motion.shape[0] < 1 or motion.shape[1] != 24 or motion.shape[2] != sc.in_channels \
                 or motion.shape[3] < 1:
             raise ValueError(f"motion must be [B >= 1, 24, {sc.in_channels}, T >= 1], got {tuple(motion.shape)}")

@@ -44,7 +44,14 @@ def _lengths(lengths, B: int, L: int) -> torch.Tensor:
     return ln
 
 
-class _T2mModule(_EngineModule):
+class _EvaluatorModule(_EngineModule):
+    """An evaluation network: its engine's handle holds only this network."""
+
+    def _make_config(self):
+        return make_config(num_layers=0, vae="none")
+
+
+class _T2mModule(_EvaluatorModule):
     _part = 0
 
     def __init__(self, **dims):
@@ -55,9 +62,6 @@ class _T2mModule(_EngineModule):
             setattr(cfg, k, int(v))
         self._t2m_cfg = cfg
         _register_tree(self, synth.t2m_state_dicts(seed=0, **dims)[self._key])
-
-    def _make_config(self):
-        return make_config(num_layers=0, vae="none")            # a handle that holds only this evaluator part
 
     def _configure_engine(self, eng):
         eng.t2m_configure(self._t2m_cfg)
@@ -101,7 +105,7 @@ class B200MotionEncoderBiGRUCo(_T2mModule):
         return self.engine().t2m_motion(inputs, m_lens)
 
 
-class B200MotionDiscriminator(_EngineModule):
+class B200MotionDiscriminator(_EvaluatorModule):
     """``MotionDiscriminator`` (mld/models/architectures/humanact12_gru.py:6-55): nn.GRU(input_size, hidden_size,
     hidden_layer), the output at ``lengths - 1``, Linear(hidden_size, 30), tanh, Linear(30, output_size).
 
@@ -122,9 +126,6 @@ class B200MotionDiscriminator(_EngineModule):
         self._a2m_cfg = cfg
         _register_tree(self, synth.a2m_state_dict(seed=0, input_size=input_size, hidden_size=hidden_size,
                                                    hidden_layer=hidden_layer, output_size=output_size))
-
-    def _make_config(self):
-        return make_config(num_layers=0, vae="none")            # a handle that holds only the classifier
 
     def _configure_engine(self, eng):
         eng.a2m_configure(self._a2m_cfg)
@@ -159,7 +160,7 @@ class B200MotionDiscriminatorForFID(B200MotionDiscriminator):
         return self._classify(motion_sequence, lengths, hidden_unit)[1]
 
 
-class B200STGCN(_EngineModule):
+class B200STGCN(_EvaluatorModule):
     """``STGCN`` (mld/models/architectures/uestc_stgcn.py:8-130), the UESTC action classifier of ``UESTCMetrics``
     (mld/models/metrics/stgcn.py:32-40): data_bn, ten st_gcn blocks over the SMPL graph, a global average pool and a
     1 x 1 convolution head.  Same constructor kwargs; ``A`` is built from ``kintree_path`` with the same spatial
@@ -198,20 +199,7 @@ class B200STGCN(_EngineModule):
                 if "num_batches_tracked" not in k:
                     w = k.rsplit(".", 1)[0]
                     sd[w + ".weight"], sd[w + ".bias"] = torch.ones_like(sd[k]), torch.zeros_like(sd[k])
-        for key, value in sd.items():
-            parts = key.split(".")
-            m = self
-            for p in parts[:-1]:
-                if p not in m._modules:
-                    m.add_module(p, torch.nn.Module())
-                m = m._modules[p]
-            if parts[-1] in self._BUFFERS:
-                m.register_buffer(parts[-1], value.clone())
-            else:
-                m.register_parameter(parts[-1], torch.nn.Parameter(value.clone(), requires_grad=False))
-
-    def _make_config(self):
-        return make_config(num_layers=0, vae="none")            # a handle that holds only the classifier
+        _register_tree(self, sd, buffers=self._BUFFERS)
 
     def _configure_engine(self, eng):
         eng.stgcn_configure(self._stgcn_cfg)

@@ -11,7 +11,7 @@ math runs in ``libmldb200.so``.  Inference only (parameters do not require grad)
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Sequence
 
 import torch
 from torch import nn
@@ -20,8 +20,9 @@ from . import synth
 from .engine import Engine, make_config
 
 
-def _register_tree(root: nn.Module, tensors: Dict[str, torch.Tensor]):
-    """Create nested sub-modules so that ``root.state_dict()`` has exactly these keys."""
+def _register_tree(root: nn.Module, tensors: Dict[str, torch.Tensor], buffers: Sequence[str] = ()):
+    """Create nested sub-modules so that ``root.state_dict()`` has exactly these keys.  A tensor whose last key
+    component is in ``buffers`` becomes a buffer, every other one a parameter."""
     for key, value in tensors.items():
         parts = key.split(".")
         m = root
@@ -29,7 +30,10 @@ def _register_tree(root: nn.Module, tensors: Dict[str, torch.Tensor]):
             if p not in m._modules:
                 m.add_module(p, nn.Module())
             m = m._modules[p]
-        m.register_parameter(parts[-1], nn.Parameter(value.clone(), requires_grad=False))
+        if parts[-1] in buffers:
+            m.register_buffer(parts[-1], value.clone())
+        else:
+            m.register_parameter(parts[-1], nn.Parameter(value.clone(), requires_grad=False))
 
 
 class _EngineModule(nn.Module):
