@@ -436,6 +436,38 @@ int mldb_stgcn_configure(mldb_handle* h, const mldb_stgcn_config* cfg);
 int mldb_stgcn_classify(mldb_handle* h, const float* x, int32_t B, int32_t T, float* yhat, float* features,
                         void* stream);
 
+/* ---- SMPL layer (Rotation2xyz, mld/transforms/rotation2xyz.py, as MLD.a2m_eval calls it: pose_rep "rot6d",
+ * glob, translation, zero betas): smplx 0.1.28's SMPLLayer -> lbs(..., pose2rot=False) with the 24 joints of
+ * `parents`.  Keys (strict) under "smpl.": v_template [V, 3], posedirs [207, 3 V] (smplx's layout: row 9 (j - 1) + 3 r
+ * + c of (R_j - I), column 3 v + c), J_regressor [24, V], lbs_weights [V, 24], parents [24] (parents[0] = -1 and
+ * 0 <= parents[j] < j; checked at mldb_finalize_weights).  The rest joints J_regressor v_template are computed once
+ * there, in double.  There is no CUDA-core twin of this path: option gemm=simt does not apply to it (the float64
+ * oracle is its yardstick). */
+#define MLDB_SMPL_ABI_VERSION 1
+#define MLDB_SMPL_JOINTS 0      /* jointstype "smpl": the 24 posed joints, joint 0 subtracted per frame */
+#define MLDB_SMPL_VERTICES 1    /* jointstype "vertices": the V skinned vertices */
+typedef struct mldb_smpl_config {
+  int32_t abi_version;        /* must be MLDB_SMPL_ABI_VERSION */
+  int32_t num_vertices;       /* V: 6890 (SMPL); 1 .. 2^20 */
+} mldb_smpl_config;
+void mldb_default_smpl_config(mldb_smpl_config* cfg);
+/* Add the model's keys to the strict key spec; after mldb_create, before mldb_finalize_weights. */
+int mldb_smpl_configure(mldb_handle* h, const mldb_smpl_config* cfg);
+/* Replaces: Rotation2xyz.__call__(x, mask, pose_rep="rot6d", translation=True, glob=True, jointstype, vertstrans).
+ *   feats       [B, T, 150] fp32: frame t's joint j rotation at feats[b, t, c * 25 + j] (c < 6, j < 24), its translation
+ *               at feats[b, t, c * 25 + 24] (c < 3) - MLD's sample.view(B, T, 6, 25) before the permute
+ *   mask        device uint8 [B, T] (any pattern; 0: the frame's features are never read and its output is zero before
+ *               the translation), or NULL for every frame
+ *   jointstype  MLDB_SMPL_JOINTS -> out [B, 24, 3, T];  MLDB_SMPL_VERTICES -> out [B, V, 3, T]
+ *   vertstrans  1: every frame, masked or not, gets trans[t] - trans[0] of its sequence added (as the reference)
+ * The arguments are checked on the host before anything is launched.  Runs eagerly on `stream`; the vertex path's
+ * workspace grows on demand (outside any capture, synchronising the device when it does) and long batches run in
+ * chunks of whole sequences (option smpl_chunk); every sequence is computed independently of the others and of the
+ * chunking.  Kernels: one k_smpl_fk (MLDB_KSTAT_MISC) per chunk, and for the vertices one
+ * k_smpl_lbs (MLDB_KSTAT_GEMM_TC: the split16 pose-blend GEMM with skinning in its epilogue). */
+int mldb_smpl_forward(mldb_handle* h, const float* feats, const uint8_t* mask, int32_t B, int32_t T,
+                      int32_t jointstype, int32_t vertstrans, float* out, void* stream);
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);
@@ -445,7 +477,8 @@ int64_t mldb_launch_count(const mldb_handle* h);
  * graph counts once, at capture).  out: HOST int64[MLDB_KSTAT_COUNT], index = MLDB_KSTAT_*.  Lets a caller
  * (and the tests) assert that nothing fell back from the wgmma kernels to the CUDA-core kernels. */
 #define MLDB_KSTAT_GEMM_TC 0      /* k_gemm_tc, plain epilogue; k_proj_tc (its K = 256 split16 projections);
-                                     k_tconv_tc (the UESTC classifier's temporal convolutions) */
+                                     k_tconv_tc (the UESTC classifier's temporal convolutions); k_smpl_lbs (the SMPL
+                                     layer's pose-blend GEMM + skinning) */
 #define MLDB_KSTAT_GEMM_LN_TC 1   /* k_gemm_tc, fused residual + LayerNorm epilogue */
 #define MLDB_KSTAT_FFN_TC 2       /* k_ffn_tc (fused FFN block; in the encoder layers it also runs the folded
                                      out-projection + residual + LayerNorm in front of the FFN) */
@@ -455,7 +488,7 @@ int64_t mldb_launch_count(const mldb_handle* h);
 #define MLDB_KSTAT_GEMM_SIMT 6    /* k_gemm_simt (CUDA cores: odd-K embeddings, time MLP, gemm=simt) */
 #define MLDB_KSTAT_LN_SIMT 7      /* k_ln stand-alone LayerNorm (stack-final norms, cross-attention collapse) */
 #define MLDB_KSTAT_LN_UNFUSED 8   /* k_ln behind a GEMM whose LayerNorm could NOT be fused (a fallback) */
-#define MLDB_KSTAT_MISC 9         /* token assembly, scheduler step, feats2joints, ... */
+#define MLDB_KSTAT_MISC 9         /* token assembly, scheduler step, feats2joints, k_smpl_fk, ... */
 #define MLDB_KSTAT_TEXT_LN 10     /* k_text_ln: the text tower's row LayerNorm (+ embedding / eos gather) */
 #define MLDB_KSTAT_GRU_TC 11      /* k_gru_step_tc: one recurrent step of the T2M evaluator's bidirectional GRU;
                                      k_gru_seq_tc: one whole layer of the action classifier's GRU */
@@ -477,6 +510,8 @@ int mldb_reset_kernel_stats(mldb_handle* h);
  *   "t2m_chunk"  0 | n                  T2M evaluator: sequences per batch chunk (0: sized from the workspace budget)
  *   "a2m_chunk"  0 | n                  action classifier: sequences per batch chunk (0: from the workspace budget)
  *   "stgcn_chunk" 0 | n                 UESTC classifier: sequences per batch chunk (0: from the workspace budget)
+ *   "smpl_chunk" 0 | n                  SMPL layer: sequences per batch chunk (0: from the vertex path's workspace budget;
+ *                                        the joint path needs no workspace and then runs unchunked)
  * Environment only: MLDB_PDL (programmatic dependent launch, 1); MLDB_SNAKE (1: attention and the fused FFN walk
  * the token tiles downwards, the GEMMs upwards, so every kernel starts on the rows its producer wrote last). */
 int mldb_set_option(mldb_handle* h, const char* name, const char* value);

@@ -33,6 +33,9 @@ T2M_TEXT, T2M_MOVEMENT, T2M_MOTION = 1, 2, 4
 MLDB_A2M_ABI_VERSION = 1
 # UESTC action classifier (mldb_stgcn_config, mldb_stgcn_classify)
 MLDB_STGCN_ABI_VERSION = 1
+# SMPL layer (mldb_smpl_config, mldb_smpl_forward)
+MLDB_SMPL_ABI_VERSION = 1
+SMPL_JOINTS, SMPL_VERTICES = 0, 1
 
 
 class MldbConfig(C.Structure):
@@ -85,6 +88,11 @@ class MldbStgcnConfig(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("in_channels", C.c_int32), ("num_class", C.c_int32)]
 
 
+class MldbSmplConfig(C.Structure):
+    """``mldb_smpl_config`` (include/mldb.h)."""
+    _fields_ = [("abi_version", C.c_int32), ("num_vertices", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/mldb.h declares
 _P = C.c_void_p
 _SIGNATURES = {
@@ -130,6 +138,9 @@ _SIGNATURES = {
     "mldb_default_stgcn_config": (None, [C.POINTER(MldbStgcnConfig)]),
     "mldb_stgcn_configure": (C.c_int, [_P, C.POINTER(MldbStgcnConfig)]),
     "mldb_stgcn_classify": (C.c_int, [_P, _P, C.c_int32, C.c_int32, _P, _P, _P]),
+    "mldb_default_smpl_config": (None, [C.POINTER(MldbSmplConfig)]),
+    "mldb_smpl_configure": (C.c_int, [_P, C.POINTER(MldbSmplConfig)]),
+    "mldb_smpl_forward": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
@@ -200,4 +211,10 @@ def default_a2m_config() -> MldbA2mConfig:
 def default_stgcn_config() -> MldbStgcnConfig:
     cfg = MldbStgcnConfig()
     lib().mldb_default_stgcn_config(C.byref(cfg))
+    return cfg
+
+
+def default_smpl_config() -> MldbSmplConfig:
+    cfg = MldbSmplConfig()
+    lib().mldb_default_smpl_config(C.byref(cfg))
     return cfg

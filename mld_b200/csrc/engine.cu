@@ -1,6 +1,6 @@
 // libmldb200 engine: handles and their options, the state-dict spec and weight packing of the sampling models,
 // scheduler tables, plans and CUDA-graph capture.  The models' forward passes live in stack.cu (transformer stacks),
-// denoiser.cu, vae.cu, text_tower.cu, t2m.cu, a2m.cu and stgcn.cu.
+// denoiser.cu, vae.cu, text_tower.cu, t2m.cu, a2m.cu, stgcn.cu and smpl.cu.
 #include "engine.h"
 
 #include <math.h>
@@ -431,7 +431,7 @@ extern "C" int mldb_create(const mldb_config* cfg, int device, mldb_handle** out
   // kernel setup, on this handle's device (the shared-memory opt-ins apply per device): each step records its own
   // message in mldb_last_error() when it fails
   if (!simt_init() || !mma_attention_init() || !tc_attention_init() || !gru_tc_init() ||
-      !tconv_tc_init()) { delete h; return MLDB_ERR_CUDA; }
+      !tconv_tc_init() || !smpl_tc_init()) { delete h; return MLDB_ERR_CUDA; }
   h->tc = tc_create(device);
   if (!h->tc) { delete h; return MLDB_ERR_CUDA; }
   const char* env = getenv("MLDB_GEMM");
@@ -508,6 +508,8 @@ extern "C" int mldb_set_option(mldb_handle* h, const char* name, const char* val
     h->a2m.chunk = std::max(atoi(value), 0);
   } else if (!strcmp(name, "stgcn_chunk")) {
     h->stgcn.chunk = std::max(atoi(value), 0);
+  } else if (!strcmp(name, "smpl_chunk")) {
+    h->smpl.chunk = std::max(atoi(value), 0);
   } else {
     FAIL(MLDB_ERR_INVALID, "unknown option %s", name);
   }
@@ -609,6 +611,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
   if (h->t2m.on) TRY(pack_t2m(h));
   if (h->a2m.on) TRY(pack_a2m(h));
   if (h->stgcn.on) TRY(pack_stgcn(h));
+  if (h->smpl.on) TRY(pack_smpl(h));
   for (auto& kv : h->raw) { kv.second.host.clear(); kv.second.host.shrink_to_fit(); }
   h->finalized = true;
   return MLDB_OK;

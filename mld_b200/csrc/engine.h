@@ -187,6 +187,22 @@ struct StgcnW {
   GrowBuf col, acc;               // gemm=simt: the temporal convolution's im2col (split16) and its fp32 GEMM output
 };
 
+// SMPL layer (mldb_smpl_configure): zero betas, 24 joints, V vertices
+struct SmplW {
+  bool on = false;
+  mldb_smpl_config cfg{};
+  float J[24 * 3] = {};           // rest joints J_regressor v_template (computed in double)
+  int parents[24] = {};
+  LinW posedirs;                  // [3 V', 256]: posedirs^T (K 207 zero padded), 32-vertex tiles coordinate-planar
+  float* v_template = nullptr;    // [V', 3] fp32, V' = V rounded up to 32, zero past V
+  float* lbsw = nullptr;          // [V' / 32][24][32] fp32 lbs_weights, transposed per vertex tile
+  uint32_t* jmask = nullptr;      // [V' / 32] joints with a non-zero weight in the tile
+  int chunk = 0;                  // option smpl_chunk (0: the vertex path's workspace budget, the joints unchunked)
+  // workspace of mldb_smpl_forward (vertices)
+  GrowBuf feat;                   // split16 [frames, 256]: the pose features (R_j - I), the LBS GEMM's A
+  GrowBuf xf;                     // fp32 [frames][24 * 12 + 4]: A_j, valid, translation offset
+};
+
 struct RawTensor {
   std::vector<float> host;
   std::vector<int64_t> shape;
@@ -271,6 +287,7 @@ struct mldb_handle {
   T2mW t2m;            // T2M evaluator (mldb_t2m_configure)
   A2mW a2m;            // HumanAct12 action classifier (mldb_a2m_configure)
   StgcnW stgcn;        // UESTC action classifier (mldb_stgcn_configure)
+  SmplW smpl;          // SMPL layer (mldb_smpl_configure)
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;
@@ -408,6 +425,7 @@ int pack_text(mldb_handle* h);
 int pack_t2m(mldb_handle* h);
 int pack_a2m(mldb_handle* h);   // a2m.cu
 int pack_stgcn(mldb_handle* h); // stgcn.cu
+int pack_smpl(mldb_handle* h);  // smpl.cu
 
 // comm.cu
 void mldb_comm_release(mldb_handle* h);

@@ -188,5 +188,7 @@ bool tconv_tc_init();                                            // per device, 
 bool tconv_tc_supported(const TconvArgs& a);                     // C in {64, 128, 256}, C_res % 64 == 0, stride 1 | 2
 // at most sm_count CTAs; false: tensor-map encoding failed, nothing launched
 bool tconv_tc(const TconvArgs& a, int sm_count, cudaStream_t st);
+// --- the SMPL layer's skinning kernel (smpl.cu) ---
+bool smpl_tc_init();                                             // per device, outside stream capture
 // --- wgmma implementations (gemm_tc.cu) ---
 struct TcCtx;

@@ -298,6 +298,34 @@ class Engine:
               "mldb_stgcn_classify")
         return yhat, feats
 
+    # ------------------------------------------------------------------ SMPL layer
+    def smpl_configure(self, scfg):
+        """Add the SMPL model's keys (``smpl.`` prefix) to the strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_smpl_configure(self._h, C.byref(scfg)), "mldb_smpl_configure")
+        self.smpl_cfg = scfg
+
+    def smpl_forward(self, feats: torch.Tensor, mask: Optional[torch.Tensor], jointstype: int,
+                     vertstrans: bool) -> torch.Tensor:
+        """Rotation2xyz on rot6d features [B, T, 150] (MLD's layout before its view / permute) with an optional
+        bool mask [B, T] -> [B, 24, 3, T] (SMPL_JOINTS) or [B, V, 3, T] (SMPL_VERTICES), float32."""
+        sc = self._configured("smpl_cfg", "the SMPL layer was not configured (smpl_configure) before finalize()")
+        if feats.dim() != 3 or feats.shape[0] < 1 or feats.shape[1] < 1 or feats.shape[2] != 150:
+            raise ValueError(f"feats must be [B >= 1, T >= 1, 150], got {tuple(feats.shape)}")
+        if jointstype not in (_lib.SMPL_JOINTS, _lib.SMPL_VERTICES):
+            raise ValueError(f"jointstype must be SMPL_JOINTS or SMPL_VERTICES, got {jointstype}")
+        f = _f32c(feats, self.device)
+        B, T = f.shape[:2]
+        md = None
+        if mask is not None:
+            if tuple(mask.shape) != (B, T):
+                raise ValueError(f"mask must be [{B}, {T}], got {tuple(mask.shape)}")
+            md = mask.to(device=self.device, dtype=torch.uint8).contiguous()
+        n = 24 if jointstype == _lib.SMPL_JOINTS else sc.num_vertices
+        out = torch.empty((B, n, 3, T), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_smpl_forward(self._h, _ptr(f), _ptr(md), B, T, int(jointstype), int(bool(vertstrans)),
+                                         _ptr(out), self._stream()), "mldb_smpl_forward")
+        return out
+
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:
         """Which kernel each operator was enqueued on since the last reset (mldb_kernel_stats)."""
         arr = (C.c_int64 * len(_lib.KSTAT_NAMES))()

@@ -11,6 +11,7 @@ math runs in ``libmldb200.so``.  Inference only (parameters do not require grad)
 """
 from __future__ import annotations
 
+import itertools
 from typing import Dict, List, Optional, Sequence
 
 import torch
@@ -60,15 +61,19 @@ class _EngineModule(nn.Module):
         self._weights_epoch += 1
         return super().load_state_dict(state_dict, strict=strict, **kw)
 
+    def _engine_state_dict(self) -> Dict[str, torch.Tensor]:
+        """The tensors uploaded to the engine, keyed without ``_prefix``."""
+        return self.state_dict()
+
     def engine(self) -> Engine:
-        dev = next(self.parameters()).device
+        dev = next(itertools.chain(self.parameters(), self.buffers())).device
         if dev.type != "cuda":
             raise RuntimeError(f"{type(self).__name__} runs on a H100 only: move it with .cuda() "
                                "(no CPU/PyTorch fallback exists)")
         if self._engine is None or self._engine_epoch != self._weights_epoch or self._engine.device != dev:
             eng = Engine(self._make_config(), dev)
             self._configure_engine(eng)
-            eng.load_state_dict(self.state_dict(), self._prefix)
+            eng.load_state_dict(self._engine_state_dict(), self._prefix)
             eng.finalize()
             self._engine, self._engine_epoch = eng, self._weights_epoch
         return self._engine

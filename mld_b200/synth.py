@@ -435,3 +435,68 @@ def uestc_motions(B: int, T: int = 60, seed: int = 31, njoints: int = 24) -> Ten
     col0 = torch.stack([c + kx * kx * C1, kz * s + ky * kx * C1, -ky * s + kz * kx * C1], 2)
     col1 = torch.stack([-kz * s + kx * ky * C1, c + ky * ky * C1, kx * s + kz * ky * C1], 2)
     return torch.cat([col0, col1], 2).float()                          # [B, J, 6, T]
+
+
+SMPL_PARENTS = (-1, 0, 0, 0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 9, 9, 12, 13, 14, 16, 17, 18, 19, 20, 21)   # SMPL's kintree
+
+
+def smpl_model(seed: int = 99, V: int = 333, dense_every: int = 37) -> Dict[str, Tensor]:
+    """A seeded synthetic SMPL model in the layout ``mld_b200.smpl.load_smpl`` returns: SMPL's public parent table, a
+    body-sized ``v_template`` [V, 3] (metres), ``J_regressor`` [24, V] with sparse convex rows (6 vertices each),
+    ``lbs_weights`` [V, 24] whose rows sum to 1 with 1 to 4 non-zeros, except every ``dense_every``-th row which
+    weighs all 24 joints, and ``posedirs`` [207, 3 V] of size about 1e-2."""
+    g = torch.Generator().manual_seed(seed)
+    lo, hi = torch.tensor([-0.45, -1.15, -0.15]), torch.tensor([0.45, 0.55, 0.15])
+    vt = lo + (hi - lo) * torch.rand(V, 3, generator=g)
+    jr = torch.zeros(24, V)
+    for j in range(24):
+        idx = torch.randperm(V, generator=g)[:min(6, V)]
+        w = torch.rand(len(idx), generator=g) + 0.1
+        jr[j, idx] = w / w.sum()
+    lw = torch.zeros(V, 24)
+    for v in range(V):
+        k = 24 if dense_every and v % dense_every == 0 else 1 + int(torch.randint(0, 4, (1,), generator=g))
+        idx = torch.randperm(24, generator=g)[:k]
+        w = torch.rand(k, generator=g) + 0.05
+        lw[v, idx] = w / w.sum()
+    posedirs = torch.randn(207, 3 * V, generator=g) * 1e-2
+    return {"v_template": vt, "posedirs": posedirs, "J_regressor": jr, "lbs_weights": lw,
+            "parents": torch.tensor(SMPL_PARENTS, dtype=torch.int64)}
+
+
+def write_smpl_pkl(path: str, model: Dict[str, Tensor], array=None):
+    """Write ``model`` (``smpl_model``'s layout) as ``SMPL_NEUTRAL.pkl`` is laid out: ``posedirs`` [V, 3, 207],
+    ``weights``, ``kintree_table`` [2, 24] (row 0 the parents, the root's 4294967295), a scipy sparse
+    ``J_regressor``, zero ``shapedirs`` [V, 3, 10] and ``f``.  ``array`` wraps every dense array (a chumpy stand-in)."""
+    import pickle
+
+    import numpy as np
+    import scipy.sparse
+    wrap = array or (lambda a: a)
+    V = model["v_template"].shape[0]
+    parents = model["parents"].numpy().astype(np.int64).copy()
+    parents[0] = 4294967295
+    data = {
+        "v_template": wrap(model["v_template"].double().numpy()),
+        "posedirs": wrap(model["posedirs"].double().numpy().T.reshape(V, 3, 207)),
+        "J_regressor": scipy.sparse.csc_matrix(model["J_regressor"].double().numpy()),
+        "weights": wrap(model["lbs_weights"].double().numpy()),
+        "kintree_table": np.stack([parents, np.arange(24, dtype=np.int64)]),
+        "shapedirs": wrap(np.zeros((V, 3, 10))),
+        "f": np.zeros((1, 3), dtype=np.uint32),
+    }
+    with open(path, "wb") as f:
+        pickle.dump(data, f, protocol=2)
+
+
+def smpl_feats(B: int, T: int = 60, seed: int = 51) -> Tensor:
+    """Rot6d features ``[B, T, 150]`` as ``MLD`` holds them (``view(B, T, 6, 25)``): ``uestc_motions``'s smooth
+    rotations for the 24 joints and a smooth root translation (metres) in column 24."""
+    rot = uestc_motions(B, T, seed=seed)                                   # [B, 24, 6, T]
+    g = torch.Generator().manual_seed(seed + 1)
+    t = torch.arange(T, dtype=torch.float32) / 30.0
+    trans = torch.randn(B, 3, 1, generator=g) * 0.3 + torch.randn(B, 3, 1, generator=g) * 0.5 * t
+    x = torch.zeros(B, T, 6, 25)
+    x[..., :24] = rot.permute(0, 3, 2, 1)
+    x[:, :, :3, 24] = trans.permute(0, 2, 1)
+    return x.reshape(B, T, 150)
