@@ -330,6 +330,49 @@ int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg);
  * indices with gemm=simt / attn=simt), the row LayerNorms under MLDB_KSTAT_TEXT_LN. */
 int mldb_text_encode(mldb_handle* h, const int64_t* ids, int32_t n, int32_t L, int32_t mode, float* out, void* stream);
 
+/* ---- BERT text encoder (MldTextEncoder with a "bert" model path, mld_clip.py:44-46,65-68,83-86): token ids and the
+ * attention mask -> last_hidden_state, the denoiser's context.  DistilBERT (the shipped distilbert-base-uncased) or
+ * BERT: word + position (+ token-type row 0) embedding and LayerNorm, then `layers` post-norm blocks (non-causal
+ * self-attention over the row's real tokens -> + residual -> LayerNorm, lin1 -> exact GELU -> lin2 -> + residual ->
+ * LayerNorm).  A handle holds one text tower: this and mldb_text_configure exclude each other (MLDB_ERR_STATE). */
+#define MLDB_BERT_ABI_VERSION 1
+#define MLDB_BERT_DISTILBERT 0  /* DistilBertModel: keys embeddings.word_embeddings / position_embeddings / LayerNorm,
+                                   transformer.layer.{i}.attention.{q,k,v,out}_lin, sa_layer_norm, ffn.lin1 / lin2,
+                                   output_layer_norm */
+#define MLDB_BERT_BERT 1        /* BertModel: embeddings.{word,position,token_type}_embeddings / LayerNorm,
+                                   encoder.layer.{i}.attention.self.{query,key,value}, attention.output.dense /
+                                   LayerNorm, intermediate.dense, output.dense / LayerNorm; pooler.dense.* accepted and
+                                   not uploaded (it does not reach last_hidden_state) */
+typedef struct mldb_bert_config {
+  int32_t abi_version;       /* must be MLDB_BERT_ABI_VERSION */
+  int32_t family;            /* MLDB_BERT_DISTILBERT | MLDB_BERT_BERT */
+  int32_t vocab_size;        /* 30522 */
+  int32_t max_positions;     /* 512; 1 .. 512 */
+  int32_t type_vocab;        /* BERT: token_type_embeddings rows (2); ignored for DistilBERT */
+  int32_t hidden;            /* 768 (a multiple of 128, <= 1024) */
+  int32_t heads;             /* 12 (head_dim 64 or 128 runs the wgmma attention) */
+  int32_t layers;            /* 6 */
+  int32_t ff;                /* 3072 */
+  float   ln_eps;            /* 1e-12 */
+} mldb_bert_config;
+void mldb_default_bert_config(mldb_bert_config* cfg);   /* distilbert-base-uncased */
+/* Add the tower's keys to the strict key spec; after mldb_create, before mldb_finalize_weights.  Keys are
+ * "text_encoder.text_model." + the Hugging Face model's state_dict() keys ("text_encoder.text_model.transformer.layer.0.
+ * attention.q_lin.weight", ...); an embeddings.position_ids buffer is not one of them.  q/k/v are packed into one
+ * [3 * hidden, hidden] operand at finalize. */
+int mldb_bert_configure(mldb_handle* h, const mldb_bert_config* cfg);
+/* Replaces: MldTextEncoder.forward after the tokenizer for "bert" (text_model(**text_inputs).last_hidden_state).
+ *   ids      device int64 [n, L], 1 <= L <= max_positions; an id outside [0, vocab_size) yields a NaN row
+ *   lengths  device int32 [n], each in [1, L]: row s's attention mask is lengths[s] ones then zeros (right padding);
+ *            token types are all zero.  Copied to the host and checked before anything is launched (the call
+ *            synchronises `stream`)
+ *   out      [n, L, hidden]: every position, padding positions included (a padding query attends to the real keys)
+ * Enqueued eagerly on `stream`; the workspace grows on demand (outside any capture: synchronises the device when it
+ * does).  Per call: 1 + 2 * layers MLDB_KSTAT_TEXT_LN, 4 * layers GEMMs and `layers` attentions.  The attention is
+ * k_attn_tc (ATTN_TC) for L <= 256 and the CUDA-core kernel (ATTN_SIMT) for longer rows. */
+int mldb_bert_encode(mldb_handle* h, const int64_t* ids, const int32_t* lengths, int32_t n, int32_t L, float* out,
+                     void* stream);
+
 /* ---- T2M evaluator (MLD.t2m_eval, mld/models/modeltype/mld.py:618-708): the movement, motion and text encoders of
  * Guo et al.'s text-motion matching model (mld/models/architectures/t2m_motionenc.py, t2m_textenc.py) whose embeddings
  * feed R-precision, matching score, FID, diversity and MultiModality.  Weights come from finest.tar (keys text_encoder,

@@ -26,6 +26,9 @@ KSTAT_NAMES = ("gemm_tc", "gemm_ln_tc", "ffn_tc", "attn_tc", "attn_mma", "attn_s
 # CLIP text tower (mldb_text_config, mldb_text_encode)
 MLDB_TEXT_ABI_VERSION = 1
 TEXT_HIDDEN, TEXT_POOLED = 0, 1
+# BERT text tower (mldb_bert_config, mldb_bert_encode)
+MLDB_BERT_ABI_VERSION = 1
+BERT_DISTILBERT, BERT_BERT = 0, 1
 # T2M evaluator (mldb_t2m_config, mldb_t2m_*)
 MLDB_T2M_ABI_VERSION = 1
 T2M_TEXT, T2M_MOVEMENT, T2M_MOTION = 1, 2, 4
@@ -62,6 +65,15 @@ class MldbTextConfig(C.Structure):
         ("abi_version", C.c_int32), ("vocab_size", C.c_int32), ("max_positions", C.c_int32),
         ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32), ("ff", C.c_int32),
         ("projection_dim", C.c_int32), ("eos_token_id", C.c_int32), ("ln_eps", C.c_float),
+    ]
+
+
+class MldbBertConfig(C.Structure):
+    """``mldb_bert_config`` (include/mldb.h)."""
+    _fields_ = [
+        ("abi_version", C.c_int32), ("family", C.c_int32), ("vocab_size", C.c_int32), ("max_positions", C.c_int32),
+        ("type_vocab", C.c_int32), ("hidden", C.c_int32), ("heads", C.c_int32), ("layers", C.c_int32),
+        ("ff", C.c_int32), ("ln_eps", C.c_float),
     ]
 
 
@@ -127,6 +139,9 @@ _SIGNATURES = {
     "mldb_default_text_config": (None, [C.POINTER(MldbTextConfig)]),
     "mldb_text_configure": (C.c_int, [_P, C.POINTER(MldbTextConfig)]),
     "mldb_text_encode": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_default_bert_config": (None, [C.POINTER(MldbBertConfig)]),
+    "mldb_bert_configure": (C.c_int, [_P, C.POINTER(MldbBertConfig)]),
+    "mldb_bert_encode": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, _P, _P]),
     "mldb_default_t2m_config": (None, [C.POINTER(MldbT2mConfig)]),
     "mldb_t2m_configure": (C.c_int, [_P, C.POINTER(MldbT2mConfig)]),
     "mldb_t2m_movement": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
@@ -193,6 +208,12 @@ def default_config() -> MldbConfig:
 def default_text_config() -> MldbTextConfig:
     cfg = MldbTextConfig()
     lib().mldb_default_text_config(C.byref(cfg))
+    return cfg
+
+
+def default_bert_config() -> MldbBertConfig:
+    cfg = MldbBertConfig()
+    lib().mldb_default_bert_config(C.byref(cfg))
     return cfg
 
 

@@ -608,6 +608,7 @@ extern "C" int mldb_finalize_weights(mldb_handle* h, void* stream) {
     if (actor_enc) TRY(pack_actor_encoder(h));
   }
   if (h->text.on) TRY(pack_text(h));
+  if (h->bert.on) TRY(pack_bert(h));
   if (h->t2m.on) TRY(pack_t2m(h));
   if (h->a2m.on) TRY(pack_a2m(h));
   if (h->stgcn.on) TRY(pack_stgcn(h));

@@ -116,6 +116,21 @@ struct TextW {
   GrowBuf pooled;                 // [seqs, hidden] final LN of the eos rows (split16, A of text_projection)
 };
 
+// BERT / DistilBERT text tower (mldb_bert_configure): post-norm layers; ln1 / ln2 are the attention / output
+// LayerNorms (sa_layer_norm / output_layer_norm)
+struct BertW {
+  bool on = false;
+  mldb_bert_config cfg{};
+  std::vector<TextLayerW> layers;
+  LnW emb_ln;
+  float* word = nullptr;          // [vocab, hidden] fp32
+  float* pos = nullptr;           // [max_positions, hidden] fp32
+  float* type0 = nullptr;         // BERT: token_type_embeddings row 0 [hidden]; DistilBERT: null
+  // workspace of mldb_bert_encode
+  GrowBuf x;                      // [rows, hidden] fp32 residual stream (post-norm: each LayerNorm writes it back)
+  GrowBuf a, qkv, att, h;         // LayerNorm output, q|k|v, attention output, lin1 output (split16)
+};
+
 // T2M evaluator (mldb_t2m_configure): bidirectional GRU + BiGRUCo head, the movement convolutions
 struct GruW {
   int H = 0;
@@ -284,6 +299,7 @@ struct mldb_handle {
   float* global_token = nullptr;     // [2*n_lat, d]; ActorVae: [mu_token; logvar_token]
   float* mean = nullptr; float* stdv = nullptr; int nstat = 0;
   TextW text;          // CLIP text tower (mldb_text_configure)
+  BertW bert;          // BERT text tower (mldb_bert_configure); a handle holds one of the two
   T2mW t2m;            // T2M evaluator (mldb_t2m_configure)
   A2mW a2m;            // HumanAct12 action classifier (mldb_a2m_configure)
   StgcnW stgcn;        // UESTC action classifier (mldb_stgcn_configure)
@@ -420,8 +436,10 @@ int dec_plan(mldb_handle* h, int B, int T, Plan** out);
 int run_decode(mldb_handle* h, const float* z, const int32_t* lengths, int B, int T, float* feats_out, cudaStream_t st,
                Plan** plan_out);
 int run_f2j(mldb_handle* h, const float* feats, int B, int T, float* joints, cudaStream_t st);
-// text_tower.cu, t2m.cu, a2m.cu, stgcn.cu
+// text_tower.cu, bert.cu, t2m.cu, a2m.cu, stgcn.cu
 int pack_text(mldb_handle* h);
+int pack_bert(mldb_handle* h);
+void op_text_ln(mldb_handle* h, const TextLnArgs& a, cudaStream_t st);   // text_ln counted under MLDB_KSTAT_TEXT_LN
 int pack_t2m(mldb_handle* h);
 int pack_a2m(mldb_handle* h);   // a2m.cu
 int pack_stgcn(mldb_handle* h); // stgcn.cu

@@ -101,17 +101,22 @@ bool tc_attention_supported(const AttnArgs& a);
 // at most sm_count CTAs; false: tensor-map encoding failed, nothing launched
 bool tc_attention(const AttnArgs& a, int sm_count, cudaStream_t st);
 bool simt_init();                                         // reads MLDB_PDL; per device, outside stream capture
-// --- CLIP text tower row kernels (text_ln.cu) ---
+// --- text tower row kernels (text_ln.cu) ---
 // One warp per row, d a multiple of 128 up to 1024, exact two-pass statistics, no shared memory.
-//   TEXT_LN_ROWS:  out = LN(x[r])                                   (pre-norm LN1 / LN2, final LN of every row)
-//   TEXT_LN_EMBED: x[r] = tok[ids[r]] + pos[r % L]; out = LN(x[r])  (layer 0; an id outside [0, vocab) -> NaN row)
-//   TEXT_LN_EOS:   out[s] = LN(x[s * L + eos_pos(ids[s, :])])       (pooled mode: only the gathered rows)
-enum TextLnMode { TEXT_LN_ROWS = 0, TEXT_LN_EMBED = 1, TEXT_LN_EOS = 2 };
+//   TEXT_LN_ROWS:     out = LN(x[r])                                   (CLIP: pre-norm LN1 / LN2, final LN of every
+//                                                                      row; BERT: the post-norm LN with out_f32 = x)
+//   TEXT_LN_EMBED:    x[r] = tok[ids[r]] + pos[r % L]; out = LN(x[r])  (CLIP layer 0; an id outside [0, vocab) -> NaN
+//                                                                      row)
+//   TEXT_LN_EOS:      out[s] = LN(x[s * L + eos_pos(ids[s, :])])       (pooled mode: only the gathered rows)
+//   TEXT_LN_EMBED_LN: out = LN(tok[ids[r]] + pos[r % L] (+ type0))     (BERT embeddings; x is not written: out_f32 = x
+//                                                                      makes the normalised row the residual stream)
+enum TextLnMode { TEXT_LN_ROWS = 0, TEXT_LN_EMBED = 1, TEXT_LN_EOS = 2, TEXT_LN_EMBED_LN = 3 };
 struct TextLnArgs {
   int mode = TEXT_LN_ROWS;
-  float* x = nullptr;                 // fp32 residual stream [rows, d] (written in TEXT_LN_EMBED, read otherwise)
+  float* x = nullptr;                 // fp32 residual stream [rows, d] (written in TEXT_LN_EMBED, read by ROWS / EOS)
   const int64_t* ids = nullptr; int L = 0;
   const float* tok = nullptr; const float* pos = nullptr; int vocab = 0;
+  const float* type0 = nullptr;       // TEXT_LN_EMBED_LN: token-type row 0 added to every row (null: none)
   int eos_id = 0;                     // eos_id == 2: eos_pos = argmax(ids) (legacy configs); else first id == eos_id, or 0
   const float* gamma = nullptr; const float* beta = nullptr; float eps = 1e-5f;
   int M = 0, d = 0;                   // output rows (TEXT_LN_EOS: sequences)

@@ -1,5 +1,6 @@
-// Row LayerNorm of the CLIP text tower (pre-norm: LN1 / LN2 of every layer, the final LN) on the fp32 residual
-// stream, fused with the token + position embedding for layer 0 and with the eos-row gather of pooled mode.
+// Row LayerNorm of the text towers on the fp32 residual stream: CLIP's pre-norm LN1 / LN2 and final LN, fused with the
+// token + position embedding for layer 0 and with the eos-row gather of pooled mode; BERT's post-norm LNs (written
+// back into the stream) and its embedding LN.
 // One warp per row, the row in registers (d / 32 floats per lane, float4 loads), exact two-pass statistics with
 // warp shuffles and no shared memory; the output is the split16 A operand of the next GEMM and/or fp32.
 #include "ops.cuh"
@@ -40,7 +41,7 @@ __global__ void __launch_bounds__(256) k_text_ln(const TextLnArgs a) {
   float v[NV][4];
   int64_t irow = r;
   if (a.mode == TEXT_LN_EOS) irow = (int64_t)r * a.L + eos_position(a.ids + (int64_t)r * a.L, a.L, a.eos_id, lane);
-  if (a.mode == TEXT_LN_EMBED) {
+  if (a.mode == TEXT_LN_EMBED || a.mode == TEXT_LN_EMBED_LN) {
     const int64_t id = a.ids[r];
     const bool ok = id >= 0 && id < a.vocab;            // never read outside the table: a bad id is a NaN row
     const float* te = a.tok + (ok ? id : 0) * D;
@@ -48,10 +49,16 @@ __global__ void __launch_bounds__(256) k_text_ln(const TextLnArgs a) {
 #pragma unroll
     for (int i = 0; i < NV; ++i) {
       const int n = 4 * (lane + 32 * i);
-      const float4 t = __ldg(reinterpret_cast<const float4*>(te + n)), p = __ldg(reinterpret_cast<const float4*>(pe + n));
+      float4 t = __ldg(reinterpret_cast<const float4*>(te + n));
+      const float4 p = __ldg(reinterpret_cast<const float4*>(pe + n));
+      if (a.type0) {                                     // BERT: (word + token_type) + position, torch's order
+        const float4 y = __ldg(reinterpret_cast<const float4*>(a.type0 + n));
+        t.x += y.x; t.y += y.y; t.z += y.z; t.w += y.w;
+      }
       v[i][0] = t.x + p.x; v[i][1] = t.y + p.y; v[i][2] = t.z + p.z; v[i][3] = t.w + p.w;
       if (!ok) v[i][0] = v[i][1] = v[i][2] = v[i][3] = __int_as_float(0x7fc00000);
-      *reinterpret_cast<float4*>(a.x + (int64_t)r * D + n) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
+      if (a.mode == TEXT_LN_EMBED)
+        *reinterpret_cast<float4*>(a.x + (int64_t)r * D + n) = make_float4(v[i][0], v[i][1], v[i][2], v[i][3]);
     }
   } else {
 #pragma unroll

@@ -17,7 +17,7 @@ extern "C" void mldb_default_text_config(mldb_text_config* c) {
 
 extern "C" int mldb_text_configure(mldb_handle* h, const mldb_text_config* cfg) {
   if (!h || !cfg) FAIL(MLDB_ERR_INVALID, "null argument");
-  TRY(may_configure(h, cfg->abi_version, MLDB_TEXT_ABI_VERSION, h->text.on, "text", "the text tower"));
+  TRY(may_configure(h, cfg->abi_version, MLDB_TEXT_ABI_VERSION, h->text.on || h->bert.on, "text", "the text tower"));
   const mldb_text_config& c = *cfg;
   if (c.vocab_size < 1 || c.layers < 1 || c.heads < 1 || c.ff < 1 || c.projection_dim < 1 || !(c.ln_eps > 0.0f))
     FAIL(MLDB_ERR_INVALID, "bad text config");
@@ -83,7 +83,7 @@ int pack_text(mldb_handle* h) {
 }
 
 // ----------------------------------------------------------------------------- CLIP text tower: forward
-static void op_text_ln(mldb_handle* h, const TextLnArgs& a, cudaStream_t st) { text_ln(a, st); kcount(h, MLDB_KSTAT_TEXT_LN); }
+void op_text_ln(mldb_handle* h, const TextLnArgs& a, cudaStream_t st) { text_ln(a, st); kcount(h, MLDB_KSTAT_TEXT_LN); }
 
 extern "C" int mldb_text_encode(mldb_handle* h, const int64_t* ids, int32_t n, int32_t L, int32_t mode, float* out,
                                 void* stream) {

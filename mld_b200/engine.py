@@ -176,6 +176,28 @@ class Engine:
               "mldb_text_encode")
         return out
 
+    # ------------------------------------------------------------------ BERT text tower
+    def bert_configure(self, bcfg):
+        """Add the BERT tower's keys (``text_encoder.`` prefix) to the strict key spec; before :meth:`finalize`."""
+        check(self.lib.mldb_bert_configure(self._h, C.byref(bcfg)), "mldb_bert_configure")
+        self.bert_cfg = bcfg
+
+    def bert_encode(self, ids: torch.Tensor, lengths) -> torch.Tensor:
+        """int64 token ids [n, L] + real tokens per row (each in [1, L], the right-padded attention mask) ->
+        last_hidden_state [n, L, hidden], every position, on the current stream.  Bad ids are rejected here."""
+        bc = self._configured("bert_cfg", "bert_configure() was not called before finalize()")
+        if ids.dim() != 2 or ids.shape[0] < 1 or not 1 <= ids.shape[1] <= bc.max_positions:
+            raise ValueError(f"ids must be [n, L] with 1 <= L <= {bc.max_positions}, got {tuple(ids.shape)}")
+        if int(ids.min()) < 0 or int(ids.max()) >= bc.vocab_size:
+            raise ValueError(f"token ids must lie in [0, {bc.vocab_size})")
+        d_ids = ids.to(device=self.device, dtype=torch.int64).contiguous()
+        n, L = d_ids.shape
+        ln = self._seq_lengths(lengths, n, L)
+        out = torch.empty((n, L, bc.hidden), dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_bert_encode(self._h, _ptr(d_ids), _ptr(ln), n, L, _ptr(out), self._stream()),
+              "mldb_bert_encode")
+        return out
+
     # ------------------------------------------------------------------ T2M evaluator
     def t2m_configure(self, tcfg):
         """Add the evaluator parts' keys (``t2m_textencoder.`` / ``t2m_moveencoder.`` / ``t2m_motionencoder.``) to the

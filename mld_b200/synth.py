@@ -238,6 +238,62 @@ def clip_text_ids(n: int, L: int = 77, seed: int = 7, eos_lo: int = 8, eos_hi: i
     return ids
 
 
+def bert_text_state_dict(seed: int = 5151, family: str = "distilbert", vocab_size: int = 30522,
+                         max_positions: int = 512, type_vocab: int = 2, hidden: int = 768, layers: int = 6,
+                         ff: int = 3072, **_unused) -> Dict[str, Tensor]:
+    """State dict of a BERT text tower as ``MldTextEncoder.state_dict()`` names it for a ``"bert"`` model path: its
+    ``text_model`` is the ``AutoModel``, so the keys are ``text_model.`` + those of transformers' ``DistilBertModel``
+    (``family="distilbert"``, the default shape is distilbert-base-uncased) or ``BertModel`` (``"bert"``, with its
+    pooler).  ``heads`` does not change the weights and is accepted for symmetry with the config."""
+    g, sd = _Gen(seed), {}
+    p = "text_model."
+    sd[p + "embeddings.word_embeddings.weight"] = g.normal(vocab_size, hidden, std=0.02)
+    sd[p + "embeddings.position_embeddings.weight"] = g.normal(max_positions, hidden, std=0.02)
+    if family == "bert":
+        sd[p + "embeddings.token_type_embeddings.weight"] = g.normal(type_vocab, hidden, std=0.02)
+    elif family != "distilbert":
+        raise ValueError(f"family must be 'distilbert' or 'bert', got {family!r}")
+    _ln(sd, g, p + "embeddings.LayerNorm.", hidden)
+    for i in range(layers):
+        if family == "distilbert":
+            q = f"{p}transformer.layer.{i}."
+            lin = [q + f"attention.{n}." for n in ("q_lin", "k_lin", "v_lin", "out_lin")]
+            ln1, fc1, fc2, ln2 = q + "sa_layer_norm.", q + "ffn.lin1.", q + "ffn.lin2.", q + "output_layer_norm."
+        else:
+            q = f"{p}encoder.layer.{i}."
+            lin = [q + f"attention.self.{n}." for n in ("query", "key", "value")] + [q + "attention.output.dense."]
+            ln1, fc1, fc2, ln2 = (q + "attention.output.LayerNorm.", q + "intermediate.dense.", q + "output.dense.",
+                                  q + "output.LayerNorm.")
+        for k in lin:
+            sd[k + "weight"] = g.xavier(hidden, hidden)
+            sd[k + "bias"] = g.normal(hidden, std=0.02)
+        _ln(sd, g, ln1, hidden)
+        sd[fc1 + "weight"] = g.xavier(ff, hidden)
+        sd[fc1 + "bias"] = g.normal(ff, std=0.02)
+        sd[fc2 + "weight"] = g.xavier(hidden, ff)
+        sd[fc2 + "bias"] = g.normal(hidden, std=0.02)
+        _ln(sd, g, ln2, hidden)
+    if family == "bert":
+        sd[p + "pooler.dense.weight"] = g.xavier(hidden, hidden)
+        sd[p + "pooler.dense.bias"] = g.normal(hidden, std=0.02)
+    return sd
+
+
+def bert_text_ids(n: int, L: int, seed: int = 8, len_lo: int = 8, len_hi: int = 30, vocab_size: int = 30522,
+                  cls: int = 101, sep: int = 102, pad: int = 0):
+    """Tokenizer-shaped rows as ``tokenizer(texts, padding=True)`` gives them: ``(ids [n, L] int64, lengths [n])``
+    with each row [CLS], random word ids, [SEP] over its seeded length in [len_lo, len_hi] (clamped to [1, L]), then
+    [PAD] on the right."""
+    g = torch.Generator().manual_seed(seed)
+    lengths = torch.randint(len_lo, len_hi + 1, (n,), generator=g).clamp(1, L)
+    ids = torch.randint(min(999, vocab_size // 2), vocab_size, (n, L), generator=g)
+    t = torch.arange(L).expand(n, L)
+    ids[t == lengths[:, None] - 1] = sep
+    ids[:, 0] = cls
+    ids[t >= lengths[:, None]] = pad
+    return ids, lengths
+
+
 # ---------------------------------------------------------------------------- T2M evaluator (finest.tar layout)
 T2M_DIMS = dict(dim_word=300, dim_pos_ohot=15, dim_text_hidden=512, dim_coemb_hidden=512, dim_pose=259,
                 dim_move_hidden=512, dim_move_latent=512, dim_motion_hidden=1024, dim_motion_latent=512)
