@@ -511,6 +511,28 @@ int mldb_smpl_configure(mldb_handle* h, const mldb_smpl_config* cfg);
 int mldb_smpl_forward(mldb_handle* h, const float* feats, const uint8_t* mask, int32_t B, int32_t T,
                       int32_t jointstype, int32_t vertstrans, float* out, void* stream);
 
+/* ---- APE / AVE of the text-to-motion test (TemosMetric: ComputeMetrics.update, mld/models/metrics/compute.py, with
+ * the Rifke round trip of transforms/joints2jfeats/rifke.py).  Needs no weights and no finalize: any handle runs it.
+ * The joint tables (mld/utils/joints.py) and the meter factors live in the library. */
+#define MLDB_APE_AVE_ABI_VERSION 1
+#define MLDB_JOINTS_HUMANML3D 0   /* J = 22, force_in_meter factor 1000 * 0.75 / 480 */
+#define MLDB_JOINTS_MMM 1         /* KIT: J = 21, factor 1000 */
+/* Replaces: the per-batch increments of ComputeMetrics.update(jts_text, jts_ref, lengths).
+ *   jts_text, jts_ref  [B, T, J, 3] fp32, padded to T; every frame, padding included, enters the floor (softmin of
+ *                      the lowest foot height), as in the reference
+ *   lengths            device int32 [B], each in [2, T] (the caller checks them: a sequence whose length is not
+ *                      gives NaN in every output)
+ *   force_in_meter     1: positions divided by the jointstype's factor; 0: by 1
+ *   out                fp32 [4 J + 2], in ComputeMetrics.metrics order: APE_root [1], APE_traj [1], APE_pose [J - 1],
+ *                      APE_joints [J], AVE_root [1], AVE_traj [1], AVE_pose [J - 1], AVE_joints [J]: the sums over
+ *                      the batch that update adds to the metric's states
+ * The arguments are checked on the host before anything is launched.  Enqueued on `stream` with no host
+ * synchronisation; the handle's partial-row workspace is allocated once, at the first call.  Two kernels
+ * (MLDB_KSTAT_MISC): k_ape_ave, one CTA per sequence in double, and k_ape_ave_reduce, the fixed-order sum over the
+ * batch, so a call gives the same bits every time. */
+int mldb_ape_ave(mldb_handle* h, const float* jts_text, const float* jts_ref, const int32_t* lengths, int32_t B,
+                 int32_t T, int32_t J, int32_t jointstype, int32_t force_in_meter, float* out, void* stream);
+
 /* Introspection */
 const char* mldb_last_error(void);
 int mldb_abi_version(void);

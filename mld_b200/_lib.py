@@ -39,6 +39,9 @@ MLDB_STGCN_ABI_VERSION = 1
 # SMPL layer (mldb_smpl_config, mldb_smpl_forward)
 MLDB_SMPL_ABI_VERSION = 1
 SMPL_JOINTS, SMPL_VERTICES = 0, 1
+# APE / AVE metric (mldb_ape_ave)
+MLDB_APE_AVE_ABI_VERSION = 1
+JOINTS_HUMANML3D, JOINTS_MMM = 0, 1
 
 
 class MldbConfig(C.Structure):
@@ -156,6 +159,7 @@ _SIGNATURES = {
     "mldb_default_smpl_config": (None, [C.POINTER(MldbSmplConfig)]),
     "mldb_smpl_configure": (C.c_int, [_P, C.POINTER(MldbSmplConfig)]),
     "mldb_smpl_forward": (C.c_int, [_P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_ape_ave": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_comm_unique_id": (C.c_int, [_P]),
     "mldb_comm_init": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),
     "mldb_comm_attach": (C.c_int, [_P, _P, C.c_int32, C.c_int32]),

@@ -1,6 +1,6 @@
 // libmldb200 engine: handles and their options, the state-dict spec and weight packing of the sampling models,
 // scheduler tables, plans and CUDA-graph capture.  The models' forward passes live in stack.cu (transformer stacks),
-// denoiser.cu, vae.cu, text_tower.cu, t2m.cu, a2m.cu, stgcn.cu and smpl.cu.
+// denoiser.cu, vae.cu, text_tower.cu, t2m.cu, a2m.cu, stgcn.cu and smpl.cu; the APE / AVE metric in metrics.cu.
 #include "engine.h"
 
 #include <math.h>

@@ -304,6 +304,7 @@ struct mldb_handle {
   A2mW a2m;            // HumanAct12 action classifier (mldb_a2m_configure)
   StgcnW stgcn;        // UESTC action classifier (mldb_stgcn_configure)
   SmplW smpl;          // SMPL layer (mldb_smpl_configure)
+  double* ape_part = nullptr;   // mldb_ape_ave's partial rows (metrics.cu), allocated at its first call
   // scheduler
   std::vector<float> alphas_cumprod;
   std::vector<int64_t> timesteps;

@@ -348,6 +348,26 @@ class Engine:
                                          _ptr(out), self._stream()), "mldb_smpl_forward")
         return out
 
+    # ------------------------------------------------------------------ APE / AVE metric
+    def ape_ave(self, jts_text: torch.Tensor, jts_ref: torch.Tensor, lengths: torch.Tensor, jointstype: int,
+                force_in_meter: bool) -> torch.Tensor:
+        """ComputeMetrics.update's increments of joints [B, T, J, 3] (contiguous float32 on this device) with device
+        int32 lengths [B], each in [2, T] -> float32 [4 J + 2] in ComputeMetrics.metrics order (mldb_ape_ave)."""
+        if jts_text.dim() != 4 or jts_text.shape[-1] != 3 or jts_text.shape != jts_ref.shape:
+            raise ValueError(f"joints must be two [B, T, J, 3] tensors, got {tuple(jts_text.shape)} and "
+                             f"{tuple(jts_ref.shape)}")
+        for t in (jts_text, jts_ref):
+            if t.dtype != torch.float32 or t.device != self.device or not t.is_contiguous():
+                raise ValueError("joints must be contiguous float32 tensors on the engine's device")
+        B, T, J = jts_text.shape[:3]
+        if lengths.dtype != torch.int32 or lengths.device != self.device or tuple(lengths.shape) != (B,):
+            raise ValueError(f"lengths must be int32 [{B}] on the engine's device")
+        out = torch.empty(4 * J + 2, dtype=torch.float32, device=self.device)
+        check(self.lib.mldb_ape_ave(self._h, _ptr(jts_text), _ptr(jts_ref), _ptr(lengths.contiguous()), B, T, J,
+                                    int(jointstype), int(bool(force_in_meter)), _ptr(out), self._stream()),
+              "mldb_ape_ave")
+        return out
+
     def kernel_stats(self, reset: bool = False) -> Dict[str, int]:
         """Which kernel each operator was enqueued on since the last reset (mldb_kernel_stats)."""
         arr = (C.c_int64 * len(_lib.KSTAT_NAMES))()
