@@ -58,22 +58,9 @@ struct TcParams {
 
 enum { EPI_FAST = 0, EPI_LN = 1, EPI_GENERIC = 2, EPI_RES = 3, EPI_F32 = 4 };     // epilogue variants of k_gemm_tc (see the kernel)
 
+// [A hi | A lo | W hi | W lo] stages (tc_common.cuh): two of 96 KB at BN = 256, three of 64 KB at BN = 128
 template <int BN>
-struct TileCfg {
-  static constexpr int A_BYTES = BM * BK * 2;          // one plane of the A tile (16 KB)
-  static constexpr int W_BYTES = BN * BK * 2;          // one plane of the W tile
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;       // 96 KB (BN = 256) / 64 KB
-  static constexpr int STAGES = BN == 256 ? 2 : 3;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;   // + barriers + alignment slack
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-};
-
-__device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, float x0, float x1) {
-  uint32_t h, l;
-  split2(x0, x1, h, l);
-  *reinterpret_cast<uint32_t*>(hi + o) = h;
-  *reinterpret_cast<uint32_t*>(lo + o) = l;
-}
+using TileCfg = StageLayout<BN, BN == 256 ? 2 : 3>;
 
 // The fast epilogue's math on 8-column group j of an accumulator fragment: x[0..1] = act(d * sc + b) of this
 // thread's first row, x[2..3] of its second.  b: the bias of the thread's column pair in group j.
@@ -101,15 +88,12 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&v)[4], int l) {
 
 // Ring producer of the two-warpgroup kernels (k_ffn_tc, k_proj_tc), run by warp 0 between its own MMAs: load every
 // position up to `need` (blocking on its slot: warp 0 reads that position next), then those whose slot is already
-// free.  Position q goes to slot q % stages once position q - stages has been freed (bar_empty, one arrival per
-// warp).  Warp-uniform.
-template <class Load>
-__device__ __forceinline__ void ring_produce(int& q_next, int total, int need, const uint64_t* bar_empty, int stages,
-                                             Load&& load) {
+// free.  Warp-uniform.
+template <int S, class Load>
+__device__ __forceinline__ void ring_produce(int& q_next, int total, int need, const Ring<S>& ring, Load&& load) {
   while (q_next < total) {
-    const uint32_t bar = smem_u32(&bar_empty[q_next % stages]), par = (((uint32_t)(q_next / stages)) & 1u) ^ 1u;
-    if (q_next <= need) mbar_wait(bar, par);
-    else if (!__shfl_sync(0xffffffffu, (int)mbar_test(bar, par), 0)) break;
+    if (q_next <= need) ring.wait_empty(q_next);
+    else if (!__shfl_sync(0xffffffffu, (int)ring.test_empty(q_next), 0)) break;
     load(q_next++);
   }
 }
@@ -231,8 +215,8 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);   // [STAGES] TMA tx
-  uint64_t* bar_empty = bar_full + STAGES;                                              // [STAGES] one arrival per consumer warp
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  const Ring<STAGES> ring{bar_full, bar_full + STAGES};
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
   int tl_n = 0;                                     // debug-timeline event counter of this warp
@@ -246,10 +230,7 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
   };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
-    }
+    ring.init(CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmA1h); tma_prefetch_desc(&tmA1l); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
   }
@@ -268,38 +249,33 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
       int m0, n0;
       decode(j, m0, n0);
       tl_event(p.tl, tl_n, 1, j);                                    // producer: tile j begins
-      for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
-        const int s = kbg % STAGES;
-        mbar_wait(smem_u32(&bar_empty[s]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
-        if (elect_one()) {
-          if (kb == 0 && j + 1 < nlocal) {
-            // the ring is only two or three k-blocks deep: the NEXT tile's activation rows are pulled into L2
-            // one whole tile ahead (weights are L2-resident anyway)
-            int m1, n1;
-            decode(j + 1, m1, n1);
-            if (m1 != m0) {
-              for (int k2 = 0; k2 < p.kblocks; ++k2) {
-                if (k2 < p.kb1) { tma_prefetch_2d(&tmA1h, k2 * BK, m1); tma_prefetch_2d(&tmA1l, k2 * BK, m1); }
-                else { tma_prefetch_2d(&tmA2h, (k2 - p.kb1) * BK, m1); tma_prefetch_2d(&tmA2l, (k2 - p.kb1) * BK, m1); }
-              }
+      auto prefetch = [&](int kb) {
+        if (kb == 0 && j + 1 < nlocal) {
+          // the ring is only two or three k-blocks deep: the NEXT tile's activation rows are pulled into L2
+          // one whole tile ahead (weights are L2-resident anyway)
+          int m1, n1;
+          decode(j + 1, m1, n1);
+          if (m1 != m0) {
+            for (int k2 = 0; k2 < p.kblocks; ++k2) {
+              if (k2 < p.kb1) { tma_prefetch_2d(&tmA1h, k2 * BK, m1); tma_prefetch_2d(&tmA1l, k2 * BK, m1); }
+              else { tma_prefetch_2d(&tmA2h, (k2 - p.kb1) * BK, m1); tma_prefetch_2d(&tmA2l, (k2 - p.kb1) * BK, m1); }
             }
           }
-          const uint32_t full = smem_u32(&bar_full[s]);
-          mbar_expect_tx(full, Cfg::STAGE_BYTES);
-          const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-          const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-          if (kb < p.kb1) {
-            tma_load_2d(sAh, &tmA1h, full, kb * BK, m0);
-            tma_load_2d(sAl, &tmA1l, full, kb * BK, m0);
-          } else {
-            tma_load_2d(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
-            tma_load_2d(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
-          }
-          tma_load_2d(sWh, &tmWh, full, kb * BK, n0);       // rows >= N are zero-filled (and counted)
-          tma_load_2d(sWl, &tmWl, full, kb * BK, n0);
         }
-        __syncwarp();
-      }
+      };
+      ring_feed(ring, kbg, p.kblocks, Cfg::STAGE_BYTES, [&](int kb, int s, uint32_t full) {
+        const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
+        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
+        if (kb < p.kb1) {
+          tma_load_2d(sAh, &tmA1h, full, kb * BK, m0);
+          tma_load_2d(sAl, &tmA1l, full, kb * BK, m0);
+        } else {
+          tma_load_2d(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
+          tma_load_2d(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
+        }
+        tma_load_2d(sWh, &tmWh, full, kb * BK, n0);       // rows >= N are zero-filled (and counted)
+        tma_load_2d(sWl, &tmWl, full, kb * BK, n0);
+      }, prefetch);
     }
     return;
   }
@@ -313,22 +289,10 @@ k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUt
     int m0, n0;
     decode(it, m0, n0);
     tl_event(p.tl, tl_n, 2, it);                                     // MMA: tile `it` begins
-    for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
-      const int s = kbg % STAGES;
-      mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
-      const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128), sAl = sAh + Cfg::A_BYTES;
-      const uint32_t sWh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-      wg_fence();
-      kblock_ss<BN>(d, sAh, sAl, sWh, sWl, kb == 0);
-      wg_commit();
-      if (kb > 0) {                                  // the previous k-block's MMAs have retired: free its stage
-        wg_wait<1>();
-        if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
-      }
-    }
-    wg_wait<0>();
-    acc_fence(d);
-    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+    ring_mma<BN>(d, ring, kbg, p.kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
+      ah = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128); al = ah + Cfg::A_BYTES;
+      wh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES; wl = wh + Cfg::W_BYTES;
+    });
     tl_event(p.tl, tl_n, 4, it);                                     // epilogue: accumulator of tile `it` ready
 
     const int r_lo = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -472,10 +436,9 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint8_t* ring = smem + Cfg::X_BYTES;
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
-  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
-  uint64_t* bar_xfull = bar_empty + STAGES;   // [4] k-block kb of the x tile landed
-  uint64_t* bar_xempty = bar_xfull + 4;       // [4] ... and no longer read (eight arrivals)
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);
+  const Ring<STAGES> wring{bar_full, bar_full + STAGES};                 // the weight ring
+  const Ring<4> xring{bar_full + 2 * STAGES, bar_full + 2 * STAGES + 4};  // slot kb: k-block kb of the x tile
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   int tl_n = 0;
@@ -512,14 +475,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   const int xtotal = nlocal * 4 * XG;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
-    }
-    for (int kb = 0; kb < 4; ++kb) {
-      mbar_init(smem_u32(&bar_xfull[kb]), 1);
-      mbar_init(smem_u32(&bar_xempty[kb]), CONSUMER_WARPS);
-    }
+    wring.init(CONSUMER_WARPS);
+    xring.init(CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmXh); tma_prefetch_desc(&tmXl); tma_prefetch_desc(&tmW1h);
     tma_prefetch_desc(&tmW1l); tma_prefetch_desc(&tmW2h); tma_prefetch_desc(&tmW2l);
@@ -541,7 +498,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
     const Item it = item(j);
     const int r = q - j * per_tile;
     if (elect_one()) {
-      const uint32_t full = smem_u32(&bar_full[q % STAGES]);
+      const uint32_t full = wring.full_bar(q);
       const uint32_t dst = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES);
       mbar_expect_tx(full, Cfg::STAGE_BYTES);
       if (r < PRE) {
@@ -565,7 +522,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
       const int j = v / (4 * XG), kb = v & 3;
       const bool att = p.prefix && (v >> 2) == j * XG;       // the item's first fill with the prefix: att
       const int m0 = item(j).mt * BM;
-      const uint32_t full = smem_u32(&bar_xfull[kb]);
+      const uint32_t full = smem_u32(&xring.full[kb]);
       mbar_expect_tx(full, 2 * BM * 128);
       tma_load_2d(smem_u32(smem + kb * 16384), att ? &tmAh : &tmXh, full, kb * BK, m0);
       tma_load_2d(smem_u32(smem + 65536 + kb * 16384), att ? &tmAl : &tmXl, full, kb * BK, m0);
@@ -593,8 +550,8 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   //     position past the out-projection (it needs them for its own LN1 / F1).
   // Called by warp 0 only, warp-uniformly.
   auto produce = [&](int need, int need_x) {
-    ring_produce(x_next, xtotal, need_x, bar_xempty, 4, load_x);
-    ring_produce(q_next, total, need, bar_empty, STAGES, load_slot);
+    ring_produce(x_next, xtotal, need_x, xring, load_x);
+    ring_produce(q_next, total, need, wring, load_slot);
   };
 
   // ------------------------------------------------------------------ both warpgroups: MMA + epilogue
@@ -606,10 +563,10 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
   float acc1[32];
   uint32_t hh[4][4], hl[4][4];                     // the hidden chunk as A fragments: [16-deep k-step][register]
   int rc = 0;
-  auto slot_full = [&](int r) { mbar_wait(smem_u32(&bar_full[r % STAGES]), ((uint32_t)(r / STAGES)) & 1u); };
-  auto slot_free = [&](int r) { if (lane == 0) mbar_arrive(smem_u32(&bar_empty[r % STAGES])); };
-  auto x_full = [&](int kb, uint32_t par) { mbar_wait(smem_u32(&bar_xfull[kb]), par); };
-  auto x_free = [&](int kb) { if (lane == 0) mbar_arrive(smem_u32(&bar_xempty[kb])); };
+  auto slot_full = [&](int r) { wring.wait_full(r); };
+  auto slot_free = [&](int r) { if (lane == 0) wring.release(r); };
+  auto x_full = [&](int kb, uint32_t par) { mbar_wait(smem_u32(&xring.full[kb]), par); };
+  auto x_free = [&](int kb) { if (lane == 0) mbar_arrive(smem_u32(&xring.empty[kb])); };
   for (int j = 0; j < nlocal; ++j) {
     const Item it = item(j);
     const int m0 = it.mt * BM;
@@ -783,7 +740,7 @@ k_ffn_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUten
           bulk_wait_read<0>();
         }
 #pragma unroll
-        for (int kb = 0; kb < 4; ++kb) mbar_arrive_cnt(smem_u32(&bar_xempty[kb]), 4);
+        for (int kb = 0; kb < 4; ++kb) mbar_arrive_cnt(smem_u32(&xring.empty[kb]), 4);
       }
       __syncwarp();
       tl_event(p.tl, tl_n, 63, j);                                   // the y store has read the tile
@@ -830,10 +787,10 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint8_t* ring = smem + Cfg::A_BYTES;
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);   // [STAGES] ring slot filled (TMA tx)
-  uint64_t* bar_empty = bar_full + STAGES;    // [STAGES] ring slot consumed (one arrival per warp)
-  uint64_t* bar_afull = bar_empty + STAGES;   // [4] k-block k of the A tile landed
-  uint64_t* bar_aempty = bar_afull + 4;       // [4] ... and read by the last chunk of its tile (one arrival per warp)
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(ring + STAGES * Cfg::STAGE_BYTES);
+  const Ring<STAGES> wring{bar_full, bar_full + STAGES};                 // the weight ring
+  // slot k: k-block k of the A tile, freed by the last chunk of its tile
+  const Ring<4> aring{bar_full + 2 * STAGES, bar_full + 2 * STAGES + 4};
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   int tl_n = 0;
@@ -848,14 +805,8 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   auto last_of_tile = [&](int i) { return i == n - 1 || (t0 + i + 1) % NC == 0; };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
-    }
-    for (int k = 0; k < 4; ++k) {
-      mbar_init(smem_u32(&bar_afull[k]), 1);
-      mbar_init(smem_u32(&bar_aempty[k]), CONSUMER_WARPS);
-    }
+    wring.init(CONSUMER_WARPS);
+    aring.init(CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
   }
@@ -873,7 +824,7 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   auto load_w = [&](int q) {
     if (elect_one()) {
       const int c = (t0 + (q >> 2)) % NC, k = q & 3;
-      const uint32_t full = smem_u32(&bar_full[q % STAGES]);
+      const uint32_t full = wring.full_bar(q);
       const uint32_t dst = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES);
       mbar_expect_tx(full, Cfg::STAGE_BYTES);
       tma_load_2d(dst, &tmWh, full, k * BK, c * Cfg::CHUNK);         // rows >= N are zero-filled (and counted)
@@ -884,7 +835,7 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   auto load_a = [&](int a) {
     if (elect_one()) {
       const int j = a >> 2, k = a & 3, m0 = (mt0 + j) * BM;
-      const uint32_t full = smem_u32(&bar_afull[k]);
+      const uint32_t full = smem_u32(&aring.full[k]);
       mbar_expect_tx(full, 2 * BM * 128);
       tma_load_2d(smem_u32(smem + k * 16384), &tmAh, full, k * BK, m0);
       tma_load_2d(smem_u32(smem + 65536 + k * 16384), &tmAl, full, k * BK, m0);
@@ -894,8 +845,8 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
     __syncwarp();
   };
   auto produce = [&](int need_w, int need_a) {     // warp 0 only, warp-uniformly
-    ring_produce(a_next, 4 * ntiles, need_a, bar_aempty, 4, load_a);
-    ring_produce(q_next, 4 * n, need_w, bar_empty, STAGES, load_w);
+    ring_produce(a_next, 4 * ntiles, need_a, aring, load_a);
+    ring_produce(q_next, 4 * n, need_w, wring, load_w);
   };
 
   // ------------------------------------------------------------------ both warpgroups: MMA + epilogue
@@ -905,8 +856,8 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
   float acc0[64], acc1[64];
   auto retire = [&](int q) {                       // this warp's MMAs of W position q have retired
     if (lane == 0) {
-      mbar_arrive(smem_u32(&bar_empty[q % STAGES]));
-      if (last_of_tile(q >> 2)) mbar_arrive(smem_u32(&bar_aempty[q & 3]));
+      wring.release(q);
+      if (last_of_tile(q >> 2)) mbar_arrive(smem_u32(&aring.empty[q & 3]));
     }
   };
   // The fast epilogue's math, then a quad transpose per four 8-column groups, so that each lane stores one group
@@ -951,10 +902,10 @@ k_proj_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUte
       const int q = 4 * i + k;
       if (warp == 0) produce(q, fresh ? 4 * j + k : -1);
       if (fresh) {
-        mbar_wait(smem_u32(&bar_afull[k]), (uint32_t)j & 1u);
+        mbar_wait(aring.full_bar(k), aring.phase(4 * j));     // position 4 j + k
         if (k == 0) tl_event(p.tl, tl_n, 51, j);                    // A k-block 0 of tile j landed
       }
-      mbar_wait(smem_u32(&bar_full[q % STAGES]), ((uint32_t)(q / STAGES)) & 1u);
+      wring.wait_full(q);
       const uint32_t w = smem_u32(ring + (q % STAGES) * Cfg::STAGE_BYTES), a = sA + k * 16384;
       wg_fence();
       kblock_ss<128>(cur, a, a + 65536, w, w + Cfg::STAGE_BYTES / 2, k == 0);
@@ -1150,8 +1101,6 @@ int tc_set_ffn_fused(TcCtx* c, int on) {
   c->ffn_fused = on;
   return old;
 }
-// both planes 16-byte aligned (TMA base addresses)
-static bool planes_aligned16(const ActBuf& b) { return ((uintptr_t)b.hi & 15) == 0 && ((uintptr_t)b.lo() & 15) == 0; }
 
 bool tc_ffn_supported(const TcCtx* c, const GemmArgs& g1, const GemmArgs& g2, const LnArgs& l2) {
   if (!c || !c->ffn_fused) return false;

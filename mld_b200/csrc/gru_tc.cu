@@ -17,8 +17,8 @@
 // thread holds columns 8 j + cp, 8 j + cp + 1 of every group j, so the r, z and n pre-activations of its units land
 // in its own registers and the epilogue needs no shuffle or shared memory.
 //
-// CTA = three warpgroups as in k_gemm_tc (gemm_tc.cu): warp 0 streams the A (state) and W_hh k-blocks through a
-// ring of 128B-swizzled stages with TMA, warpgroups 1 and 2 each own 64 rows of the 128-row tile.  Grid =
+// CTA = three warpgroups as in k_gemm_tc (DESIGN §2, the ring protocol): warp 0 streams the A (state) and W_hh
+// k-blocks through a ring of 128B-swizzled stages with TMA, warpgroups 1 and 2 each own 64 rows of the 128-row tile.  Grid =
 // (H / 32 unit tiles, row tiles, 2 directions); no CTA waits on another, steps are ordered by the stream.
 #include <algorithm>
 
@@ -30,11 +30,7 @@ using namespace tc;
 
 constexpr int BM = 128, BK = 64, BN = 96, UNITS = 32;        // a tile: 128 rows x 32 hidden units (96 gate columns)
 constexpr int NUM_THREADS = 384, CONSUMER_WARPS = 8;
-constexpr int A_BYTES = BM * BK * 2, W_BYTES = BN * BK * 2;  // one plane: 16 KB / 12 KB
-constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;       // 56 KB
-constexpr int STAGES = 4;
-constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
-static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+using Cfg = StageLayout<BN, 4>;                              // 56 KB stages (tc_common.cuh)
 
 // accurate expf / tanhf (not the fast intrinsics): the recurrence compounds their error over up to 49 steps
 __device__ __forceinline__ float gru_cell(float gr, float gz, float gn, float hr, float hz, float hn, float h) {
@@ -77,17 +73,14 @@ k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ 
               const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const GruStepArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* bar_empty = bar_full + STAGES;
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  const Ring<Cfg::STAGES> ring{bar_full, bar_full + Cfg::STAGES};
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int nt = (int)blockIdx.x, m0 = (int)blockIdx.y * BM, dir = (int)blockIdx.z;
   const int kblocks = a.H / BK;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
-    }
+    ring.init(CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
   }
@@ -99,14 +92,14 @@ k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ 
     reg_dec<40>();
     if (warp != 0) return;
     const int arow = dir * a.rows_pad + m0, wrow = dir * 3 * a.H + nt * BN;
+    // the ring position is the k-block: ring_feed's separate counter would change the generated code
     for (int kb = 0; kb < kblocks; ++kb) {
-      const int s = kb % STAGES;
-      mbar_wait(smem_u32(&bar_empty[s]), (((uint32_t)(kb / STAGES)) & 1u) ^ 1u);
+      ring.wait_empty(kb);
       if (elect_one()) {
-        const uint32_t full = smem_u32(&bar_full[s]);
-        mbar_expect_tx(full, STAGE_BYTES);
-        const uint32_t sAh = smem_u32(smem + s * STAGE_BYTES), sAl = sAh + A_BYTES;
-        const uint32_t sWh = sAl + A_BYTES, sWl = sWh + W_BYTES;
+        const uint32_t full = ring.full_bar(kb);
+        mbar_expect_tx(full, Cfg::STAGE_BYTES);
+        const uint32_t sAh = smem_u32(smem + (kb % Cfg::STAGES) * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
+        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
         tma_load_2d(sAh, &tmAh, full, kb * BK, arow);
         tma_load_2d(sAl, &tmAl, full, kb * BK, arow);
         tma_load_2d(sWh, &tmWh, full, kb * BK, wrow);
@@ -120,21 +113,12 @@ k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ 
   const int cw = (warp >> 2) - 1;
   const int cp = 2 * (lane & 3);
   float d[BN / 2];
-  for (int kb = 0; kb < kblocks; ++kb) {
-    const int s = kb % STAGES;
-    mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kb / STAGES)) & 1u);
-    const uint32_t base = smem_u32(smem + s * STAGE_BYTES);
-    wg_fence();
-    kblock_ss<BN>(d, base + cw * (64 * 128), base + A_BYTES + cw * (64 * 128), base + 2 * A_BYTES,
-                  base + 2 * A_BYTES + W_BYTES, kb == 0);
-    wg_commit();
-    if (kb > 0) {
-      wg_wait<1>();
-      if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kb - 1) % STAGES]));
-    }
-  }
-  wg_wait<0>();
-  acc_fence(d);
+  int q = 0;                   // one tile per CTA: the ring starts at position 0 and is not reused
+  ring_mma<BN, false>(d, ring, q, kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
+    const uint32_t base = smem_u32(smem + s * Cfg::STAGE_BYTES);
+    ah = base + cw * (64 * 128); al = base + Cfg::A_BYTES + cw * (64 * 128);
+    wh = base + 2 * Cfg::A_BYTES; wl = base + 2 * Cfg::A_BYTES + Cfg::W_BYTES;
+  });
 
   // gate epilogue.  Every load of a row (state, gi, biases) is issued before any store, so the loads of the 8
   // (unit, row) pairs overlap instead of each waiting behind the previous pair's stores.
@@ -391,7 +375,7 @@ __global__ void k_im2col_k4s2(ActBuf X, const float* __restrict__ src, int64_t l
 }  // namespace
 
 bool gru_tc_init() {
-  return smem_opt_in(k_gru_step_tc, SMEM_BYTES, "k_gru_step_tc") &&
+  return smem_opt_in(k_gru_step_tc, Cfg::SMEM_BYTES, "k_gru_step_tc") &&
          smem_opt_in(k_gru_seq_tc<64>, seq_smem_bytes(64), "k_gru_seq_tc<64>") &&
          smem_opt_in(k_gru_seq_tc<128>, seq_smem_bytes(128), "k_gru_seq_tc<128>");
 }
@@ -404,7 +388,7 @@ bool gru_step_tc(const GruStepArgs& a, cudaStream_t st) {
                   make_map(&mWh, a.w_hh, 6 * a.H, a.H, BN) && make_map(&mWl, a.w_hh + a.w_plane_stride, 6 * a.H, a.H, BN);
   if (!ok) return false;
   const dim3 grid((unsigned)(a.H / UNITS), (unsigned)((a.rows + BM - 1) / BM), 2);
-  launch_pdl(k_gru_step_tc, grid, dim3(NUM_THREADS), SMEM_BYTES, st, mAh, mAl, mWh, mWl, a);
+  launch_pdl(k_gru_step_tc, grid, dim3(NUM_THREADS), Cfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, a);
   return true;
 }
 

@@ -182,8 +182,9 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
   float* sO = reinterpret_cast<float*>(smem + OFF_O);
   float* sLw = reinterpret_cast<float*>(smem + OFF_LW);
   uint64_t* bar_a = reinterpret_cast<uint64_t*>(smem + OFF_BAR);
-  uint64_t* bar_full = bar_a + 1;
-  uint64_t* bar_empty = bar_full + STAGES;
+  // the W stream.  Its loops stay written out: through ring_feed / ring_mma nvcc folds the stage addresses
+  // differently and the kernel's code changes
+  const Ring<STAGES> ring{bar_a + 1, bar_a + 1 + STAGES};
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int nsplit = (p.vtiles + p.vtiles_per_cta - 1) / p.vtiles_per_cta;
@@ -193,10 +194,7 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
 
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(bar_a), 1);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 4);
-    }
+    ring.init(4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -217,9 +215,9 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
     for (int nt = n0; nt < n1; ++nt)
       for (int kb = 0; kb < KB; ++kb, ++kbg) {
         const int s = kbg % STAGES;
-        mbar_wait(smem_u32(&bar_empty[s]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
+        ring.wait_empty(kbg);
         if (elect_one()) {
-          const uint32_t full = smem_u32(&bar_full[s]);
+          const uint32_t full = ring.full_bar(kbg);
           const uint32_t sw = smem_u32(smem + OFF_W + s * W_STAGE);
           mbar_expect_tx(full, W_STAGE);
           tma_load_2d(sw, &tmWh, full, kb * BK, nt * BN);
@@ -248,19 +246,19 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
   for (int nt = n0; nt < n1; ++nt) {
     for (int kb = 0; kb < KB; ++kb, ++kbg) {
       const int s = kbg % STAGES;
-      mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
+      ring.wait_full(kbg);
       const uint32_t sAh = smem_u32(smem + kb * 2 * A_PLANE), sWh = smem_u32(smem + OFF_W + s * W_STAGE);
       wg_fence();
       kblock_ss<BN>(d, sAh, sAh + A_PLANE, sWh, sWh + W_PLANE, kb == 0);
       wg_commit();
       if (kb > 0) {                                   // the previous k-block's MMAs have retired: free its stage
         wg_wait<1>();
-        if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+        if (lane == 0) ring.release(kbg - 1);
       }
     }
     wg_wait<0>();
     acc_fence(d);
-    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+    if (lane == 0) ring.release(kbg - 1);
 
     for (int i = tid; i < kJ * VT; i += 128) sLw[i] = __ldg(p.lbsw + (int64_t)nt * kJ * VT + i);
     named_bar_sync(1, 128);                           // sLw and sX ready; the previous tile's staging is stored

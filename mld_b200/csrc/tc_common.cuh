@@ -334,6 +334,85 @@ __device__ __forceinline__ void kblock_ss(float (&d)[N / 2], uint32_t sAh, uint3
   }
 }
 
+// ---------------------------------------------------------------------------------- TMA rings
+// A ring of S shared-memory slots that TMA fills and MMA warps drain.  Ring position q (a running count of the
+// loads that went through the ring) lives in slot q % S, in phase (q / S) & 1 of that slot's two barriers: full[s]
+// (one arrival, the producer's expect_tx, plus the TMA bytes) and empty[s] (one arrival per consumer warp once
+// its MMAs on the slot have retired).  The producer of position q waits for empty's previous phase, so its first S
+// waits return at once on fresh barriers.  init runs on one thread, before fence.mbarrier_init.
+template <int S>
+struct Ring {
+  uint64_t* full;
+  uint64_t* empty;
+  __device__ __forceinline__ void init(uint32_t consumers) const {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(smem_u32(&full[s]), 1);
+      mbar_init(smem_u32(&empty[s]), consumers);
+    }
+  }
+  __device__ __forceinline__ static uint32_t phase(int q) { return ((uint32_t)(q / S)) & 1u; }
+  __device__ __forceinline__ uint32_t full_bar(int q) const { return smem_u32(&full[q % S]); }
+  __device__ __forceinline__ void wait_full(int q) const { mbar_wait(full_bar(q), phase(q)); }
+  __device__ __forceinline__ void wait_empty(int q) const { mbar_wait(smem_u32(&empty[q % S]), phase(q) ^ 1u); }
+  __device__ __forceinline__ bool test_empty(int q) const { return mbar_test(smem_u32(&empty[q % S]), phase(q) ^ 1u); }
+  __device__ __forceinline__ void release(int q) const { mbar_arrive(smem_u32(&empty[q % S])); }
+};
+
+// The producer warp's loop over n k-blocks, from ring position q on (q is advanced past them).  The whole warp
+// walks it (uniform control flow); one elected lane calls before(kb) (k_gemm_tc's L2 prefetch), arms full with
+// `bytes` and issues load(kb, slot, full).
+struct NoOp { __device__ __forceinline__ void operator()(int) const {} };
+template <int S, class Load, class Before = NoOp>
+__device__ __forceinline__ void ring_feed(const Ring<S>& ring, int& q, int n, uint32_t bytes, Load&& load,
+                                          Before&& before = {}) {
+  for (int kb = 0; kb < n; ++kb, ++q) {
+    ring.wait_empty(q);
+    if (elect_one()) {
+      before(kb);
+      const uint32_t full = ring.full_bar(q);
+      mbar_expect_tx(full, bytes);
+      load(kb, q % S, full);
+    }
+    __syncwarp();
+  }
+}
+
+// A consumer warpgroup's loop over n k-blocks from ring position q on (q is advanced past them): d = the sum of
+// kblock_ss<BN> over them, with stage(kb, slot, ah, al, wh, wl) giving the operand addresses.  Each position is
+// released (lane 0 of every warp) once the next one's MMAs are issued and its own have retired, the last one after
+// the drain - unless RELEASE_LAST is false: a CTA that loads nothing more leaves it.
+template <int BN, bool RELEASE_LAST = true, int S, class Stage>
+__device__ __forceinline__ void ring_mma(float (&d)[BN / 2], const Ring<S>& ring, int& q, int n, int lane, Stage&& stage) {
+  for (int kb = 0; kb < n; ++kb, ++q) {
+    ring.wait_full(q);
+    uint32_t ah, al, wh, wl;
+    stage(kb, q % S, ah, al, wh, wl);
+    wg_fence();
+    kblock_ss<BN>(d, ah, al, wh, wl, kb == 0);
+    wg_commit();
+    if (kb > 0) {
+      wg_wait<1>();
+      if (lane == 0) ring.release(q - 1);
+    }
+  }
+  wg_wait<0>();
+  acc_fence(d);
+  if (RELEASE_LAST && lane == 0) ring.release(q - 1);
+}
+
+// One ring stage of a 128 x BN split16 tile: [A hi | A lo | W hi | W lo], each plane a 64-deep k-block (one 128B
+// swizzle row per tile row), A 128 rows and W BN rows; two consumer warpgroups take 64 A rows each.  STAGES stages
+// followed by the ring's barriers, plus the alignment slack of smem_pad1024.
+template <int BN, int STAGES_>
+struct StageLayout {
+  static constexpr int STAGES = STAGES_;
+  static constexpr int A_BYTES = 128 * 64 * 2;        // one plane of the A tile (16 KB)
+  static constexpr int W_BYTES = BN * 64 * 2;         // one plane of the W tile
+  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
+  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+};
+
 // sum over the 4 lanes of a quad (the lanes that hold one accumulator row)
 __device__ __forceinline__ float quad_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 1);
@@ -347,6 +426,13 @@ __device__ __forceinline__ void split2(float x0, float x1, uint32_t& hi, uint32_
   const __half2 l2 = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
   hi = *reinterpret_cast<const uint32_t*>(&h2);
   lo = *reinterpret_cast<const uint32_t*>(&l2);
+}
+// split2 into element pair o of two fp16 planes (o even)
+__device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, float x0, float x1) {
+  uint32_t h, l;
+  split2(x0, x1, h, l);
+  *reinterpret_cast<uint32_t*>(hi + o) = h;
+  *reinterpret_cast<uint32_t*>(lo + o) = l;
 }
 
 // Debug timeline (mldb_debug_timeline): when `tl` is non-null, lane 0 of the calling warp of CTA 0 stores
@@ -364,6 +450,9 @@ __device__ __forceinline__ void tl_event(long long* tl, int& n, int tag, int aux
 long long* mldb_timeline_buffer();   // debug.cu: the device buffer while a timeline is being recorded, else nullptr
 
 // ---------------------------------------------------------------------------------- host: tensor maps
+// both planes of a split16 buffer 16-byte aligned (TMA base addresses, 16-byte accesses)
+inline bool planes_aligned16(const ActBuf& b) { return ((uintptr_t)b.hi & 15) == 0 && ((uintptr_t)b.lo() & 15) == 0; }
+
 typedef CUresult (*PFN_tmapEncodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                         const cuuint64_t*, const cuuint32_t*, const cuuint32_t*,
                                         CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,

@@ -4,8 +4,8 @@
 //   D[128 x C] = sum over k-blocks (tap, c0) of  X_tap[128 x 64] . W[:, tap C + c0 ..]^T       (split16, kblock_ss)
 //
 // The activations are split16 rows (n * T + t) * 24 + v, i.e. planes of shape [nseq][T][24][C].  A tile is 8 joints
-// x 16 output frames of one sequence (128 rows, 64 per consumer warpgroup), so k_gemm_tc's two-consumer layout and
-// register budget carry over unchanged.  Its A operand for tap `tap` is one TMA box of a 4-D tensor map over those
+// x 16 output frames of one sequence (128 rows, 64 per consumer warpgroup), so k_gemm_tc's two-consumer layout, its
+// ring (DESIGN §2, the ring protocol) and its register budget carry over unchanged.  Its A operand for tap `tap` is one TMA box of a 4-D tensor map over those
 // planes: channels c0 .. c0 + 63, joints 8 vt .. 8 vt + 7, frames s t0 + tap - 4 + s i (i < 16), sequence n.  The
 // box is one sequence deep, so no tile reads another sequence's frames, and the frames outside [0, T) are TMA's
 // out-of-bounds zero fill: the convolution's padding.  Stride 2 is the frame dimension's traversal stride in the map
@@ -28,15 +28,9 @@ constexpr int CONSUMER_WARPS = 8;
 constexpr int JOINTS = 24, TILE_V = 8, TILE_T = 16;  // a tile: 8 joints x 16 output frames
 constexpr int TAPS = 9, PAD = 4;
 
+// [A hi | A lo | W hi | W lo] stages (tc_common.cuh): k_gemm_tc's depth at BN = 256 and 128, four at 64
 template <int BN>
-struct TconvCfg {
-  static constexpr int A_BYTES = BM * BK * 2;          // one plane of the A tile (16 KB)
-  static constexpr int W_BYTES = BN * BK * 2;          // one plane of the W tile
-  static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
-  static constexpr int STAGES = BN == 256 ? 2 : (BN == 128 ? 3 : 4);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;   // + barriers + alignment slack
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
-};
+using TconvCfg = StageLayout<BN, BN == 256 ? 2 : (BN == 128 ? 3 : 4)>;
 
 struct TconvParams {
   int nseq, T_out, t_blocks;
@@ -49,13 +43,6 @@ struct TconvParams {
   float* out_f32;
 };
 
-__device__ __forceinline__ void store_split2(__half* hi, __half* lo, int64_t o, float x0, float x1) {
-  uint32_t h, l;
-  split2(x0, x1, h, l);
-  *reinterpret_cast<uint32_t*>(hi + o) = h;
-  *reinterpret_cast<uint32_t*>(lo + o) = l;
-}
-
 // Persistent: CTA c walks tiles c, c + #CTAs, ...; tile -> (sequence, 16-frame block, 8-joint group), the joint group
 // fastest so that the three tiles reading the same frames run side by side.
 template <int BN>
@@ -67,8 +54,8 @@ k_tconv_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUt
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);   // [STAGES] TMA tx
-  uint64_t* bar_empty = bar_full + STAGES;                                              // [STAGES] one arrival per consumer warp
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  const Ring<STAGES> ring{bar_full, bar_full + STAGES};
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   const int ntiles = p.nseq * p.t_blocks * 3;
@@ -82,10 +69,7 @@ k_tconv_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUt
   };
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), CONSUMER_WARPS);
-    }
+    ring.init(CONSUMER_WARPS);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmXh); tma_prefetch_desc(&tmXl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
   }
@@ -102,28 +86,21 @@ k_tconv_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUt
       int n, t0, vt;
       decode(j, n, t0, vt);
       const int f0 = p.stride * t0;                  // input frame of the tile's first output frame at tap 4
-      for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
-        const int s = kbg % STAGES;
-        mbar_wait(smem_u32(&bar_empty[s]), (((uint32_t)(kbg / STAGES)) & 1u) ^ 1u);
-        if (elect_one()) {
-          const uint32_t full = smem_u32(&bar_full[s]);
-          mbar_expect_tx(full, Cfg::STAGE_BYTES);
-          const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-          const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-          if (kb < p.ktap) {
-            const int tap = kb / p.kc, c0 = (kb - tap * p.kc) * BK;
-            tma_load_4d(sAh, &tmXh, full, c0, vt * TILE_V, f0 + tap - PAD, n);
-            tma_load_4d(sAl, &tmXl, full, c0, vt * TILE_V, f0 + tap - PAD, n);
-          } else {
-            const int c0 = (kb - p.ktap) * BK;
-            tma_load_4d(sAh, &tmRh, full, c0, vt * TILE_V, f0, n);
-            tma_load_4d(sAl, &tmRl, full, c0, vt * TILE_V, f0, n);
-          }
-          tma_load_2d(sWh, &tmWh, full, kb * BK, 0);
-          tma_load_2d(sWl, &tmWl, full, kb * BK, 0);
+      ring_feed(ring, kbg, p.kblocks, Cfg::STAGE_BYTES, [&](int kb, int s, uint32_t full) {
+        const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
+        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
+        if (kb < p.ktap) {
+          const int tap = kb / p.kc, c0 = (kb - tap * p.kc) * BK;
+          tma_load_4d(sAh, &tmXh, full, c0, vt * TILE_V, f0 + tap - PAD, n);
+          tma_load_4d(sAl, &tmXl, full, c0, vt * TILE_V, f0 + tap - PAD, n);
+        } else {
+          const int c0 = (kb - p.ktap) * BK;
+          tma_load_4d(sAh, &tmRh, full, c0, vt * TILE_V, f0, n);
+          tma_load_4d(sAl, &tmRl, full, c0, vt * TILE_V, f0, n);
         }
-        __syncwarp();
-      }
+        tma_load_2d(sWh, &tmWh, full, kb * BK, 0);
+        tma_load_2d(sWl, &tmWl, full, kb * BK, 0);
+      });
     }
     return;
   }
@@ -136,22 +113,10 @@ k_tconv_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUt
   for (int it = 0; it < nlocal; ++it) {
     int n, t0, vt;
     decode(it, n, t0, vt);
-    for (int kb = 0; kb < p.kblocks; ++kb, ++kbg) {
-      const int s = kbg % STAGES;
-      mbar_wait(smem_u32(&bar_full[s]), ((uint32_t)(kbg / STAGES)) & 1u);
-      const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128), sAl = sAh + Cfg::A_BYTES;
-      const uint32_t sWh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-      wg_fence();
-      kblock_ss<BN>(d, sAh, sAl, sWh, sWl, kb == 0);
-      wg_commit();
-      if (kb > 0) {                                  // the previous k-block's MMAs have retired: free its stage
-        wg_wait<1>();
-        if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
-      }
-    }
-    wg_wait<0>();
-    acc_fence(d);
-    if (lane == 0) mbar_arrive(smem_u32(&bar_empty[(kbg - 1) % STAGES]));
+    ring_mma<BN>(d, ring, kbg, p.kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
+      ah = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128); al = ah + Cfg::A_BYTES;
+      wh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES; wl = wh + Cfg::W_BYTES;
+    });
 
     // this thread's rows: tile rows r and r + 8 = frames t and t + 1 of joint v
     const int t = t0 + cw * 8 + (warp & 3) * 2, v = vt * TILE_V + (lane >> 2);
@@ -188,8 +153,6 @@ bool frames_map(CUtensorMap* m, const __half* base, int nseq, int T, int C, int 
   return encode_plane_map(m, base, 4, dims, strides, box, estr);
 }
 
-bool aligned16(const void* p) { return ((uintptr_t)p & 15) == 0; }
-
 }  // namespace
 
 bool tconv_tc_init() {
@@ -201,10 +164,10 @@ bool tconv_tc_init() {
 bool tconv_tc_supported(const TconvArgs& a) {
   if (a.C != 64 && a.C != 128 && a.C != 256) return false;
   if ((a.stride != 1 && a.stride != 2) || a.nseq < 1 || a.T_in < 1 || a.T_out != (a.T_in - 1) / a.stride + 1) return false;
-  if (a.x.cols != a.C || !aligned16(a.x.hi) || !aligned16(a.x.lo())) return false;
+  if (a.x.cols != a.C || !planes_aligned16(a.x)) return false;
   int kres = 0;
   if (a.res.hi) {
-    if (a.res.cols != a.C_res || !aligned16(a.res.hi) || !aligned16(a.res.lo())) return false;
+    if (a.res.cols != a.C_res || !planes_aligned16(a.res)) return false;
     if (a.res_conv) {
       if (a.C_res < 64 || a.C_res % 64) return false;
       kres = a.C_res;
@@ -212,7 +175,7 @@ bool tconv_tc_supported(const TconvArgs& a) {
       return false;
     }
   }
-  if (a.w.N != a.C || a.w.K != TAPS * a.C + kres || !aligned16(a.w.w) || !a.w.bias) return false;
+  if (a.w.N != a.C || a.w.K != TAPS * a.C + kres || ((uintptr_t)a.w.w & 15) || !a.w.bias) return false;
   if (a.out.hi ? a.out.cols != a.C : !a.out_f32) return false;
   return true;
 }
