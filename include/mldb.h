@@ -260,6 +260,72 @@ int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float*
                     const float* beta, const float* R, int32_t M, int32_t N, int32_t K, int32_t K1,
                     int32_t act, int32_t use_tc, int32_t split_out, float* out, void* stream);
 
+/* Debug aid: mldb_debug_gemm with the GEMM's whole output placement (mldb_debug_gemm is this with the identity map
+ * and a dense [M, N] output).  Row r of the product goes to output row
+ *   (r / in_group) * out_group + out_off + r % in_group
+ * (in_group = 1 << 30, out_group = out_off = 0: the identity), and columns [out_col0, out_col0 + N) of it:
+ *   y[r] = act(A[r] W^T + b + addtab[out_off + r % in_group]);  y[r] = 0 when r % in_group >= zero_lengths[r / in_group]
+ * out is a caller-filled fp32 DEVICE [out_rows, out_cols] buffer.  split_out != 0: its cells go into split16 planes
+ * before the op, the op writes the planes, and the planes are widened back into out after it, so the cells the op
+ * does not address come back as they were whenever they survive the split16 round trip (11 significant bits).
+ * split_out == 0: the op writes fp32 at out + out_col0 with leading dimension out_cols.  R (DEVICE, nullable) without
+ * gamma: the residual-add epilogue, R laid out like the fp32 output; with gamma: LayerNorm(A W^T + b + R), identity map
+ * and out [M, N] only.  a_kind: 0 split16 A, 1 fp32 A, 2 fp32 A through ReLU (1 and 2 run on the CUDA cores only:
+ * use_tc must be 0).  vec_f32: the fp32 output may take the wgmma kernel's vectorised epilogue (identity map).
+ * Every row and column the map addresses is checked against the buffers.  Synchronous on `stream`. */
+typedef struct mldb_gemm_rows_args {
+  const float* A;                  /* [M, K] fp32 DEVICE */
+  const float* W;                  /* [N, K] fp32 HOST */
+  const float* bias;               /* [N] HOST, nullable */
+  const float* gamma;              /* [N] HOST, nullable: LayerNorm epilogue */
+  const float* beta;               /* [N] HOST */
+  const float* R;                  /* DEVICE, nullable */
+  int32_t M, N, K, K1;             /* 0 < K1 < K: A as two concatenated sources */
+  int32_t act, use_tc, a_kind;
+  int32_t in_group, out_group, out_off;
+  const float* addtab;             /* [tab_rows, N] HOST, nullable */
+  int32_t tab_rows;
+  const int32_t* zero_lengths;     /* [ceil(M / in_group)] HOST, nullable */
+  int32_t vec_f32, split_out;
+  float* out;                      /* [out_rows, out_cols] fp32 DEVICE */
+  int32_t out_rows, out_cols, out_col0;
+} mldb_gemm_rows_args;
+int mldb_debug_gemm_rows(mldb_handle* h, const mldb_gemm_rows_args* a, void* stream);
+
+/* Debug aid: the CUDA-core LayerNorm of every unfused norm,
+ *   out[r] = act(LayerNorm(c[i] + res[i] + rowvec[i / rv_group]) * gamma + beta),  i = input row of r:
+ *   i = r (in_group == 0) or (r / sel_group) * in_group + r % sel_group (the kept tokens of each sequence).
+ * c: fp32 DEVICE [M_in, ldc] (nullable); res: fp32 DEVICE [M_in, d], fed as split16 (nullable); rowvec: fp32 HOST
+ * [ceil(M_in / rv_group), d] (nullable); gamma, beta: fp32 HOST [d].  out: caller-filled fp32 DEVICE [M, ld_out];
+ * split_out != 0: through split16 planes [M, ld_out] filled from out and widened back, as in mldb_debug_gemm_rows.
+ * act: 0 none or 5 LeakyReLU(0.2).  d > 1024 is refused (MLDB_ERR_UNSUPPORTED).  Synchronous on `stream`. */
+typedef struct mldb_ln_args {
+  const float* c;
+  int32_t ldc;
+  const float* res;
+  const float* rowvec;
+  int32_t rv_group;
+  const float* gamma;
+  const float* beta;
+  int32_t M_in, M, d;
+  int32_t sel_group, in_group;
+  int32_t act, split_out;
+  float* out;
+  int32_t ld_out;
+} mldb_ln_args;
+int mldb_debug_ln(mldb_handle* h, const mldb_ln_args* a, void* stream);
+
+/* Debug aid: fp32 rows into a split16 buffer with the GEMM's row map (the condition tokens and the VAE decoder's
+ * queries):  X[(r / in_group) * out_group + out_off + r % in_group, n] =
+ *   relu?(src[src_bcast ? r % in_group : r, n]) + tab[out_off + r % in_group, n]        for n < d
+ * src: fp32 DEVICE [*, ld_src] (nullable: zeros); tab: fp32 HOST [tab_rows, d] (nullable).  out: caller-filled fp32
+ * DEVICE [out_rows, out_cols] (d <= out_cols) that goes into the split16 X before the op and is widened back after it.
+ * scalar != 0: the one-column-per-thread kernel even where the 128-bit one applies.  Synchronous on `stream`. */
+int mldb_debug_rows_to_split(mldb_handle* h, const float* src, int32_t ld_src, int32_t M, int32_t d, int32_t in_group,
+                             int32_t out_group, int32_t out_off, int32_t src_bcast, const float* tab, int32_t tab_rows,
+                             int32_t relu, int32_t scalar, float* out, int32_t out_rows, int32_t out_cols,
+                             void* stream);
+
 /* Debug aid: one post-norm FFN block y = LayerNorm(x + W2 gelu(W1 x + b1) + b2) through the engine's
  * operators (cross_attention.py:266-271).  mode 0 = CUDA-core kernels, 1 = wgmma GEMMs as two
  * launches, 2 = the fused wgmma FFN kernel.  X, out [M,d]: fp32 DEVICE; W1 [ff,d], W2 [d,ff],

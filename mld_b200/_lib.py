@@ -108,6 +108,29 @@ class MldbSmplConfig(C.Structure):
     _fields_ = [("abi_version", C.c_int32), ("num_vertices", C.c_int32)]
 
 
+class MldbGemmRowsArgs(C.Structure):
+    """``mldb_gemm_rows_args`` (include/mldb.h)."""
+    _fields_ = [
+        ("A", C.c_void_p), ("W", C.c_void_p), ("bias", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("R", C.c_void_p), ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("K1", C.c_int32),
+        ("act", C.c_int32), ("use_tc", C.c_int32), ("a_kind", C.c_int32),
+        ("in_group", C.c_int32), ("out_group", C.c_int32), ("out_off", C.c_int32),
+        ("addtab", C.c_void_p), ("tab_rows", C.c_int32), ("zero_lengths", C.c_void_p),
+        ("vec_f32", C.c_int32), ("split_out", C.c_int32),
+        ("out", C.c_void_p), ("out_rows", C.c_int32), ("out_cols", C.c_int32), ("out_col0", C.c_int32),
+    ]
+
+
+class MldbLnArgs(C.Structure):
+    """``mldb_ln_args`` (include/mldb.h)."""
+    _fields_ = [
+        ("c", C.c_void_p), ("ldc", C.c_int32), ("res", C.c_void_p), ("rowvec", C.c_void_p), ("rv_group", C.c_int32),
+        ("gamma", C.c_void_p), ("beta", C.c_void_p), ("M_in", C.c_int32), ("M", C.c_int32), ("d", C.c_int32),
+        ("sel_group", C.c_int32), ("in_group", C.c_int32), ("act", C.c_int32), ("split_out", C.c_int32),
+        ("out", C.c_void_p), ("ld_out", C.c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/mldb.h declares
 _P = C.c_void_p
 _SIGNATURES = {
@@ -133,6 +156,11 @@ _SIGNATURES = {
     "mldb_debug_timeline": (C.c_int, [C.c_int32, _P, C.c_int32, C.POINTER(C.c_int32)]),
     "mldb_debug_gemm": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                   C.c_int32, C.c_int32, C.c_int32, _P, _P]),
+    "mldb_debug_gemm_rows": (C.c_int, [_P, C.POINTER(MldbGemmRowsArgs), _P]),
+    "mldb_debug_ln": (C.c_int, [_P, C.POINTER(MldbLnArgs), _P]),
+    "mldb_debug_rows_to_split": (C.c_int, [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                           C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P, C.c_int32, C.c_int32,
+                                           _P]),
     "mldb_debug_ffn": (C.c_int, [_P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, _P]),
     "mldb_debug_tail": (C.c_int, [_P] * 13 + [C.c_int32] * 5 + [_P, _P]),
     "mldb_debug_attention": (C.c_int, [_P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -4,6 +4,8 @@
 
 #include <string.h>
 
+#include <algorithm>
+
 #include "gemm_tc.h"
 #include "misc_kernels.cuh"
 
@@ -116,59 +118,172 @@ static int debug_exit(mldb_handle* h, size_t n_alloc0, cudaStream_t st, const ch
   return check_ops(h);
 }
 
-// y = act(A W^T + b) or LayerNorm(A W^T + b + R) through the engine's GEMM operators, so tests can
-// compare the wgmma kernels with the CUDA-core kernels (and with torch) shape by shape.
-//   A [M,K] fp32 device; W [N,K], bias [N], gamma/beta [N] fp32 HOST (gamma == NULL: no LN);
-//   R [M,N] fp32 device or NULL; K1 < K splits A into two concatenated sources (skip connection);
-//   out [M,N] fp32 device.  use_tc: 1 tensor-core path, 0 CUDA-core path.  Synchronous.
-extern "C" int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float* bias,
-                               const float* gamma, const float* beta, const float* R, int32_t M, int32_t N,
-                               int32_t K, int32_t K1, int32_t act, int32_t use_tc, int32_t split_out, float* out,
-                               void* stream) {
-  if (!h || !A || !W || !out || M <= 0 || N <= 0 || K <= 0) FAIL(MLDB_ERR_INVALID, "bad argument");
+// fp32 [rows, cols] (device) -> freshly allocated split16 planes, and back: the debug hooks' split16 outputs start
+// from the caller's buffer, so the cells an op must not write can be checked after it
+static int debug_to_split(mldb_handle* h, const float* src, int rows, int cols, ActBuf* out, cudaStream_t st) {
+  TRY(alloc_act(h, rows, cols, out));
+  k_rows_to_split<<<nblk((int64_t)rows * cols), 256, 0, st>>>(*out, src, cols, rows, cols, 1 << 30, 0, 0, 0, nullptr);
+  return MLDB_OK;
+}
+static void debug_from_split(ActBuf x, float* out, cudaStream_t st) {
+  k_split_to_f32<<<nblk((int64_t)x.rows * x.cols), 256, 0, st>>>(x, out, (int64_t)x.rows * x.cols);
+}
+
+// The largest output row the (in_group, out_group, out_off) map of rows [0, M) addresses, or -1 for a bad map.
+static int64_t map_max_row(int M, int in_group, int out_group, int out_off) {
+  if (M <= 0 || in_group <= 0 || out_group < 0 || out_off < 0) return -1;
+  const int64_t last_seq = (M - 1) / in_group;
+  // the last sequence ends at row M - 1; every earlier one is complete
+  int64_t mx = last_seq * out_group + out_off + (M - 1 - last_seq * in_group);
+  if (last_seq > 0) mx = std::max(mx, (last_seq - 1) * out_group + out_off + in_group - 1);
+  return mx;
+}
+
+// y = act(A W^T + b) or LayerNorm(A W^T + b + R) through the engine's GEMM operators, with the GEMM's row map and
+// output placement (include/mldb.h), so tests can compare the wgmma kernels with the CUDA-core kernels (and with
+// torch) shape by shape.
+extern "C" int mldb_debug_gemm_rows(mldb_handle* h, const mldb_gemm_rows_args* a, void* stream) {
+  if (!h || !a || !a->A || !a->W || !a->out || a->M <= 0 || a->N <= 0 || a->K <= 0) FAIL(MLDB_ERR_INVALID, "bad argument");
+  const int M = a->M, N = a->N, K = a->K;
+  const int64_t max_row = map_max_row(M, a->in_group, a->out_group, a->out_off);
+  if (max_row < 0 || max_row >= a->out_rows) FAIL(MLDB_ERR_INVALID, "the row map leaves the %d output rows", a->out_rows);
+  if (a->out_col0 < 0 || (int64_t)a->out_col0 + N > a->out_cols) FAIL(MLDB_ERR_INVALID, "columns outside the output");
+  const int tab_need = a->out_off + std::min(a->in_group, M);
+  if (a->addtab && a->tab_rows < tab_need) FAIL(MLDB_ERR_INVALID, "addtab needs %d rows", tab_need);
+  if (a->a_kind < A_SPLIT || a->a_kind > A_F32_RELU) FAIL(MLDB_ERR_INVALID, "a_kind %d", a->a_kind);
+  if (a->a_kind != A_SPLIT && a->use_tc) FAIL(MLDB_ERR_UNSUPPORTED, "an fp32 A runs on the CUDA-core kernel only");
+  const bool identity = a->in_group >= M && a->out_group == 0 && a->out_off == 0 && !a->addtab && !a->zero_lengths;
+  if (a->gamma && (!a->beta || !identity || a->out_rows != M || a->out_cols != N || a->out_col0 != 0 ||
+                   a->a_kind != A_SPLIT))
+    FAIL(MLDB_ERR_INVALID, "the LayerNorm epilogue takes a split16 A, the identity map and an [M, N] output");
   DeviceGuard guard(h->device);
   cudaStream_t st = (cudaStream_t)stream;
   const size_t n_alloc0 = h->allocs.size();
   LinW w;
-  TRY(pack_linear(h, W, N, K, bias, &w));
-  if (K1 <= 0 || K1 >= K) K1 = K;
-  ActBuf a1, a2{}, res{}, o{};
-  TRY(alloc_act(h, M, K1, &a1));
-  k_rows_to_split<<<nblk((int64_t)M * K1), 256, 0, st>>>(a1, A, K, M, K1, 1 << 30, 0, 0, 0, nullptr);
-  if (K1 < K) {
-    TRY(alloc_act(h, M, K - K1, &a2));
-    k_rows_to_split<<<nblk((int64_t)M * (K - K1)), 256, 0, st>>>(a2, A + K1, K, M, K - K1, 1 << 30, 0, 0, 0, nullptr);
-  }
-  float *g = nullptr, *b = nullptr, *cf32 = nullptr;
-  const bool saved = h->use_tc;
-  h->use_tc = use_tc != 0;
-  GemmArgs ga; ga.a1 = a1; ga.K1 = K1; ga.a2 = a2; ga.K2 = K - K1; ga.M = M; ga.w = w; ga.act = act; ga.wide_n = 1;
-  if (gamma) {
-    TRY(upload_f32(h, gamma, N, &g));
-    TRY(upload_f32(h, beta, N, &b));
-    TRY(dev_alloc(h, (void**)&cf32, (size_t)M * N * sizeof(float)));
-    TRY(alloc_act(h, M, N, &o));
-    if (R) {
-      TRY(alloc_act(h, M, N, &res));
-      k_rows_to_split<<<nblk((int64_t)M * N), 256, 0, st>>>(res, R, N, M, N, 1 << 30, 0, 0, 0, nullptr);
+  TRY(pack_linear(h, a->W, N, K, a->bias, &w));
+  const int K1 = (a->K1 <= 0 || a->K1 >= K) ? K : a->K1;
+  GemmArgs ga; ga.M = M; ga.w = w; ga.act = a->act; ga.wide_n = 1; ga.vec_f32 = a->vec_f32;
+  ga.in_group = a->in_group; ga.out_group = a->out_group; ga.out_off = a->out_off;
+  ga.a_kind = a->a_kind;
+  if (a->a_kind == A_SPLIT) {
+    ActBuf a1, a2{};
+    TRY(alloc_act(h, M, K1, &a1));
+    k_rows_to_split<<<nblk((int64_t)M * K1), 256, 0, st>>>(a1, a->A, K, M, K1, 1 << 30, 0, 0, 0, nullptr);
+    if (K1 < K) {
+      TRY(alloc_act(h, M, K - K1, &a2));
+      k_rows_to_split<<<nblk((int64_t)M * (K - K1)), 256, 0, st>>>(a2, a->A + K1, K, M, K - K1, 1 << 30, 0, 0, 0, nullptr);
     }
+    ga.a1 = a1; ga.K1 = K1; ga.a2 = a2; ga.K2 = K - K1;
+  } else {
+    ga.a_f32 = a->A; ga.lda = K; ga.K1 = K;
+  }
+  float* tab = nullptr;
+  int32_t* zl = nullptr;
+  if (a->addtab) TRY(upload_f32(h, a->addtab, (size_t)a->tab_rows * N, &tab));
+  if (a->zero_lengths) {
+    const int nseq = (int)((M - 1) / a->in_group + 1);
+    TRY(dev_alloc(h, (void**)&zl, (size_t)nseq * sizeof(int32_t)));
+    CK(cudaMemcpyAsync(zl, a->zero_lengths, (size_t)nseq * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+  }
+  ga.addtab = tab; ga.zero_lengths = zl;
+  ActBuf o{}, res{};
+  float *g = nullptr, *b = nullptr, *cf32 = nullptr;
+  if (a->gamma) {
+    TRY(upload_f32(h, a->gamma, N, &g));
+    TRY(upload_f32(h, a->beta, N, &b));
+    TRY(dev_alloc(h, (void**)&cf32, (size_t)M * N * sizeof(float)));
+    TRY(debug_to_split(h, a->out, M, N, &o, st));
+    if (a->R) TRY(debug_to_split(h, a->R, M, N, &res, st));
+  } else if (a->split_out && !a->R) {              // the production epilogue: split16 planes
+    TRY(debug_to_split(h, a->out, a->out_rows, a->out_cols, &o, st));
+  }
+  const bool saved = h->use_tc;
+  h->use_tc = a->use_tc != 0;
+  if (a->gamma) {
     LnArgs l; l.res = res; l.gamma = g; l.beta = b; l.M = M; l.d = N; l.out = o;
     op_gemm_ln(h, ga, l, cf32, st);
-    k_split_to_f32<<<nblk((int64_t)M * N), 256, 0, st>>>(o, out, (int64_t)M * N);
-  } else if (R) {                                  // residual add, fp32 out (in place when R == out)
-    ga.res_f32 = R; ga.out_f32 = out; ga.ldc = N;
+  } else if (o.hi) {
+    ga.out = o; ga.out_col0 = a->out_col0;
     op_gemm(h, ga, st);
-  } else if (split_out && N % 8 == 0) {
-    TRY(alloc_act(h, M, N, &o));                   // the production epilogue: split16 planes
-    ga.out = o;
-    op_gemm(h, ga, st);
-    k_split_to_f32<<<nblk((int64_t)M * N), 256, 0, st>>>(o, out, (int64_t)M * N);
-  } else {
-    ga.out_f32 = out; ga.ldc = N;
+  } else {                                         // fp32 out (+ residual: in place when R == out)
+    ga.out_f32 = a->out + a->out_col0; ga.ldc = a->out_cols;
+    if (a->R) ga.res_f32 = a->R + a->out_col0;
     op_gemm(h, ga, st);
   }
+  if (o.hi) debug_from_split(o, a->out, st);
   h->use_tc = saved;
   return debug_exit(h, n_alloc0, st, "debug gemm");
+}
+
+extern "C" int mldb_debug_gemm(mldb_handle* h, const float* A, const float* W, const float* bias,
+                               const float* gamma, const float* beta, const float* R, int32_t M, int32_t N,
+                               int32_t K, int32_t K1, int32_t act, int32_t use_tc, int32_t split_out, float* out,
+                               void* stream) {
+  mldb_gemm_rows_args a{};
+  a.A = A; a.W = W; a.bias = bias; a.gamma = gamma; a.beta = beta; a.R = R;
+  a.M = M; a.N = N; a.K = K; a.K1 = K1; a.act = act; a.use_tc = use_tc; a.a_kind = A_SPLIT;
+  a.in_group = 1 << 30; a.out_group = 0; a.out_off = 0;
+  a.split_out = split_out && N % 8 == 0;
+  a.out = out; a.out_rows = M; a.out_cols = N; a.out_col0 = 0;
+  return mldb_debug_gemm_rows(h, &a, stream);
+}
+
+extern "C" int mldb_debug_ln(mldb_handle* h, const mldb_ln_args* a, void* stream) {
+  if (!h || !a || !a->gamma || !a->beta || !a->out || a->M <= 0 || a->M_in <= 0 || a->d <= 0 ||
+      a->ld_out < a->d || (a->c && a->ldc < a->d) || (a->rowvec && a->rv_group <= 0))
+    FAIL(MLDB_ERR_INVALID, "bad argument");
+  if (a->d > LN_MAX_D) FAIL(MLDB_ERR_UNSUPPORTED, "LayerNorm rows of %d columns: the CUDA-core kernels take up to %d", a->d, LN_MAX_D);
+  if (a->in_group != 0 && (a->in_group < 0 || a->sel_group <= 0)) FAIL(MLDB_ERR_INVALID, "bad row gather");
+  // the input row of r: r, or (r / sel_group) * in_group + r % sel_group; the largest is one of the last two
+  // sequences' last rows
+  auto in_row = [&](int64_t r) { return a->in_group == 0 ? r : (r / a->sel_group) * a->in_group + r % a->sel_group; };
+  int64_t mx = in_row(a->M - 1);
+  if (a->in_group != 0 && a->M > a->sel_group) mx = std::max(mx, in_row(((a->M - 1) / a->sel_group) * a->sel_group - 1));
+  if (mx >= a->M_in) FAIL(MLDB_ERR_INVALID, "the row gather reads past the %d input rows", a->M_in);
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t n_alloc0 = h->allocs.size();
+  LnArgs l; l.c = a->c; l.ldc = a->ldc; l.M = a->M; l.d = a->d; l.act = a->act;
+  if (a->in_group != 0) { l.sel_group = a->sel_group; l.in_group = a->in_group; }
+  float *g = nullptr, *b = nullptr, *rv = nullptr;
+  TRY(upload_f32(h, a->gamma, a->d, &g));
+  TRY(upload_f32(h, a->beta, a->d, &b));
+  l.gamma = g; l.beta = b;
+  if (a->rowvec) {
+    TRY(upload_f32(h, a->rowvec, (size_t)((a->M_in + a->rv_group - 1) / a->rv_group) * a->d, &rv));
+    l.rowvec = rv; l.rv_group = a->rv_group;
+  }
+  if (a->res) TRY(debug_to_split(h, a->res, a->M_in, a->d, &l.res, st));
+  if (a->split_out) TRY(debug_to_split(h, a->out, a->M, a->ld_out, &l.out, st));
+  else { l.out_f32 = a->out; l.ld_out = a->ld_out; }
+  op_ln(h, l, st);
+  if (l.out.hi) debug_from_split(l.out, a->out, st);
+  return debug_exit(h, n_alloc0, st, "debug ln");
+}
+
+extern "C" int mldb_debug_rows_to_split(mldb_handle* h, const float* src, int32_t ld_src, int32_t M, int32_t d,
+                                        int32_t in_group, int32_t out_group, int32_t out_off, int32_t src_bcast,
+                                        const float* tab, int32_t tab_rows, int32_t relu, int32_t scalar, float* out,
+                                        int32_t out_rows, int32_t out_cols, void* stream) {
+  if (!h || !out || M <= 0 || d <= 0 || d > out_cols || (src && ld_src < d)) FAIL(MLDB_ERR_INVALID, "bad argument");
+  const int64_t max_row = map_max_row(M, in_group, out_group, out_off);
+  if (max_row < 0 || max_row >= out_rows) FAIL(MLDB_ERR_INVALID, "the row map leaves the %d output rows", out_rows);
+  const int tab_need = out_off + std::min(in_group, M);
+  if (tab && tab_rows < tab_need) FAIL(MLDB_ERR_INVALID, "tab needs %d rows", tab_need);
+  DeviceGuard guard(h->device);
+  cudaStream_t st = (cudaStream_t)stream;
+  const size_t n_alloc0 = h->allocs.size();
+  float* tb = nullptr;
+  if (tab) TRY(upload_f32(h, tab, (size_t)tab_rows * d, &tb));
+  ActBuf x;
+  TRY(debug_to_split(h, out, out_rows, out_cols, &x, st));
+  if (scalar)
+    k_rows_to_split<<<nblk((int64_t)M * d), 256, 0, st>>>(x, src, ld_src, M, d, in_group, out_group, out_off, src_bcast,
+                                                          tb, relu);
+  else
+    rows_to_split(h, x, src, ld_src, M, d, in_group, out_group, out_off, src_bcast, tb, relu, st);
+  debug_from_split(x, out, st);
+  return debug_exit(h, n_alloc0, st, "debug rows_to_split");
 }
 
 extern "C" int mldb_debug_ffn(mldb_handle* h, const float* X, const float* W1, const float* b1, const float* W2,

@@ -997,7 +997,7 @@ bool tc_gemm_ln_supported(const TcCtx* c, const GemmArgs& g, const LnArgs& l) {
   if (g.w.N != 256 || l.d != 256 || g.act != ACT_NONE) return false;
   if (l.in_group != 0 || l.c != nullptr || l.out_f32 != nullptr || !l.out.hi) return false;
   if (l.out.cols != 256 || (l.res.hi && l.res.cols != 256)) return false;
-  if (l.gamma2 || l.rowvec) return false;
+  if (l.rowvec) return false;
   if (g.addtab || g.zero_lengths || g.in_group < g.M || g.out_group != 0 || g.out_off != 0) return false;
   return true;
 }

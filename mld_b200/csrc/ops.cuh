@@ -30,7 +30,8 @@ struct GemmArgs {
   ActBuf out{};               // split output when out.hi != nullptr (ld = out.cols)
   int out_col0 = 0;           // column offset inside out
   float* out_f32 = nullptr; int ldc = 0;
-  // row r -> out row (r / in_group) * out_group + out_off + r % in_group (identity when in_group >= M)
+  // row r -> out row (r / in_group) * out_group + out_off + r % in_group, on every path (so out_off + r when
+  // in_group >= M; the defaults give the identity)
   int in_group = 1 << 30, out_group = 0, out_off = 0;
   const float* addtab = nullptr;        // [*, N]: row (out_off + r % in_group)
   const int32_t* zero_lengths = nullptr;  // zero rows with (r % in_group) >= zero_lengths[r / in_group]
@@ -44,15 +45,13 @@ struct GemmArgs {
                                         // sampling path keeps the generic epilogue it was validated with
 };
 
-// y = LayerNorm(c + res + rowvec[r / rv_group]) * gamma + beta, eps 1e-5; optional second LN
-// (gamma2/beta2) applied on top (last block's norm2 followed by the stack's final norm).
+// y = LayerNorm(c + res + rowvec[in_row / rv_group]) * gamma + beta, eps 1e-5
 struct LnArgs {
   const float* c = nullptr; int ldc = 0;   // fp32 GEMM result incl. bias (nullable)
   ActBuf res{};                              // residual (nullable: res.hi == nullptr)
   const float* rowvec = nullptr; int rv_group = 1;
   const float* gamma = nullptr; const float* beta = nullptr;
-  const float* gamma2 = nullptr; const float* beta2 = nullptr;
-  int M = 0, d = 0;
+  int M = 0, d = 0;                          // d <= LN_MAX_D on the CUDA cores (simt_ln)
   // input row selection: in_row = (r / sel_group) * in_group + r % sel_group (identity default)
   int sel_group = 1 << 30, in_group = 0;
   ActBuf out{}; float* out_f32 = nullptr; int ld_out = 0;
@@ -86,6 +85,9 @@ struct StepCoef {
 
 // --- SIMT implementations (simt.cu) ---
 void simt_gemm(const GemmArgs& a, cudaStream_t st);
+// One warp per row; the widest kernel keeps 32 columns per lane, so rows of up to LN_MAX_D columns.  Callers keep
+// d within it (mldb_create's latent_dim, gru_shape_supported's H, mldb_debug_ln).
+constexpr int LN_MAX_D = 1024;
 void simt_ln(const LnArgs& a, cudaStream_t st);
 // CUDA-core attention: any Lq / Lk (K and V stream through shared memory in key chunks).  false: the head is too
 // wide for the shared memory (simt_attention_supported), nothing launched.

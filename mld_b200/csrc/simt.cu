@@ -73,9 +73,7 @@ __global__ void __launch_bounds__(256) k_gemm_simt(const GemmArgs a) {
     const int m = m0 + ty * 4 + i;
     if (m >= M) continue;
     const int seq = m / a.in_group, pos = m - seq * a.in_group;
-    const int64_t orow = (a.in_group >= M && a.out_group == 0)
-                             ? (int64_t)m
-                             : (int64_t)seq * a.out_group + a.out_off + pos;
+    const int64_t orow = (int64_t)seq * a.out_group + a.out_off + pos;
     const bool zero = a.zero_lengths != nullptr && pos >= a.zero_lengths[seq];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
@@ -127,7 +125,7 @@ __global__ void __launch_bounds__(256) k_ln(const LnArgs a) {
     s += x;
   }
   const float inv_d = 1.0f / (float)a.d;
-  float mean = warp_sum(s) * inv_d;
+  const float mean = warp_sum(s) * inv_d;
   float q = 0.0f;
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
@@ -135,29 +133,11 @@ __global__ void __launch_bounds__(256) k_ln(const LnArgs a) {
     float dlt = (n < a.d) ? v[i] - mean : 0.0f;
     q += dlt * dlt;
   }
-  float rstd = rsqrtf(warp_sum(q) * inv_d + 1e-5f);
+  const float rstd = rsqrtf(warp_sum(q) * inv_d + 1e-5f);
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
     const int n = i * 32 + lane;
     if (n < a.d) v[i] = (v[i] - mean) * rstd * a.gamma[n] + a.beta[n];
-  }
-  if (a.gamma2) {  // stack-final LayerNorm on top (cross_attention.py:62-63)
-    s = 0.0f;
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) s += (i * 32 + lane < a.d) ? v[i] : 0.0f;
-    mean = warp_sum(s) * inv_d;
-    q = 0.0f;
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) {
-      float dlt = (i * 32 + lane < a.d) ? v[i] - mean : 0.0f;
-      q += dlt * dlt;
-    }
-    rstd = rsqrtf(warp_sum(q) * inv_d + 1e-5f);
-#pragma unroll
-    for (int i = 0; i < VPL; ++i) {
-      const int n = i * 32 + lane;
-      if (n < a.d) v[i] = (v[i] - mean) * rstd * a.gamma2[n] + a.beta2[n];
-    }
   }
 #pragma unroll
   for (int i = 0; i < VPL; ++i) {
@@ -368,7 +348,6 @@ __global__ void __launch_bounds__(256) k_ln_vec(const LnArgs a) {
   };
   (void)s;
   normalise(a.gamma, a.beta);
-  if (a.gamma2) normalise(a.gamma2, a.beta2);   // stack-final LayerNorm on top (cross_attention.py:62-63)
   if (a.act != ACT_NONE)
 #pragma unroll
     for (int i = 0; i < NIT; ++i)
@@ -407,6 +386,7 @@ void simt_gemm(const GemmArgs& a, cudaStream_t st) {
   k_gemm_simt<<<grid, 256, 0, st>>>(a);
 }
 
+// d <= LN_MAX_D (k_ln<32> covers 32 x 32 columns; the callers keep d within it)
 void simt_ln(const LnArgs& a, cudaStream_t st) {
   const int rows_per_block = 8;
   dim3 grid((a.M + rows_per_block - 1) / rows_per_block);
@@ -416,7 +396,7 @@ void simt_ln(const LnArgs& a, cudaStream_t st) {
                       (!a.out.hi || (a.out.cols % 8 == 0 && ((uintptr_t)a.out.hi & 15) == 0 && (a.out.plane_stride % 8) == 0)) &&
                       (!a.out_f32 || (a.ld_out % 4 == 0 && ((uintptr_t)a.out_f32 & 15) == 0)) &&
                       (!a.rowvec || ((uintptr_t)a.rowvec & 15) == 0) && ((uintptr_t)a.gamma & 15) == 0 &&
-                      ((uintptr_t)a.beta & 15) == 0 && (!a.gamma2 || (((uintptr_t)a.gamma2 & 15) == 0 && ((uintptr_t)a.beta2 & 15) == 0));
+                      ((uintptr_t)a.beta & 15) == 0;
   if (vec_ok && a.d == 256) launch_pdl(k_ln_vec<1>, grid, dim3(256), 0, st, a);
   else if (vec_ok) launch_pdl(k_ln_vec<2>, grid, dim3(256), 0, st, a);
   else if (a.d <= 256) launch_pdl(k_ln<8>, grid, dim3(256), 0, st, a);

@@ -104,6 +104,88 @@ class Engine:
               "mldb_debug_gemm")
         return out
 
+    def _out_buffer(self, out, what):
+        if out.dtype != torch.float32 or out.device != self.device or out.dim() != 2 or not out.is_contiguous():
+            raise ValueError(f"{what}: out must be a contiguous fp32 [rows, cols] tensor on {self.device}")
+        return out
+
+    def _rows_view(self, t, what):
+        """A device fp32 2-D tensor whose rows may be strided (a column slice of a wider buffer): (t, ld)."""
+        if t.dtype != torch.float32 or t.device != self.device or t.dim() != 2 or t.stride(1) != 1:
+            raise ValueError(f"{what} must be an fp32 2-D tensor on {self.device} with unit column stride")
+        return t, t.stride(0)
+
+    def debug_gemm_rows(self, A, W, bias=None, *, out, out_col0=0, split_out=False, act=0, use_tc=True, K1=0,
+                        a_kind=0, in_group=1 << 30, out_group=0, out_off=0, addtab=None, zero_lengths=None,
+                        vec_f32=False, R=None, gamma=None, beta=None):
+        """Kernel unit-test hook (mldb_debug_gemm_rows): the GEMM with its row map and output placement.  Row r of
+        act(A W^T + b + addtab[out_off + r % in_group]) goes to row (r / in_group) * out_group + out_off + r % in_group,
+        columns [out_col0, out_col0 + N) of ``out`` (device fp32, filled by the caller, written in place and returned;
+        ``split_out``: through split16 planes).  ``zero_lengths`` (host, one per sequence of in_group rows) zeroes rows
+        r % in_group >= zero_lengths[r / in_group].  a_kind 1 / 2: fp32 A / fp32 A through ReLU (CUDA cores)."""
+        A = _f32c(A, self.device)
+        out = self._out_buffer(out, "debug_gemm_rows")
+        Wc = W.detach().float().contiguous().cpu()
+        host = [None if t is None else t.detach().float().contiguous().cpu() for t in (bias, gamma, beta, addtab)]
+        M, K = A.shape
+        N = Wc.shape[0]
+        zl = None
+        if zero_lengths is not None:
+            zl = torch.as_tensor(zero_lengths, dtype=torch.int32).contiguous().cpu()
+            if zl.numel() != (M - 1) // in_group + 1:
+                raise ValueError("debug_gemm_rows: zero_lengths needs one entry per sequence of in_group rows")
+        Rd = None if R is None else _f32c(R, self.device)
+        a = _lib.MldbGemmRowsArgs(
+            A=A.data_ptr(), W=Wc.data_ptr(), bias=_ptr(host[0]), gamma=_ptr(host[1]), beta=_ptr(host[2]),
+            R=_ptr(Rd), M=M, N=N, K=K, K1=K1, act=act, use_tc=int(use_tc), a_kind=a_kind, in_group=in_group,
+            out_group=out_group, out_off=out_off, addtab=_ptr(host[3]),
+            tab_rows=0 if addtab is None else host[3].shape[0], zero_lengths=_ptr(zl), vec_f32=int(vec_f32),
+            split_out=int(split_out), out=out.data_ptr(), out_rows=out.shape[0], out_cols=out.shape[1],
+            out_col0=out_col0)
+        check(self.lib.mldb_debug_gemm_rows(self._h, C.byref(a), self._stream()), "mldb_debug_gemm_rows")
+        return out
+
+    def debug_ln(self, gamma, beta, *, out, c=None, res=None, rowvec=None, rv_group=1, M_in=None, sel_group=0,
+                 in_group=0, act=0, split_out=False):
+        """Kernel unit-test hook (mldb_debug_ln): out[r, :d] = act(LayerNorm(c[i] + res[i] + rowvec[i / rv_group])),
+        i = r, or (r / sel_group) * in_group + r % sel_group when in_group > 0.  c: device [M_in, >= d] (rows may
+        be strided), res: device [M_in, d], rowvec / gamma / beta: host.  ``out`` (device fp32 [M, >= d], filled by
+        the caller) is written in place and returned; ``split_out``: through split16 planes."""
+        out = self._out_buffer(out, "debug_ln")
+        g, b = (t.detach().float().contiguous().cpu() for t in (gamma, beta))
+        d = g.numel()
+        ldc = 0
+        if c is not None:
+            c, ldc = self._rows_view(c, "debug_ln: c")
+        if res is not None:
+            res = _f32c(res, self.device)
+        rv = None if rowvec is None else rowvec.detach().float().contiguous().cpu()
+        if M_in is None:
+            M_in = (c if c is not None else res).shape[0]
+        a = _lib.MldbLnArgs(
+            c=_ptr(c), ldc=ldc, res=_ptr(res), rowvec=_ptr(rv), rv_group=rv_group, gamma=g.data_ptr(),
+            beta=b.data_ptr(), M_in=M_in, M=out.shape[0], d=d, sel_group=sel_group, in_group=in_group, act=act,
+            split_out=int(split_out), out=out.data_ptr(), ld_out=out.shape[1])
+        check(self.lib.mldb_debug_ln(self._h, C.byref(a), self._stream()), "mldb_debug_ln")
+        return out
+
+    def debug_rows_to_split(self, src, M, d, *, out, in_group=1 << 30, out_group=0, out_off=0, src_bcast=False,
+                            tab=None, relu=False, scalar=False):
+        """Kernel unit-test hook (mldb_debug_rows_to_split): row r of relu?(src[r or r % in_group, :d]) +
+        tab[out_off + r % in_group] into row (r / in_group) * out_group + out_off + r % in_group of ``out`` (device
+        fp32, filled by the caller, passed through split16 planes and returned).  src: device [rows, >= d] (rows may
+        be strided) or None; tab: host [rows, d].  ``scalar``: the one-column-per-thread kernel."""
+        out = self._out_buffer(out, "debug_rows_to_split")
+        ld = 0
+        if src is not None:
+            src, ld = self._rows_view(src, "debug_rows_to_split: src")
+        tb = None if tab is None else tab.detach().float().contiguous().cpu()
+        check(self.lib.mldb_debug_rows_to_split(self._h, _ptr(src), ld, M, d, in_group, out_group, out_off,
+                                                int(src_bcast), _ptr(tb), 0 if tb is None else tb.shape[0], int(relu),
+                                                int(scalar), out.data_ptr(), out.shape[0], out.shape[1],
+                                                self._stream()), "mldb_debug_rows_to_split")
+        return out
+
     def debug_ffn(self, X, W1, b1, W2, b2, gamma, beta, mode=2):
         """Kernel unit-test hook (mldb_debug_ffn): LayerNorm(X + W2 gelu(W1 X + b1) + b2); mode 0 CUDA-core,
         1 wgmma GEMMs (two launches), 2 fused wgmma FFN kernel.  X [M,d] (device), the rest host."""
