@@ -24,7 +24,6 @@
 namespace {
 using namespace tc;
 
-constexpr int ATC_THREADS = 384;          // producer warpgroup (warps 0 / 1 feed pipelines 0 / 1) + two consumer warpgroups
 constexpr int KBLK = 64;                  // keys per block
 constexpr int QROWS = 64;                 // query rows per item
 constexpr int MAX_KB = 4;                 // key blocks of the longest score row (256 keys)
@@ -73,7 +72,7 @@ __device__ __forceinline__ float quad_max(float v) {
 // warpgroup has 168 (three warpgroups per CTA), so the <= 128-key shapes (the denoiser's 79 tokens, the text
 // tower's 77) compile without spills or serialised MMAs only when the row is sized for them.
 template <int HD, bool CAUSAL, int KB>
-__global__ void __launch_bounds__(ATC_THREADS, 1)
+__global__ void __launch_bounds__(WS_THREADS, 1)        // warps 0 / 1 of the producer warpgroup feed pipelines 0 / 1
 k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
           const __grid_constant__ CUtensorMap tmKh, const __grid_constant__ CUtensorMap tmKl,    // 64-row boxes
           const __grid_constant__ CUtensorMap tmRh, const __grid_constant__ CUtensorMap tmRl,    // rem-row boxes
@@ -88,6 +87,10 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * PIPE_BYTES);
+  // pipeline g's barriers: its Q buffer's full and empty, then its K / V ring's RS full and RS empty.  Every empty
+  // barrier takes one arrival per warp of the pipeline's consumer warpgroup.
+  auto q_ring = [&](int g) { uint64_t* b = bars + g * (2 + 2 * RS); return Ring<1>{b, b + 1}; };
+  auto kv_ring = [&](int g) { uint64_t* b = bars + g * (2 + 2 * RS) + 2; return Ring<RS>{b, b + RS}; };
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
   int tl_n = 0;                                       // debug-timeline event counter of this warp
@@ -95,10 +98,8 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   const int nkb = p.nkb;
   if (threadIdx.x == 0) {
     for (int g = 0; g < 2; ++g) {
-      uint64_t* b = bars + g * (2 + 2 * MAX_RS);
-      mbar_init(smem_u32(&b[0]), 1);                  // q_full (TMA tx)
-      mbar_init(smem_u32(&b[1]), 4);                  // q_empty (one arrival per warp of the consumer warpgroup)
-      for (int i = 0; i < MAX_RS; ++i) { mbar_init(smem_u32(&b[2 + i]), 1); mbar_init(smem_u32(&b[2 + MAX_RS + i]), 4); }
+      q_ring(g).init(4);
+      kv_ring(g).init(4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     tma_prefetch_desc(&tmQh); tma_prefetch_desc(&tmQl); tma_prefetch_desc(&tmKh); tma_prefetch_desc(&tmKl);
@@ -112,15 +113,13 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
   const int g = producer ? (warp & 1) : (warp >> 2) - 1;    // pipeline of this warp
   uint8_t* const sQ = smem + g * PIPE_BYTES;
   uint8_t* const sR = sQ + SLOT_BYTES;
-  uint64_t* const q_full = bars + g * (2 + 2 * MAX_RS);
-  uint64_t* const q_empty = q_full + 1;
-  uint64_t* const r_full = q_full + 2;
-  uint64_t* const r_empty = r_full + MAX_RS;
+  const Ring<1> qr = q_ring(g);
+  const Ring<RS> kvr = kv_ring(g);
   const int pid = (int)blockIdx.x * 2 + g, npipes = (int)gridDim.x * 2;
   const int nlocal = (p.items - pid + npipes - 1) / npipes;
 
   if (producer) {
-    reg_dec<40>();
+    reg_dec<PRODUCER_REGS>();
     if (warp >= 2) return;
     // ------------------------------------------------------------------ TMA producer of pipeline g:
     // Q(j), the K blocks of item j, its V blocks - exactly the order the consumer takes them
@@ -128,10 +127,10 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     for (int j = 0; j < nlocal; ++j) {
       const Item it = decode_item(pid + j * npipes, p);
       const int nkb_i = item_kblocks<CAUSAL>(it, nkb);
-      mbar_wait(smem_u32(q_empty), ((uint32_t)j & 1u) ^ 1u);
+      qr.wait_empty(j);
       tl_event(p.tl, tl_n, 20, j);                                     // producer: Q buffer free, loads issued
       if (elect_one()) {
-        const uint32_t full = smem_u32(q_full);
+        const uint32_t full = qr.full_bar(j);
         mbar_expect_tx(full, (uint32_t)SLOT_BYTES);
         const uint32_t base = smem_u32(sQ);
         const int r0 = it.s * p.Lq + it.qt * QROWS;
@@ -145,14 +144,13 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
       for (int kv = 0; kv < 2; ++kv) {
         const int col0 = (kv ? p.v_col0 : p.k_col0) + it.h * HD;
         for (int kb = 0; kb < nkb_i; ++kb, ++rc) {
-          const int sl_i = rc % RS;
-          mbar_wait(smem_u32(&r_empty[sl_i]), (((uint32_t)(rc / RS)) & 1u) ^ 1u);
+          kvr.wait_empty(rc);
           if (elect_one()) {
             const bool last = kb == nkb - 1;
             const int rows = last ? p.rem : KBLK;
-            const uint32_t full = smem_u32(&r_full[sl_i]);
+            const uint32_t full = kvr.full_bar(rc);
             mbar_expect_tx(full, (uint32_t)(2 * NS * rows * 128));
-            const uint32_t base = smem_u32(sR + sl_i * SLOT_BYTES);
+            const uint32_t base = smem_u32(sR + (rc % RS) * SLOT_BYTES);
             // the last block's rows past Lk would be the next sequence's first keys: its [seq, key, col] map
             // zero-fills them, since P = 0 times a non-finite V is NaN
 #pragma unroll
@@ -173,7 +171,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     return;
   }
   // -------------------------------------------------------------------- consumer warpgroup of pipeline g
-  reg_inc<232>();
+  reg_inc<CONSUMER_REGS>();
   const int cp = 2 * (lane & 3);                      // column offset inside an 8-column group
   const int row = (warp & 3) * 16 + (lane >> 2);      // this thread's first query row (the second is row + 8)
   const float sc = p.scale_log2e;
@@ -188,16 +186,15 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
     // valid keys of this thread's two query rows (causal: keys j <= i)
     const int q0 = it.qt * QROWS + row;
     const int nk0 = CAUSAL ? min(nk, q0 + 1) : nk, nk1 = CAUSAL ? min(nk, q0 + 9) : nk;
-    mbar_wait(smem_u32(q_full), (uint32_t)j & 1u);
+    qr.wait_full(j);
     tl_event(p.tl, tl_n, 22, j);                                       // Q(j) landed
     // ---- S = Q K^T, block by block; a block's ring slot is freed when the NEXT block's MMAs have been issued
     const uint32_t qbase = smem_u32(sQ);
 #pragma unroll
     for (int kb = 0; kb < KB; ++kb) {
       if (kb < nkb_i) {
-        const int sl_i = (rc + kb) % RS;
-        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
-        const uint32_t kbase = smem_u32(sR + sl_i * SLOT_BYTES);
+        kvr.wait_full(rc + kb);
+        const uint32_t kbase = smem_u32(sR + ((rc + kb) % RS) * SLOT_BYTES);
         wg_fence();
 #pragma unroll
         for (int sl = 0; sl < NS; ++sl)               // one k-block per 64-wide slice of the head dimension
@@ -206,14 +203,14 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
         wg_commit();
         if (kb > 0) {
           wg_wait<1>();
-          if (lane == 0) mbar_arrive(smem_u32(&r_empty[(rc + kb - 1) % RS]));
+          if (lane == 0) kvr.release(rc + kb - 1);
         }
       }
     }
     wg_wait<0>();
     if (lane == 0) {
-      mbar_arrive(smem_u32(&r_empty[(rc + nkb_i - 1) % RS]));
-      mbar_arrive(smem_u32(q_empty));                 // Q only feeds the scores
+      kvr.release(rc + nkb_i - 1);
+      qr.release(j);                                  // Q only feeds the scores
     }
     rc += nkb_i;
 #pragma unroll
@@ -272,9 +269,8 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
         for (int ks = 0; ks < 4; ++ks)
 #pragma unroll
           for (int i = 0; i < 4; ++i) split2(S[kb][8 * ks + 2 * i], S[kb][8 * ks + 2 * i + 1], ph[ks][i], pl[ks][i]);
-        const int sl_i = (rc + kb) % RS;
-        mbar_wait(smem_u32(&r_full[sl_i]), ((uint32_t)((rc + kb) / RS)) & 1u);
-        const uint32_t vbase = smem_u32(sR + sl_i * SLOT_BYTES);
+        kvr.wait_full(rc + kb);
+        const uint32_t vbase = smem_u32(sR + ((rc + kb) % RS) * SLOT_BYTES);
         const int nks = (kb == nkb - 1 ? p.rem : KBLK) / 16;           // rows beyond `rem` of the slot are stale
         wg_fence();
 #pragma unroll
@@ -292,7 +288,7 @@ k_attn_tc(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUte
         }
         wg_commit();
         wg_wait<0>();
-        if (lane == 0) mbar_arrive(smem_u32(&r_empty[sl_i]));
+        if (lane == 0) kvr.release(rc + kb);
       }
     }
     rc += nkb_i;
@@ -382,6 +378,6 @@ bool tc_attention(const AttnArgs& a, int sm_count, cudaStream_t st) {
   const int grid = pairs < sm_count ? pairs : sm_count;
   auto kernel = a.hd == 64 ? (a.causal ? pick_kernel<64, true>(p.nkb) : pick_kernel<64, false>(p.nkb))
                            : (a.causal ? pick_kernel<128, true>(p.nkb) : pick_kernel<128, false>(p.nkb));
-  launch_pdl(kernel, dim3(grid), dim3(ATC_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
+  launch_pdl(kernel, dim3(grid), dim3(WS_THREADS), (size_t)SMEM_BYTES, st, mQh, mQl, mKh, mKl, mRh, mRl, p);
   return true;
 }

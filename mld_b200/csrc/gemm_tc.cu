@@ -30,10 +30,7 @@
 namespace {
 using namespace tc;
 
-constexpr int BM = 128, BK = 64;
-constexpr int NUM_THREADS = 384;                     // k_gemm_tc: producer warpgroup + two consumer warpgroups
 constexpr int MMA_THREADS = 256;                     // k_ffn_tc, k_proj_tc: the two MMA warpgroups only
-constexpr int CONSUMER_WARPS = 8;
 constexpr int MAX_N = 1024;
 constexpr int MAX_N_WIDE = 4096;                     // GemmArgs::wide_n
 
@@ -205,174 +202,120 @@ __device__ __forceinline__ void ln_tile(float (&d)[128], float sc, const float* 
 // table, row remapping, zeroed padding rows, fp32 output, ragged N: the per-batch embedding / final-layer
 // GEMMs) kept out of the hot kernels' instruction stream; EPI_RES = bias + fp32 residual -> fp32, N even;
 // EPI_F32 = bias + activation -> fp32, identity row mapping, N even.
+struct GemmTile { int m0, n0; };
 template <int BN, int EPI, int ACT = ACT_NONE>      // ACT: the fast / fp32 epilogue's activation (NONE | GELU | QUICKGELU | LEAKY)
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(WS_THREADS, 1)
 k_gemm_tc(const __grid_constant__ CUtensorMap tmA1h, const __grid_constant__ CUtensorMap tmA1l,
           const __grid_constant__ CUtensorMap tmA2h, const __grid_constant__ CUtensorMap tmA2l,
           const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const TcParams p) {
   static_assert(EPI != EPI_LN || BN == 256, "the LayerNorm epilogue covers a full 256-wide row");
-  using Cfg = TileCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
-  const Ring<STAGES> ring{bar_full, bar_full + STAGES};
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
-  int tl_n = 0;                                     // debug-timeline event counter of this warp
-  tl_event(p.tl, tl_n, 40);                       // kernel entry
-  const int ntiles = p.m_tiles * p.n_tiles;
-  const int nlocal = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  auto decode = [&](int j, int& m0, int& n0) {
+  const auto tile = [&](int j) {
     const int t = (int)blockIdx.x + j * (int)gridDim.x;
-    m0 = (t / p.n_tiles) * BM;
-    n0 = (t % p.n_tiles) * BN;
+    return GemmTile{(t / p.n_tiles) * BM, (t % p.n_tiles) * BN};
   };
-
-  if (threadIdx.x == 0) {
-    ring.init(CONSUMER_WARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tmA1h); tma_prefetch_desc(&tmA1l); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
-  }
-  pdl_trigger();               // let the next kernel's prologue overlap our tail
-  __syncthreads();
-  pdl_wait();                  // everything below touches activations of the previous kernel
-  tl_event(p.tl, tl_n, 41);                       // the previous kernel has completed
-
-  if (warp < 4) {
-    reg_dec<40>();
-    if (warp != 0) return;
-    // ---------------------------------------------------------------- TMA producer
-    // The whole warp walks the loop (uniform control flow), one elected lane issues.
-    int kbg = 0;                                   // k-block counter across tiles (ring position)
-    for (int j = 0; j < nlocal; ++j) {
-      int m0, n0;
-      decode(j, m0, n0);
-      tl_event(p.tl, tl_n, 1, j);                                    // producer: tile j begins
-      auto prefetch = [&](int kb) {
-        if (kb == 0 && j + 1 < nlocal) {
+  ws_cta<TileCfg<BN>>(
+      tmA1h, tmA1l, tmWh, tmWl, p.tl, p.kblocks, [&] { return persistent_count(p.m_tiles * p.n_tiles); }, tile,
+      [&](const GemmTile& t, int kb, const auto& s, uint32_t full) {
+        if (kb < p.kb1) {
+          tma_load_2d(s.ah, &tmA1h, full, kb * BK, t.m0);
+          tma_load_2d(s.al, &tmA1l, full, kb * BK, t.m0);
+        } else {
+          tma_load_2d(s.ah, &tmA2h, full, (kb - p.kb1) * BK, t.m0);
+          tma_load_2d(s.al, &tmA2l, full, (kb - p.kb1) * BK, t.m0);
+        }
+        tma_load_2d(s.wh, &tmWh, full, kb * BK, t.n0);   // rows >= N are zero-filled (and counted)
+        tma_load_2d(s.wl, &tmWl, full, kb * BK, t.n0);
+      },
+      [&](const GemmTile& t, float (&d)[BN / 2], const TileThread& th) {
+        const int r_lo = t.m0 + th.row(), n0 = t.n0, cp = th.cp;
+        if constexpr (EPI == EPI_LN) {
+          ln_epilogue(d, p.inv_scale, p.bias, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
+                      r_lo, p.M, cp);
+        } else if constexpr (EPI == EPI_FAST) {
+          const bool ok0 = r_lo < p.M, ok1 = r_lo + 8 < p.M;
+          const int64_t o0 = (int64_t)r_lo * p.ld_out + p.out_col0 + n0 + cp, o1 = o0 + (int64_t)8 * p.ld_out;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            float x[4];
+            fast_group<ACT>(d, j, p.inv_scale, __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp)), x);
+            if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x[0], x[1]);
+            if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x[2], x[3]);
+          }
+        } else if constexpr (EPI == EPI_RES) {
+          // each element of R is read and then overwritten by the same thread: in place is safe (plain loads, no __ldg)
+          const float sc = p.inv_scale;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + cp;
+            if (n >= p.N) continue;                    // N even: a column pair is in or out together
+            const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (r_lo + 8 * h >= p.M) continue;
+              const int64_t o = (int64_t)(r_lo + 8 * h) * p.ldc + n;
+              const float2 r = *reinterpret_cast<const float2*>(p.res_f32 + o);
+              *reinterpret_cast<float2*>(p.out_f32 + o) =
+                  make_float2(fmaf(d[4 * j + 2 * h], sc, b.x) + r.x, fmaf(d[4 * j + 2 * h + 1], sc, b.y) + r.y);
+            }
+          }
+        } else if constexpr (EPI == EPI_F32) {
+          const float sc = p.inv_scale;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int n = n0 + 8 * j + cp;
+            if (n >= p.N) continue;                    // N even: a column pair is in or out together
+            const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (r_lo + 8 * h >= p.M) continue;
+              const float x0 = apply_act(fmaf(d[4 * j + 2 * h], sc, b.x), ACT), x1 = apply_act(fmaf(d[4 * j + 2 * h + 1], sc, b.y), ACT);
+              *reinterpret_cast<float2*>(p.out_f32 + (int64_t)(r_lo + 8 * h) * p.ldc + n) = make_float2(x0, x1);
+            }
+          }
+        } else {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int m = r_lo + 8 * h;
+            if (m >= p.M) continue;
+            int seq = 0, pos = m;
+            if (p.in_group < p.M) { seq = m / p.in_group; pos = m - seq * p.in_group; }
+            const int64_t orow = (int64_t)seq * p.out_group + p.out_off + pos;
+            const bool zero = p.zero_lengths != nullptr && pos >= p.zero_lengths[seq];
+            const float* tab = p.addtab ? p.addtab + (int64_t)(p.out_off + pos) * p.N : nullptr;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * j + cp + e;
+                if (n >= p.N) continue;
+                float x = d[4 * j + 2 * h + e] * p.inv_scale + (p.bias ? p.bias[n] : 0.0f);
+                if (tab) x += tab[n];
+                x = zero ? 0.0f : apply_act(x, p.act);
+                if (p.out_hi) {
+                  __half hh, ll;
+                  split_f32(x, hh, ll);
+                  const int64_t o = orow * p.ld_out + p.out_col0 + n;
+                  p.out_hi[o] = hh; p.out_lo[o] = ll;
+                }
+                if (p.out_f32) p.out_f32[orow * p.ldc + n] = x;
+              }
+            }
+          }
+        }
+      },
+      [&](const GemmTile& t, int j, int ntiles, int kb) {
+        if (kb == 0 && j + 1 < ntiles) {
           // the ring is only two or three k-blocks deep: the NEXT tile's activation rows are pulled into L2
           // one whole tile ahead (weights are L2-resident anyway)
-          int m1, n1;
-          decode(j + 1, m1, n1);
-          if (m1 != m0) {
+          const int m1 = tile(j + 1).m0;
+          if (m1 != t.m0) {
             for (int k2 = 0; k2 < p.kblocks; ++k2) {
               if (k2 < p.kb1) { tma_prefetch_2d(&tmA1h, k2 * BK, m1); tma_prefetch_2d(&tmA1l, k2 * BK, m1); }
               else { tma_prefetch_2d(&tmA2h, (k2 - p.kb1) * BK, m1); tma_prefetch_2d(&tmA2l, (k2 - p.kb1) * BK, m1); }
             }
           }
         }
-      };
-      ring_feed(ring, kbg, p.kblocks, Cfg::STAGE_BYTES, [&](int kb, int s, uint32_t full) {
-        const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-        if (kb < p.kb1) {
-          tma_load_2d(sAh, &tmA1h, full, kb * BK, m0);
-          tma_load_2d(sAl, &tmA1l, full, kb * BK, m0);
-        } else {
-          tma_load_2d(sAh, &tmA2h, full, (kb - p.kb1) * BK, m0);
-          tma_load_2d(sAl, &tmA2l, full, (kb - p.kb1) * BK, m0);
-        }
-        tma_load_2d(sWh, &tmWh, full, kb * BK, n0);       // rows >= N are zero-filled (and counted)
-        tma_load_2d(sWl, &tmWl, full, kb * BK, n0);
-      }, prefetch);
-    }
-    return;
-  }
-  // ------------------------------------------------------------------ consumer warpgroups
-  reg_inc<232>();
-  const int cw = (warp >> 2) - 1;                    // which 64 rows of the tile
-  const int cp = 2 * (lane & 3);                     // column offset inside an 8-column group
-  float d[BN / 2];
-  int kbg = 0;
-  for (int it = 0; it < nlocal; ++it) {
-    int m0, n0;
-    decode(it, m0, n0);
-    tl_event(p.tl, tl_n, 2, it);                                     // MMA: tile `it` begins
-    ring_mma<BN>(d, ring, kbg, p.kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
-      ah = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128); al = ah + Cfg::A_BYTES;
-      wh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES; wl = wh + Cfg::W_BYTES;
-    });
-    tl_event(p.tl, tl_n, 4, it);                                     // epilogue: accumulator of tile `it` ready
-
-    const int r_lo = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
-    if constexpr (EPI == EPI_LN) {
-      ln_epilogue(d, p.inv_scale, p.bias, p.res_hi, p.res_lo, p.ld_res, p.gamma, p.beta, p.out_hi, p.out_lo, p.ld_out,
-                  r_lo, p.M, cp);
-    } else if constexpr (EPI == EPI_FAST) {
-      const bool ok0 = r_lo < p.M, ok1 = r_lo + 8 < p.M;
-      const int64_t o0 = (int64_t)r_lo * p.ld_out + p.out_col0 + n0 + cp, o1 = o0 + (int64_t)8 * p.ld_out;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        float x[4];
-        fast_group<ACT>(d, j, p.inv_scale, __ldg(reinterpret_cast<const float2*>(p.bias + n0 + 8 * j + cp)), x);
-        if (ok0) store_split2(p.out_hi, p.out_lo, o0 + 8 * j, x[0], x[1]);
-        if (ok1) store_split2(p.out_hi, p.out_lo, o1 + 8 * j, x[2], x[3]);
-      }
-    } else if constexpr (EPI == EPI_RES) {
-      // each element of R is read and then overwritten by the same thread: in place is safe (plain loads, no __ldg)
-      const float sc = p.inv_scale;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + cp;
-        if (n >= p.N) continue;                        // N even: a column pair is in or out together
-        const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (r_lo + 8 * h >= p.M) continue;
-          const int64_t o = (int64_t)(r_lo + 8 * h) * p.ldc + n;
-          const float2 r = *reinterpret_cast<const float2*>(p.res_f32 + o);
-          *reinterpret_cast<float2*>(p.out_f32 + o) =
-              make_float2(fmaf(d[4 * j + 2 * h], sc, b.x) + r.x, fmaf(d[4 * j + 2 * h + 1], sc, b.y) + r.y);
-        }
-      }
-    } else if constexpr (EPI == EPI_F32) {
-      const float sc = p.inv_scale;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + cp;
-        if (n >= p.N) continue;                        // N even: a column pair is in or out together
-        const float2 b = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + n)) : make_float2(0.0f, 0.0f);
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          if (r_lo + 8 * h >= p.M) continue;
-          const float x0 = apply_act(fmaf(d[4 * j + 2 * h], sc, b.x), ACT), x1 = apply_act(fmaf(d[4 * j + 2 * h + 1], sc, b.y), ACT);
-          *reinterpret_cast<float2*>(p.out_f32 + (int64_t)(r_lo + 8 * h) * p.ldc + n) = make_float2(x0, x1);
-        }
-      }
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = r_lo + 8 * h;
-        if (m >= p.M) continue;
-        int seq = 0, pos = m;
-        if (p.in_group < p.M) { seq = m / p.in_group; pos = m - seq * p.in_group; }
-        const int64_t orow = (int64_t)seq * p.out_group + p.out_off + pos;
-        const bool zero = p.zero_lengths != nullptr && pos >= p.zero_lengths[seq];
-        const float* tab = p.addtab ? p.addtab + (int64_t)(p.out_off + pos) * p.N : nullptr;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int n = n0 + 8 * j + cp + e;
-            if (n >= p.N) continue;
-            float x = d[4 * j + 2 * h + e] * p.inv_scale + (p.bias ? p.bias[n] : 0.0f);
-            if (tab) x += tab[n];
-            x = zero ? 0.0f : apply_act(x, p.act);
-            if (p.out_hi) {
-              __half hh, ll;
-              split_f32(x, hh, ll);
-              const int64_t o = orow * p.ld_out + p.out_col0 + n;
-              p.out_hi[o] = hh; p.out_lo[o] = ll;
-            }
-            if (p.out_f32) p.out_f32[orow * p.ldc + n] = x;
-          }
-        }
-      }
-    }
-    tl_event(p.tl, tl_n, 5, it);                                     // epilogue: tile `it` stored
-  }
-  tl_event(p.tl, tl_n, 42);                       // kernel exit
+      });
 }
 
 // ------------------------------------------------------------------------------ fused FFN
@@ -1068,7 +1011,7 @@ bool tc_gemm(TcCtx* c, const GemmArgs& g, const LnArgs* ln, cudaStream_t st) {
   const int ntiles = p.m_tiles * p.n_tiles;
   dim3 grid(ntiles < c->sm_count ? ntiles : c->sm_count);
 #define MLDB_LAUNCH(BN_, ...)                                                                                      \
-  launch_pdl(k_gemm_tc<BN_, __VA_ARGS__>, grid, dim3(NUM_THREADS), TileCfg<BN_>::SMEM_BYTES, st, mA1h, mA1l, mA2h, \
+  launch_pdl(k_gemm_tc<BN_, __VA_ARGS__>, grid, dim3(WS_THREADS), TileCfg<BN_>::SMEM_BYTES, st, mA1h, mA1l, mA2h, \
              mA2l, mWh, mWl, p)
 #define MLDB_LAUNCH_SHAPE(...)                                                       \
   do {                                                                               \

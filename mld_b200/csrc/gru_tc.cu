@@ -17,9 +17,9 @@
 // thread holds columns 8 j + cp, 8 j + cp + 1 of every group j, so the r, z and n pre-activations of its units land
 // in its own registers and the epilogue needs no shuffle or shared memory.
 //
-// CTA = three warpgroups as in k_gemm_tc (DESIGN §2, the ring protocol): warp 0 streams the A (state) and W_hh
-// k-blocks through a ring of 128B-swizzled stages with TMA, warpgroups 1 and 2 each own 64 rows of the 128-row tile.  Grid =
-// (H / 32 unit tiles, row tiles, 2 directions); no CTA waits on another, steps are ordered by the stream.
+// CTA = k_gemm_tc's (ws_cta, DESIGN §2): warp 0 streams the A (state) and W_hh k-blocks through a ring of
+// 128B-swizzled stages with TMA, warpgroups 1 and 2 each own 64 rows of the 128-row tile.  Grid = (H / 32 unit
+// tiles, row tiles, 2 directions), one tile per CTA; no CTA waits on another, steps are ordered by the stream.
 #include <algorithm>
 
 #include "ops.cuh"
@@ -28,8 +28,7 @@
 namespace {
 using namespace tc;
 
-constexpr int BM = 128, BK = 64, BN = 96, UNITS = 32;        // a tile: 128 rows x 32 hidden units (96 gate columns)
-constexpr int NUM_THREADS = 384, CONSUMER_WARPS = 8;
+constexpr int BN = 96, UNITS = 32;                           // a tile: 128 rows x 32 hidden units (96 gate columns)
 using Cfg = StageLayout<BN, 4>;                              // 56 KB stages (tc_common.cuh)
 
 // accurate expf / tanhf (not the fast intrinsics): the recurrence compounds their error over up to 49 steps
@@ -68,105 +67,76 @@ __device__ __forceinline__ void gru_update(const GruStepArgs& a, int dir, int m,
   a.h_out.lo()[o] = lo;
 }
 
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+// One tile per CTA: unit tile nt, rows m0.., direction dir; arow / wrow: its first row of A (the state of both
+// directions) and of W_hh.
+struct GruTile { int nt, m0, dir, arow, wrow; };
+__global__ void __launch_bounds__(WS_THREADS, 1)
 k_gru_step_tc(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUtensorMap tmAl,
               const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const GruStepArgs a) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  const Ring<Cfg::STAGES> ring{bar_full, bar_full + Cfg::STAGES};
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int nt = (int)blockIdx.x, m0 = (int)blockIdx.y * BM, dir = (int)blockIdx.z;
-  const int kblocks = a.H / BK;
-
-  if (threadIdx.x == 0) {
-    ring.init(CONSUMER_WARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tmAh); tma_prefetch_desc(&tmAl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
-  }
-  pdl_trigger();
-  __syncthreads();
-  pdl_wait();                  // the previous step's state (and gi) are complete
-
-  if (warp < 4) {
-    reg_dec<40>();
-    if (warp != 0) return;
-    const int arow = dir * a.rows_pad + m0, wrow = dir * 3 * a.H + nt * BN;
-    // the ring position is the k-block: ring_feed's separate counter would change the generated code
-    for (int kb = 0; kb < kblocks; ++kb) {
-      ring.wait_empty(kb);
-      if (elect_one()) {
-        const uint32_t full = ring.full_bar(kb);
-        mbar_expect_tx(full, Cfg::STAGE_BYTES);
-        const uint32_t sAh = smem_u32(smem + (kb % Cfg::STAGES) * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
-        tma_load_2d(sAh, &tmAh, full, kb * BK, arow);
-        tma_load_2d(sAl, &tmAl, full, kb * BK, arow);
-        tma_load_2d(sWh, &tmWh, full, kb * BK, wrow);
-        tma_load_2d(sWl, &tmWl, full, kb * BK, wrow);
-      }
-      __syncwarp();
-    }
-    return;
-  }
-  reg_inc<232>();
-  const int cw = (warp >> 2) - 1;
-  const int cp = 2 * (lane & 3);
-  float d[BN / 2];
-  int q = 0;                   // one tile per CTA: the ring starts at position 0 and is not reused
-  ring_mma<BN, false>(d, ring, q, kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
-    const uint32_t base = smem_u32(smem + s * Cfg::STAGE_BYTES);
-    ah = base + cw * (64 * 128); al = base + Cfg::A_BYTES + cw * (64 * 128);
-    wh = base + 2 * Cfg::A_BYTES; wl = base + 2 * Cfg::A_BYTES + Cfg::W_BYTES;
-  });
-
-  // gate epilogue.  Every load of a row (state, gi, biases) is issued before any store, so the loads of the 8
-  // (unit, row) pairs overlap instead of each waiting behind the previous pair's stores.
-  const int r_lo = m0 + cw * 64 + (warp & 3) * 16 + (lane >> 2);
-  const int H = a.H, u0 = nt * UNITS + cp;
-  const float sc = a.w_inv_scale;
-  float bh[4][2][3];
+  // one tile per CTA: nothing more goes through the ring, so its last position is not released
+  ws_cta<Cfg, false>(
+      tmAh, tmAl, tmWh, tmWl, nullptr, a.H / BK, [] { return 1; },
+      [&](int) {
+        GruTile t;
+        t.nt = (int)blockIdx.x; t.m0 = (int)blockIdx.y * BM; t.dir = (int)blockIdx.z;
+        t.arow = t.dir * a.rows_pad + t.m0; t.wrow = t.dir * 3 * a.H + t.nt * BN;
+        return t;
+      },
+      [&](const GruTile& t, int kb, const auto& s, uint32_t full) {
+        tma_load_2d(s.ah, &tmAh, full, kb * BK, t.arow);
+        tma_load_2d(s.al, &tmAl, full, kb * BK, t.arow);
+        tma_load_2d(s.wh, &tmWh, full, kb * BK, t.wrow);
+        tma_load_2d(s.wl, &tmWl, full, kb * BK, t.wrow);
+      },
+      [&](const GruTile& t, const float (&d)[BN / 2], const TileThread& th) {
+        // gate epilogue.  Every load of a row (state, gi, biases) is issued before any store, so the loads of the 8
+        // (unit, row) pairs overlap instead of each waiting behind the previous pair's stores.
+        const int dir = t.dir, r_lo = t.m0 + th.row();
+        const int H = a.H, u0 = t.nt * UNITS + th.cp;
+        const float sc = a.w_inv_scale;
+        float bh[4][2][3];
 #pragma unroll
-  for (int jj = 0; jj < 4; ++jj)
+        for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-    for (int e = 0; e < 2; ++e)
+          for (int e = 0; e < 2; ++e)
 #pragma unroll
-      for (int g = 0; g < 3; ++g) bh[jj][e][g] = __ldg(a.b_hh + dir * 3 * H + g * H + u0 + 8 * jj + e);
+            for (int g = 0; g < 3; ++g) bh[jj][e][g] = __ldg(a.b_hh + dir * 3 * H + g * H + u0 + 8 * jj + e);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int m = r_lo + 8 * h;
-    if (m >= a.rows) continue;
-    int len = __ldg(a.lengths + m);
-    len = len < 0 ? 0 : (len > a.L ? a.L : len);
-    const bool live = a.step < len;
-    const int64_t so = ((int64_t)dir * a.rows_pad + m) * H + u0;
-    const float* gi = a.gi + ((int64_t)m * a.L + (dir ? len - 1 - a.step : a.step)) * (6 * H) + dir * 3 * H + u0;
-    float hp[4][2], gv[4][2][3];
+        for (int h = 0; h < 2; ++h) {
+          const int m = r_lo + 8 * h;
+          if (m >= a.rows) continue;
+          int len = __ldg(a.lengths + m);
+          len = len < 0 ? 0 : (len > a.L ? a.L : len);
+          const bool live = a.step < len;
+          const int64_t so = ((int64_t)dir * a.rows_pad + m) * H + u0;
+          const float* gi = a.gi + ((int64_t)m * a.L + (dir ? len - 1 - a.step : a.step)) * (6 * H) + dir * 3 * H + u0;
+          float hp[4][2], gv[4][2][3];
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj)
+          for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        hp[jj][e] = __ldg(a.hf_in + so + 8 * jj + e);
+            for (int e = 0; e < 2; ++e) {
+              hp[jj][e] = __ldg(a.hf_in + so + 8 * jj + e);
 #pragma unroll
-        for (int g = 0; g < 3; ++g) gv[jj][e][g] = live ? __ldg(gi + g * H + 8 * jj + e) : 0.0f;
-      }
+              for (int g = 0; g < 3; ++g) gv[jj][e][g] = live ? __ldg(gi + g * H + 8 * jj + e) : 0.0f;
+            }
 #pragma unroll
-    for (int jj = 0; jj < 4; ++jj)
+          for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-      for (int e = 0; e < 2; ++e) {
-        const int c = 2 * h + e;
-        const float hn = live ? gru_cell(gv[jj][e][0], gv[jj][e][1], gv[jj][e][2], d[4 * (3 * jj) + c] * sc + bh[jj][e][0],
-                                         d[4 * (3 * jj + 1) + c] * sc + bh[jj][e][1], d[4 * (3 * jj + 2) + c] * sc + bh[jj][e][2],
-                                         hp[jj][e])
-                              : hp[jj][e];
-        const int64_t o = so + 8 * jj + e;
-        a.hf_out[o] = hn;
-        __half hi, lo;
-        split_f32(hn, hi, lo);
-        a.h_out.hi[o] = hi;
-        a.h_out.lo()[o] = lo;
-      }
-  }
+            for (int e = 0; e < 2; ++e) {
+              const int c = 2 * h + e;
+              const float hn = live ? gru_cell(gv[jj][e][0], gv[jj][e][1], gv[jj][e][2], d[4 * (3 * jj) + c] * sc + bh[jj][e][0],
+                                               d[4 * (3 * jj + 1) + c] * sc + bh[jj][e][1], d[4 * (3 * jj + 2) + c] * sc + bh[jj][e][2],
+                                               hp[jj][e])
+                                    : hp[jj][e];
+              const int64_t o = so + 8 * jj + e;
+              a.hf_out[o] = hn;
+              __half hi, lo;
+              split_f32(hn, hi, lo);
+              a.h_out.hi[o] = hi;
+              a.h_out.lo()[o] = lo;
+            }
+        }
+      });
 }
 
 // CUDA-core gate step (gemm=simt): gh [2 * rows_pad, 3H] fp32 in the packed column order, from k_gemm_simt
@@ -388,7 +358,7 @@ bool gru_step_tc(const GruStepArgs& a, cudaStream_t st) {
                   make_map(&mWh, a.w_hh, 6 * a.H, a.H, BN) && make_map(&mWl, a.w_hh + a.w_plane_stride, 6 * a.H, a.H, BN);
   if (!ok) return false;
   const dim3 grid((unsigned)(a.H / UNITS), (unsigned)((a.rows + BM - 1) / BM), 2);
-  launch_pdl(k_gru_step_tc, grid, dim3(NUM_THREADS), Cfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, a);
+  launch_pdl(k_gru_step_tc, grid, dim3(WS_THREADS), Cfg::SMEM_BYTES, st, mAh, mAl, mWh, mWl, a);
   return true;
 }
 

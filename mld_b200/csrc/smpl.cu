@@ -151,13 +151,13 @@ __global__ void __launch_bounds__(128) k_smpl_fk(const FkParams p) {
 }
 
 // ---------------------------------------------------------------------------------------------------- LBS
-constexpr int BM = 64, BN = 96, VT = 32, BK = 64, KB = kPoseKpad / BK, STAGES = 2;
+constexpr int LBS_BM = 64, BN = 96, VT = 32, BK = 64, KB = kPoseKpad / BK, STAGES = 2;
 constexpr int LBS_THREADS = 160;                      // one consumer warpgroup + one TMA producer warp
 constexpr int OUT_LD = 68;                            // staging row (frames) stride: conflict-free epilogue writes
-constexpr int A_PLANE = BM * BK * 2, A_BYTES = KB * 2 * A_PLANE;          // 8 KB, 64 KB
+constexpr int A_PLANE = LBS_BM * BK * 2, A_BYTES = KB * 2 * A_PLANE;      // 8 KB, 64 KB
 constexpr int W_PLANE = BN * BK * 2, W_STAGE = 2 * W_PLANE;                // 12 KB, 24 KB
 constexpr int OFF_W = A_BYTES, OFF_X = OFF_W + STAGES * W_STAGE;
-constexpr int OFF_O = OFF_X + BM * kXf * 4, OFF_LW = OFF_O + BN * OUT_LD * 4;
+constexpr int OFF_O = OFF_X + LBS_BM * kXf * 4, OFF_LW = OFF_O + BN * OUT_LD * 4;
 constexpr int OFF_BAR = OFF_LW + kJ * VT * 4;
 constexpr int LBS_SMEM = OFF_BAR + 64 + 1024;
 static_assert(LBS_SMEM <= 232448, "shared memory budget");
@@ -190,7 +190,7 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
   const int nsplit = (p.vtiles + p.vtiles_per_cta - 1) / p.vtiles_per_cta;
   const int mt = blockIdx.x / nsplit, n0 = (blockIdx.x % nsplit) * p.vtiles_per_cta;
   const int n1 = min(p.vtiles, n0 + p.vtiles_per_cta);
-  const int m0 = mt * BM;
+  const int m0 = mt * LBS_BM;
 
   if (threadIdx.x == 0) {
     mbar_init(smem_u32(bar_a), 1);
@@ -231,7 +231,7 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
   // ------------------------------------------------------------------ consumer warpgroup
   const int tid = threadIdx.x;
   // this CTA's frames' transforms (rows past the last frame: zero, never stored)
-  for (int i = tid; i < BM * (kXf / 4); i += 128) {
+  for (int i = tid; i < LBS_BM * (kXf / 4); i += 128) {
     const int r = i / (kXf / 4), q = i - r * (kXf / 4);
     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
     if (m0 + r < p.frames) v = __ldg(reinterpret_cast<const float4*>(p.xf + (int64_t)(m0 + r) * kXf) + q);
@@ -318,8 +318,8 @@ k_smpl_lbs(const __grid_constant__ CUtensorMap tmAh, const __grid_constant__ CUt
     }
     named_bar_sync(1, 128);                           // the tile is staged
     // store along t: consecutive threads take consecutive frames of one (vertex, coordinate)
-    for (int i = tid; i < BN * BM; i += 128) {
-      const int col = i / BM, r = i - col * BM;
+    for (int i = tid; i < BN * LBS_BM; i += 128) {
+      const int col = i / LBS_BM, r = i - col * LBS_BM;
       const int row = m0 + r, c = col / VT, v = nt * VT + (col - c * VT);
       if (row >= p.frames || v >= p.V) continue;
       const int b = row / p.T, t = row - b * p.T;
@@ -440,7 +440,7 @@ extern "C" int mldb_smpl_forward(mldb_handle* h, const float* feats, const uint8
     if (!verts) continue;
     const LinW& w = s.posedirs;
     CUtensorMap mAh, mAl, mWh, mWl;
-    if (!make_map(&mAh, A.hi, frames, kPoseKpad, BM) || !make_map(&mAl, A.lo(), frames, kPoseKpad, BM) ||
+    if (!make_map(&mAh, A.hi, frames, kPoseKpad, LBS_BM) || !make_map(&mAl, A.lo(), frames, kPoseKpad, LBS_BM) ||
         !make_map(&mWh, w.w, w.N, w.K, BN) || !make_map(&mWl, w.w + w.plane_stride, w.N, w.K, BN)) {
       h->op_failed = true;
       break;
@@ -450,7 +450,7 @@ extern "C" int mldb_smpl_forward(mldb_handle* h, const float* feats, const uint8
     lp.inv_scale = w.inv_scale; lp.xf = (const float*)s.xf.p; lp.vt = s.v_template; lp.lbsw = s.lbsw;
     lp.jmask = s.jmask; lp.out = o;
     // split the vertex tiles over CTAs until the grid covers the SMs (each CTA loads its 64 frames once)
-    const int mtiles = (frames + BM - 1) / BM;
+    const int mtiles = (frames + LBS_BM - 1) / LBS_BM;
     const int nsplit = std::max(1, std::min(lp.vtiles, (h->sm_count + mtiles - 1) / mtiles));
     lp.vtiles_per_cta = (lp.vtiles + nsplit - 1) / nsplit;
     const int grid = mtiles * ((lp.vtiles + lp.vtiles_per_cta - 1) / lp.vtiles_per_cta);

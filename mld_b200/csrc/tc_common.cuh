@@ -1,6 +1,7 @@
-// PTX wrappers shared by the warpgroup-MMA kernels (gemm_tc.cu, attn_tc.cu, gru_tc.cu): mbarriers, TMA (bulk
-// tensor copies), wgmma.mma_async and its shared-memory matrix descriptors, the split16 k-block; on the host, the
-// tensor maps of split16 planes.  sm_90a only.
+// PTX wrappers shared by the warpgroup-MMA kernels (gemm_tc.cu, attn_tc.cu, gru_tc.cu, tconv_tc.cu, smpl.cu):
+// mbarriers, TMA (bulk tensor copies), wgmma.mma_async and its shared-memory matrix descriptors, the split16
+// k-block, the TMA rings and the 128-row warp-specialised CTA; on the host, the tensor maps of split16 planes.
+// sm_90a only.
 #pragma once
 #include <cuda.h>
 #include <stdio.h>
@@ -361,7 +362,7 @@ struct Ring {
 // The producer warp's loop over n k-blocks, from ring position q on (q is advanced past them).  The whole warp
 // walks it (uniform control flow); one elected lane calls before(kb) (k_gemm_tc's L2 prefetch), arms full with
 // `bytes` and issues load(kb, slot, full).
-struct NoOp { __device__ __forceinline__ void operator()(int) const {} };
+struct NoOp { template <class... A> __device__ __forceinline__ void operator()(A&&...) const {} };
 template <int S, class Load, class Before = NoOp>
 __device__ __forceinline__ void ring_feed(const Ring<S>& ring, int& q, int n, uint32_t bytes, Load&& load,
                                           Before&& before = {}) {
@@ -400,17 +401,33 @@ __device__ __forceinline__ void ring_mma(float (&d)[BN / 2], const Ring<S>& ring
   if (RELEASE_LAST && lane == 0) ring.release(q - 1);
 }
 
+// ---------------------------------------------------------------------------------- the 128-row CTA
+// The CTA shape of k_gemm_tc, k_tconv_tc and k_gru_step_tc (ws_cta below) and of k_attn_tc (DESIGN §2): a producer
+// warpgroup that gives its registers away and two consumer warpgroups of 64 rows each.  At 384 threads ptxas
+// compiles the consumers under 168 registers, whatever setmaxnreg raises them to at run time.
+constexpr int BM = 128, BK = 64;                       // tile rows; k-block depth (one 128B swizzle row of fp16)
+constexpr int WS_THREADS = 384;
+constexpr int CONSUMER_WARPS = 8;
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+
 // One ring stage of a 128 x BN split16 tile: [A hi | A lo | W hi | W lo], each plane a 64-deep k-block (one 128B
 // swizzle row per tile row), A 128 rows and W BN rows; two consumer warpgroups take 64 A rows each.  STAGES stages
 // followed by the ring's barriers, plus the alignment slack of smem_pad1024.
-template <int BN, int STAGES_>
+template <int BN_, int STAGES_>
 struct StageLayout {
-  static constexpr int STAGES = STAGES_;
-  static constexpr int A_BYTES = 128 * 64 * 2;        // one plane of the A tile (16 KB)
-  static constexpr int W_BYTES = BN * 64 * 2;         // one plane of the W tile
+  static constexpr int BN = BN_, STAGES = STAGES_;
+  static constexpr int A_BYTES = BM * BK * 2;         // one plane of the A tile (16 KB)
+  static constexpr int W_BYTES = BN * BK * 2;         // one plane of the W tile
   static constexpr int STAGE_BYTES = 2 * A_BYTES + 2 * W_BYTES;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  // the shared-memory addresses of slot s's planes, the A planes from byte a_off of the tile on; smem: the first stage
+  struct Planes { uint32_t ah, al, wh, wl; };
+  __device__ __forceinline__ static Planes planes(const uint8_t* smem, int s, uint32_t a_off = 0) {
+    const uint32_t ah = smem_u32(smem + s * STAGE_BYTES) + a_off, al = ah + A_BYTES;
+    const uint32_t wh = smem_u32(smem + s * STAGE_BYTES) + 2 * A_BYTES, wl = wh + W_BYTES;
+    return {ah, al, wh, wl};
+  }
 };
 
 // sum over the 4 lanes of a quad (the lanes that hold one accumulator row)
@@ -448,6 +465,87 @@ __device__ __forceinline__ void tl_event(long long* tl, int& n, int tag, int aux
   }
 }
 long long* mldb_timeline_buffer();   // debug.cu: the device buffer while a timeline is being recorded, else nullptr
+
+// A consumer thread of ws_cta: its warp and lane, its warpgroup's 64 rows of the tile (cw) and its column offset
+// inside an 8-column group (cp).  Its accumulator fragment holds tile rows row() and row() + 8.
+struct TileThread {
+  int warp, lane, cw, cp;
+  __device__ __forceinline__ int row() const { return cw * 64 + (warp & 3) * 16 + (lane >> 2); }
+};
+
+// The tiles this CTA runs of a persistent grid over ntiles tiles: CTA c takes tiles c, c + #CTAs, ...
+__device__ __forceinline__ int persistent_count(int ntiles) {
+  return (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+}
+
+// The whole body of a kernel launched with WS_THREADS threads and L::SMEM_BYTES of dynamic shared memory: L::STAGES
+// stages of the StageLayout L, then the ring's barriers.  Thread 0 sets up the ring and prefetches the tensor maps
+// m0..m3.  After the PDL wait, warpgroup 0 drops to PRODUCER_REGS registers and its warp 0 feeds the ring
+// (ring_feed); warpgroups 1 and 2 raise themselves to CONSUMER_REGS and each multiply 64 rows of every tile
+// (ring_mma).  Every tile is kblocks k-blocks deep.  The kernel supplies
+//   count()                   how many tiles this CTA runs (called once, in the prologue);
+//   tile(j)                   the j-th of them, in whatever form load, epilogue and before take it;
+//   load(t, kb, planes, full) tile t's loads of k-block kb into the stage at `planes` (one elected lane);
+//   epilogue(t, d, th)        the consumers' epilogue on their [64 x L::BN] accumulator fragment d;
+//   before(t, j, ntiles, kb)  run by the producer's elected lane before it arms k-block kb of t, the j-th of the
+//                             CTA's ntiles tiles.
+// RELEASE_LAST as in ring_mma.  tl: the debug timeline (nullptr: none), with tags 40 at entry, 41 after the PDL
+// wait, 1 as the producer starts a tile, 2 / 4 / 5 as the consumers start its MMAs, have its accumulator and have
+// run its epilogue, and 42 at the consumers' exit.  tl and kblocks are taken by reference, so that a kernel
+// parameter is read where it is used: a copy made at the call is computed ahead of the prologue, and nvcc then
+// schedules the whole kernel differently.
+template <class L, bool RELEASE_LAST = true, class Count, class Tile, class Load, class Epilogue, class Before = NoOp>
+__device__ __forceinline__ void ws_cta(const CUtensorMap& m0, const CUtensorMap& m1, const CUtensorMap& m2,
+                                       const CUtensorMap& m3, long long* const& tl, const int& kblocks, Count&& count, Tile&& tile,
+                                       Load&& load, Epilogue&& epilogue, Before&& before = {}) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
+  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + L::STAGES * L::STAGE_BYTES);
+  const Ring<L::STAGES> ring{bar_full, bar_full + L::STAGES};
+  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
+  int tl_n = 0;                                     // debug-timeline event counter of this warp
+  tl_event(tl, tl_n, 40);
+  const int ntiles = count();
+  if (threadIdx.x == 0) {
+    ring.init(CONSUMER_WARPS);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    tma_prefetch_desc(&m0); tma_prefetch_desc(&m1); tma_prefetch_desc(&m2); tma_prefetch_desc(&m3);
+  }
+  pdl_trigger();               // let the next kernel's prologue overlap our tail
+  __syncthreads();
+  pdl_wait();                  // everything below touches the previous kernel's outputs
+  tl_event(tl, tl_n, 41);
+
+  if (warp < 4) {
+    reg_dec<PRODUCER_REGS>();
+    if (warp != 0) return;
+    int q = 0;                 // ring position, across tiles
+    for (int j = 0; j < ntiles; ++j) {
+      const auto t = tile(j);
+      tl_event(tl, tl_n, 1, j);
+      ring_feed(ring, q, kblocks, L::STAGE_BYTES,
+                [&](int kb, int s, uint32_t full) { load(t, kb, L::planes(smem, s), full); },
+                [&](int kb) { before(t, j, ntiles, kb); });
+    }
+    return;
+  }
+  reg_inc<CONSUMER_REGS>();
+  const TileThread th{warp, lane, (warp >> 2) - 1, 2 * (lane & 3)};
+  float d[L::BN / 2];
+  int q = 0;
+  for (int j = 0; j < ntiles; ++j) {
+    const auto t = tile(j);
+    tl_event(tl, tl_n, 2, j);
+    ring_mma<L::BN, RELEASE_LAST>(d, ring, q, kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
+      const auto pl = L::planes(smem, s, th.cw * (64 * 128));             // the warpgroup's 64 A rows
+      ah = pl.ah; al = pl.al; wh = pl.wh; wl = pl.wl;
+    });
+    tl_event(tl, tl_n, 4, j);
+    epilogue(t, d, th);
+    tl_event(tl, tl_n, 5, j);
+  }
+  tl_event(tl, tl_n, 42);
+}
 
 // ---------------------------------------------------------------------------------- host: tensor maps
 // both planes of a split16 buffer 16-byte aligned (TMA base addresses, 16-byte accesses)

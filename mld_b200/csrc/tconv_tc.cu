@@ -4,8 +4,8 @@
 //   D[128 x C] = sum over k-blocks (tap, c0) of  X_tap[128 x 64] . W[:, tap C + c0 ..]^T       (split16, kblock_ss)
 //
 // The activations are split16 rows (n * T + t) * 24 + v, i.e. planes of shape [nseq][T][24][C].  A tile is 8 joints
-// x 16 output frames of one sequence (128 rows, 64 per consumer warpgroup), so k_gemm_tc's two-consumer layout, its
-// ring (DESIGN §2, the ring protocol) and its register budget carry over unchanged.  Its A operand for tap `tap` is one TMA box of a 4-D tensor map over those
+// x 16 output frames of one sequence (128 rows, 64 per consumer warpgroup), so it runs on k_gemm_tc's CTA (ws_cta,
+// DESIGN §2) within its register budget.  Its A operand for tap `tap` is one TMA box of a 4-D tensor map over those
 // planes: channels c0 .. c0 + 63, joints 8 vt .. 8 vt + 7, frames s t0 + tap - 4 + s i (i < 16), sequence n.  The
 // box is one sequence deep, so no tile reads another sequence's frames, and the frames outside [0, T) are TMA's
 // out-of-bounds zero fill: the convolution's padding.  Stride 2 is the frame dimension's traversal stride in the map
@@ -22,9 +22,6 @@
 namespace {
 using namespace tc;
 
-constexpr int BM = 128, BK = 64;
-constexpr int NUM_THREADS = 384;                     // producer warpgroup + two consumer warpgroups (k_gemm_tc's layout)
-constexpr int CONSUMER_WARPS = 8;
 constexpr int JOINTS = 24, TILE_V = 8, TILE_T = 16;  // a tile: 8 joints x 16 output frames
 constexpr int TAPS = 9, PAD = 4;
 
@@ -45,101 +42,60 @@ struct TconvParams {
 
 // Persistent: CTA c walks tiles c, c + #CTAs, ...; tile -> (sequence, 16-frame block, 8-joint group), the joint group
 // fastest so that the three tiles reading the same frames run side by side.
+struct TconvTile { int n, t0, vt, f0; };
 template <int BN>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(WS_THREADS, 1)
 k_tconv_tc(const __grid_constant__ CUtensorMap tmXh, const __grid_constant__ CUtensorMap tmXl,
            const __grid_constant__ CUtensorMap tmRh, const __grid_constant__ CUtensorMap tmRl,
            const __grid_constant__ CUtensorMap tmWh, const __grid_constant__ CUtensorMap tmWl, const TconvParams p) {
-  using Cfg = TconvCfg<BN>;
-  constexpr int STAGES = Cfg::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + smem_pad1024(smem_raw);
-  uint64_t* bar_full = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
-  const Ring<STAGES> ring{bar_full, bar_full + STAGES};
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int ntiles = p.nseq * p.t_blocks * 3;
-  const int nlocal = (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  auto decode = [&](int j, int& n, int& t0, int& vt) {
-    const int t = (int)blockIdx.x + j * (int)gridDim.x;
-    vt = t % 3;
-    const int r = t / 3;
-    t0 = (r % p.t_blocks) * TILE_T;
-    n = r / p.t_blocks;
-  };
-
-  if (threadIdx.x == 0) {
-    ring.init(CONSUMER_WARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    tma_prefetch_desc(&tmXh); tma_prefetch_desc(&tmXl); tma_prefetch_desc(&tmWh); tma_prefetch_desc(&tmWl);
-  }
-  pdl_trigger();
-  __syncthreads();
-  pdl_wait();                  // everything below touches activations of the previous kernel
-
-  if (warp < 4) {
-    reg_dec<40>();
-    if (warp != 0) return;
-    // ---------------------------------------------------------------- TMA producer (one elected lane issues)
-    int kbg = 0;
-    for (int j = 0; j < nlocal; ++j) {
-      int n, t0, vt;
-      decode(j, n, t0, vt);
-      const int f0 = p.stride * t0;                  // input frame of the tile's first output frame at tap 4
-      ring_feed(ring, kbg, p.kblocks, Cfg::STAGE_BYTES, [&](int kb, int s, uint32_t full) {
-        const uint32_t sAh = smem_u32(smem + s * Cfg::STAGE_BYTES), sAl = sAh + Cfg::A_BYTES;
-        const uint32_t sWh = sAl + Cfg::A_BYTES, sWl = sWh + Cfg::W_BYTES;
+  ws_cta<TconvCfg<BN>>(
+      tmXh, tmXl, tmWh, tmWl, nullptr, p.kblocks, [&] { return persistent_count(p.nseq * p.t_blocks * 3); },
+      [&](int j) {
+        TconvTile tile;
+        const int t = (int)blockIdx.x + j * (int)gridDim.x;
+        tile.vt = t % 3;
+        const int r = t / 3;
+        tile.t0 = (r % p.t_blocks) * TILE_T;
+        tile.n = r / p.t_blocks;
+        tile.f0 = p.stride * tile.t0;                 // input frame of the tile's first output frame at tap 4
+        return tile;
+      },
+      [&](const TconvTile& t, int kb, const auto& s, uint32_t full) {
         if (kb < p.ktap) {
           const int tap = kb / p.kc, c0 = (kb - tap * p.kc) * BK;
-          tma_load_4d(sAh, &tmXh, full, c0, vt * TILE_V, f0 + tap - PAD, n);
-          tma_load_4d(sAl, &tmXl, full, c0, vt * TILE_V, f0 + tap - PAD, n);
+          tma_load_4d(s.ah, &tmXh, full, c0, t.vt * TILE_V, t.f0 + tap - PAD, t.n);
+          tma_load_4d(s.al, &tmXl, full, c0, t.vt * TILE_V, t.f0 + tap - PAD, t.n);
         } else {
           const int c0 = (kb - p.ktap) * BK;
-          tma_load_4d(sAh, &tmRh, full, c0, vt * TILE_V, f0, n);
-          tma_load_4d(sAl, &tmRl, full, c0, vt * TILE_V, f0, n);
+          tma_load_4d(s.ah, &tmRh, full, c0, t.vt * TILE_V, t.f0, t.n);
+          tma_load_4d(s.al, &tmRl, full, c0, t.vt * TILE_V, t.f0, t.n);
         }
-        tma_load_2d(sWh, &tmWh, full, kb * BK, 0);
-        tma_load_2d(sWl, &tmWl, full, kb * BK, 0);
+        tma_load_2d(s.wh, &tmWh, full, kb * BK, 0);
+        tma_load_2d(s.wl, &tmWl, full, kb * BK, 0);
+      },
+      [&](const TconvTile& tile, const float (&d)[BN / 2], const TileThread& th) {
+        // this thread's rows: tile rows r and r + 8 = frames t and t + 1 of joint v
+        const int t = tile.t0 + th.cw * 8 + (th.warp & 3) * 2, v = tile.vt * TILE_V + (th.lane >> 2);
+        const float sc = p.inv_scale;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (t + h >= p.T_out) continue;
+          const int64_t o = (((int64_t)tile.n * p.T_out + t + h) * JOINTS + v) * BN + th.cp;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + 8 * j + th.cp));
+            float x0 = fmaf(d[4 * j + 2 * h], sc, b.x), x1 = fmaf(d[4 * j + 2 * h + 1], sc, b.y);
+            if (p.res_hi) {
+              const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(p.res_hi + o + 8 * j));
+              const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o + 8 * j));
+              x0 = (x0 + rh.x) + rl.x; x1 = (x1 + rh.y) + rl.y;
+            }
+            x0 = x0 < 0.0f ? 0.0f : x0; x1 = x1 < 0.0f ? 0.0f : x1;      // torch.relu: a NaN stays NaN
+            if (p.out_hi) store_split2(p.out_hi, p.out_lo, o + 8 * j, x0, x1);
+            else *reinterpret_cast<float2*>(p.out_f32 + o + 8 * j) = make_float2(x0, x1);
+          }
+        }
       });
-    }
-    return;
-  }
-  // ------------------------------------------------------------------ consumer warpgroups
-  reg_inc<232>();
-  const int cw = (warp >> 2) - 1;                    // which 64 rows (8 frames) of the tile
-  const int cp = 2 * (lane & 3);                     // column offset inside an 8-column group
-  float d[BN / 2];
-  int kbg = 0;
-  for (int it = 0; it < nlocal; ++it) {
-    int n, t0, vt;
-    decode(it, n, t0, vt);
-    ring_mma<BN>(d, ring, kbg, p.kblocks, lane, [&](int, int s, uint32_t& ah, uint32_t& al, uint32_t& wh, uint32_t& wl) {
-      ah = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128); al = ah + Cfg::A_BYTES;
-      wh = smem_u32(smem + s * Cfg::STAGE_BYTES) + 2 * Cfg::A_BYTES; wl = wh + Cfg::W_BYTES;
-    });
-
-    // this thread's rows: tile rows r and r + 8 = frames t and t + 1 of joint v
-    const int t = t0 + cw * 8 + (warp & 3) * 2, v = vt * TILE_V + (lane >> 2);
-    const float sc = p.inv_scale;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      if (t + h >= p.T_out) continue;
-      const int64_t o = (((int64_t)n * p.T_out + t + h) * JOINTS + v) * BN + cp;
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + 8 * j + cp));
-        float x0 = fmaf(d[4 * j + 2 * h], sc, b.x), x1 = fmaf(d[4 * j + 2 * h + 1], sc, b.y);
-        if (p.res_hi) {
-          const float2 rh = __half22float2(*reinterpret_cast<const __half2*>(p.res_hi + o + 8 * j));
-          const float2 rl = __half22float2(*reinterpret_cast<const __half2*>(p.res_lo + o + 8 * j));
-          x0 = (x0 + rh.x) + rl.x; x1 = (x1 + rh.y) + rl.y;
-        }
-        x0 = x0 < 0.0f ? 0.0f : x0; x1 = x1 < 0.0f ? 0.0f : x1;      // torch.relu: a NaN stays NaN
-        if (p.out_hi) store_split2(p.out_hi, p.out_lo, o + 8 * j, x0, x1);
-        else *reinterpret_cast<float2*>(p.out_f32 + o + 8 * j) = make_float2(x0, x1);
-      }
-    }
-  }
 }
 
 // A split16 plane [nseq * T * 24, C] seen as [nseq][T][24][C]: boxes of 64 channels x 8 joints x 16 frames (every
@@ -198,8 +154,8 @@ bool tconv_tc(const TconvArgs& a, int sm_count, cudaStream_t st) {
   if (a.out.hi) { p.out_hi = a.out.hi; p.out_lo = a.out.lo(); } else p.out_f32 = a.out_f32;
   const int ntiles = a.nseq * p.t_blocks * 3;
   const dim3 grid((unsigned)std::min(ntiles, std::max(sm_count, 1)));
-  if (a.C == 64) launch_pdl(k_tconv_tc<64>, grid, dim3(NUM_THREADS), TconvCfg<64>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
-  else if (a.C == 128) launch_pdl(k_tconv_tc<128>, grid, dim3(NUM_THREADS), TconvCfg<128>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
-  else launch_pdl(k_tconv_tc<256>, grid, dim3(NUM_THREADS), TconvCfg<256>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
+  if (a.C == 64) launch_pdl(k_tconv_tc<64>, grid, dim3(WS_THREADS), TconvCfg<64>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
+  else if (a.C == 128) launch_pdl(k_tconv_tc<128>, grid, dim3(WS_THREADS), TconvCfg<128>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
+  else launch_pdl(k_tconv_tc<256>, grid, dim3(WS_THREADS), TconvCfg<256>::SMEM_BYTES, st, mXh, mXl, mRh, mRl, mWh, mWl, p);
   return true;
 }
